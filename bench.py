@@ -33,12 +33,10 @@ WORKLOADS = {
     "llama2-7b-q4_0-q6k": ("LLAMA2_7B", "Q4_0", "Q6_K"),
     "llama2-7b-q4_k": ("LLAMA2_7B", "Q4_K", "Q6_K"),
     "tinyllamas-15m-q8_0": ("TINYLLAMAS_15M", "Q8_0", "Q8_0"),
-    # BASELINE.json config 5: the dense matmuls of a 4096-token prefill (TMA + tcgen05 path, csrc/prefill_gemm.cu); see run_prefill
+    # BASELINE.json config 5: the dense matmuls of a 4096-token prefill (TMA + wgmma path, csrc/prefill_gemm.cu); see run_prefill
     "mistral-7b-q8_0-prefill": ("MISTRAL_7B", "Q8_0", "Q8_0"),
     "llama2-7b-q8_0-prefill": ("LLAMA2_7B", "Q8_0", "Q8_0"),
 }
-# dram bytes per megakernel launch from the committed ncu --set full capture (profiles/); None until captured
-TRAFFIC = {("llama2-7b-q8_0", 1): 7040893000 + 49879296}     # profiles/r02p_mega_ring_q8_0_ncu_raw.csv (mega_ring_kernel: dram__bytes_read.sum + dram__bytes_write.sum)
 MEGA_NAMES = {1: ("mega_kernel", "mega.cu, weights through registers"), 2: ("mega_ring_kernel", "mega_ring.cu, weights through a TMA-fed shared-memory ring")}
 TYPE_ID = {"Q4_0": 2, "Q4_1": 3, "Q5_0": 6, "Q5_1": 7, "Q8_0": 8, "Q2_K": 10, "Q3_K": 11, "Q4_K": 12, "Q5_K": 13, "Q6_K": 14}
 
@@ -62,11 +60,36 @@ def measured_peaks():
     if os.path.exists(p):
         with open(p) as f:
             return json.load(f), "measured (MEASURED_PEAKS.json)"
-    return {"hbm_gbs": 6650.0, "sm_max_mhz": 1965.0}, "fallback (B200_PROFILING.md)"
+    return {"hbm_gbs": 3350.0, "sm_max_mhz": 1980.0, "bf16_tflops": 989.0}, "H100 SXM data sheet (700 W), not a measured figure"
+
+
+def dump_outputs(out_dir, arrays, budget=64 << 20, seed=SEED):
+    """--dump-outputs: writes each array as out_dir/<name>.npy (float32; float64 for integer ids).  An array larger than its share
+    of the 64 MB budget is replaced by a fixed, seeded sample of its flattened elements (the same indices on every run)."""
+    os.makedirs(out_dir, exist_ok=True)
+    share = budget // max(1, len(arrays))
+    for name, a in arrays.items():
+        a = np.asarray(a)
+        a = a.astype(np.float64) if a.dtype.kind in "iu" else a.astype(np.float32)
+        if a.nbytes > share:
+            idx = np.sort(np.random.default_rng(seed).choice(a.size, share // a.itemsize, replace=False))
+            a = a.reshape(-1)[idx]
+        np.save(os.path.join(out_dir, f"{name}.npy"), a)
+
+
+def gpu_identity(gpu_index: int):
+    """Name, power limit and maximum SM clock of the GPU (read-only nvidia-smi query): an absolute number means little without them."""
+    try:
+        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader,nounits", "-i", str(gpu_index)],
+                             capture_output=True, text=True, timeout=30).stdout.strip().split(", ")
+        name, power, smax = out[0], float(out[1]), float(out[2])
+    except (OSError, subprocess.SubprocessError, IndexError, ValueError):
+        return {"name": None, "power_limit_w": None, "clocks_max_sm_mhz": None}
+    return {"name": name, "power_limit_w": power, "clocks_max_sm_mhz": smax}
 
 
 class ClockSampler:
-    """nvidia-smi clocks/throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks/throttle reasons DURING the timed region (read-only queries)."""
     Q = "index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown," \
         "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
 
@@ -207,7 +230,7 @@ def run_reference(args, rank, world):
     print(json.dumps(line))
 
 
-def quick_decode(workload: str, local_rank: int, K: int, W: int, start_pos: int):
+def quick_decode(workload: str, local_rank: int, K: int, W: int, start_pos: int, dump: dict | None = None):
     """Second measurement of the default run: the same decode loop (device-resident and e2e) for another weight type, so that one
     bench line covers the whole metric (Q8_0 AND Q4_0).  Returns a dict that is embedded in the main JSON line."""
     from crabml_b200 import CudaTensorDevice
@@ -242,13 +265,15 @@ def quick_decode(workload: str, local_rank: int, K: int, W: int, start_pos: int)
             runner.forward([(tok * 31 + 7 * i) % conf.vocab_size], pos, export=False); pos += 1
         val_ms = dev.timer_end()
         launches = dev.launch_count() - l0
+        if dump is not None:          # the last timed step again (same token, same position): its logits
+            dump[f"{workload}_logits"] = runner.forward([(tok * 31 + 7 * (K - 1)) % conf.vocab_size], pos - 1, export=True).copy()
         peaks, _ = measured_peaks()
         gbs = bytes_per_token / (val_ms / K * 1e-3) / 1e9
         out = {"workload": f"{workload}-decode-synthetic", "weights": wt_name, "classifier": ct_name, "value": K / (val_ms * 1e-3), "unit": "tok/s",
                "ms_per_step": val_ms / K, "e2e": {"value": K / (e2e_ms * 1e-3), "unit": "tok/s", "h2d_bytes_per_step": 8, "d2h_bytes_per_step": conf.vocab_size * 4},
                "gpu_launches_device_resident": int(launches), "steps": K, "warmup": W,
                "roofline": {"bound": "hbm", "kernel": MEGA_NAMES.get(dev.mega_variant(), MEGA_NAMES[1])[0] if launches == K else "fused kernels (CUDA graph)", "achieved": gbs, "peak": peaks["hbm_gbs"], "unit": "GB/s",
-                            "frac": gbs / peaks["hbm_gbs"], "algorithmic_bytes_per_launch": bytes_per_token, "frac_of_8TBs_nominal": gbs / 8000.0}}
+                            "frac": gbs / peaks["hbm_gbs"], "algorithmic_bytes_per_launch": bytes_per_token}}
         runner.close()
         return out
     finally:
@@ -355,6 +380,12 @@ def run_b200(args, rank, world, local_rank):
     launches_val = dev.launch_count() - launches1
     clocks = sampler.stop()
     barrier()
+    dump = None
+    if args.dump_outputs:
+        # the last timed step once more (same token at the same position, so the same KV row and the same logits), exported this time;
+        # the e2e region's greedy ids and its last logits are what the host received inside that region
+        last_logits = runner.forward([toks[K - 1]], pos - 1, export=True).copy()
+        dump = {"logits": last_logits, "e2e_logits": lgs[-1], "e2e_ids": np.asarray(ids, np.int64)}
 
     # ---- roofline of the dominant kernel: ffn_gate/ffn_up-shaped matvec over all layers' weights (>> L2) ----------
     # (timed through an eager-mode device handle on the same GPU so that each matmul_vec is its own launch pair)
@@ -389,13 +420,12 @@ def run_b200(args, rank, world, local_rank):
             mk_name, mk_file = MEGA_NAMES.get(dev.mega_variant(), MEGA_NAMES[1])
             roofline = {"bound": "hbm", "kernel": f"{mk_name} ({mk_file}): one persistent launch per decoded token, all matvec/attention/norm phases",
                         "achieved": mega_gbs, "peak": peaks["hbm_gbs"], "peak_source": peak_src, "unit": "GB/s", "frac": mega_gbs / peaks["hbm_gbs"],
-                        "traffic": TRAFFIC.get((args.workload, world)), "traffic_source": "profiles/ (ncu --set full, dram__bytes_read.sum + dram__bytes_write.sum per launch)" if TRAFFIC.get((args.workload, world)) else None,
-                        "algorithmic_bytes_per_launch": bytes_per_token, "us_per_launch": val_ms / K * 1e3, "frac_of_8TBs_nominal": mega_gbs / 8000.0}
+                        "traffic": None, "algorithmic_bytes_per_launch": bytes_per_token, "us_per_launch": val_ms / K * 1e3}
         else:
             roofline = {"bound": "hbm", "kernel": f"matvec_stream_kernel<{wt_name}> {m}x{k} (+ activation quantize: {launches_per_mv:.0f} launches per matmul_vec)",
                         "achieved": mv_gbs, "peak": peaks["hbm_gbs"], "peak_source": peak_src, "unit": "GB/s",
                         "frac": mv_gbs / peaks["hbm_gbs"], "traffic": None, "algorithmic_bytes_per_launch": mv_bytes,
-                        "us_per_launch": mv_ms / n_mv * 1e3, "frac_of_8TBs_nominal": mv_gbs / 8000.0}
+                        "us_per_launch": mv_ms / n_mv * 1e3}
         line = {
             "metric": "decode_tokens_per_s", "value": value, "unit": "tok/s", "n_gpus": world, "steps": K, "warmup": W,
             "ms_per_step": val_ms / K, "higher_is_better": True, "scaling": "strong" if sharded else "weak", "vs_baseline": None, "dtype": "int8",
@@ -407,7 +437,7 @@ def run_b200(args, rank, world, local_rank):
                                      f"exchange = {'one-shot NVLink peer stores fused into the megakernel' if transport == 'p2p' and lazy == 2 else 'one-shot NVLink peer-store kernel' if transport == 'p2p' else 'ncclAllReduce/ncclAllGather'} "
                                      f"(2 allreduce of [dim] f32 per layer + 1 allgather of logits)" if sharded else f"{world} independent replicas"),
                        "weight_bytes_per_token_per_gpu": bytes_per_token,
-                       "l2_policy": f"weights streamed once per token ({bytes_per_token / 1e9:.2f} GB >> 126 MB L2): inputs larger than L2",
+                       "l2_policy": f"weights streamed once per token ({bytes_per_token / 1e9:.2f} GB >> 50 MB L2): inputs larger than L2",
                        "weight_bytes_per_token": bytes_per_token,
                        "hbm_frac_whole_step": bytes_per_token / (val_ms / K * 1e-3) / 1e9 / peaks["hbm_gbs"]},
             "e2e": {"value": e2e, "unit": "tok/s", "h2d_bytes_per_step": 8, "d2h_bytes_per_step": conf.vocab_size * 4 + 8,
@@ -421,6 +451,7 @@ def run_b200(args, rank, world, local_rank):
                                       "achieved": mv_gbs, "unit": "GB/s", "frac": mv_gbs / peaks["hbm_gbs"], "algorithmic_bytes_per_launch": mv_bytes,
                                       "us_per_launch": mv_ms / n_mv * 1e3},
             "clocks": clocks,
+            "gpu": gpu_identity(local_rank),
             "lazy_stats": dev.lazy_stats() if args.lazy else None,
             "host_ms_per_step": {"issue_total": host_issue_ms / K,
                                  **({k: (st1[k] - st0[k]) / 1e3 / K for k in ("host_us_record", "host_us_fuse", "host_us_submit")} if args.lazy else {})},
@@ -436,9 +467,11 @@ def run_b200(args, rank, world, local_rank):
             # run `--workload llama2-7b-q4_0-q6k` for that variant)
             weights = None
             try:
-                line["also"] = {"llama2-7b-q4_0": quick_decode("llama2-7b-q4_0", local_rank, K, W, args.start_pos)}
+                line["also"] = {"llama2-7b-q4_0": quick_decode("llama2-7b-q4_0", local_rank, K, W, args.start_pos, dump)}
             except Exception as e:      # the second block must never cost the main line
                 line["also"] = {"llama2-7b-q4_0": {"error": repr(e)}}
+        if dump is not None:
+            dump_outputs(args.dump_outputs, dump)
         print(json.dumps(line))
     if dist is not None:
         dist.destroy_process_group()
@@ -473,11 +506,13 @@ def run_prefill(args, rank, world, local_rank):
     wbytes = sum(R.weight_bytes(t.dtype(), *t.shape()) for key in ("wq", "wk", "wv", "wo", "ffn_gate", "ffn_up", "ffn_down") for t in weights[key])
 
     def step():
+        outs = {}
         for l in range(conf.n_layers):
             for key in ("wq", "wk", "wv", "wo", "ffn_gate", "ffn_up"):
-                weights[key][l].matmul_vec(x_dim)
-            weights["ffn_down"][l].matmul_vec(x_hid)
-        return weights["output_weight"].matmul_vec(x_last)
+                outs[key] = weights[key][l].matmul_vec(x_dim)
+            outs["ffn_down"] = weights["ffn_down"][l].matmul_vec(x_hid)
+        outs["logits"] = weights["output_weight"].matmul_vec(x_last)
+        return outs            # the last layer's (b, m) products and the classifier row
     K, W = args.steps, args.warmup
     for _ in range(W):
         step()
@@ -486,9 +521,12 @@ def run_prefill(args, rank, world, local_rank):
     l0 = dev.launch_count()
     dev.timer_begin()
     for _ in range(K):
-        step()
+        outs = step()
     ms = dev.timer_end()
     launches = dev.launch_count() - l0
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, {k: v.export() for k, v in outs.items()})
+        outs = None
     # e2e: what crosses the host boundary in a prompt pass -- the token ids go host->device (the embedding rows are gathered on the
     # device, llama2.rs:223-224), the logits of the last position come back
     ids = [int(v) for v in rng.integers(0, conf.vocab_size, b)]
@@ -507,7 +545,7 @@ def run_prefill(args, rank, world, local_rank):
     clocks = sampler.stop()
     peaks, peak_src = measured_peaks()
     tf = flops / (ms / K * 1e-3) / 1e12
-    peak_tf = peaks.get("bf16_tflops_sustained", 1431.9)
+    peak_tf = peaks.get("bf16_tflops", 989.0)
     line = {"metric": "prefill_tokens_per_s", "value": b * K / (ms * 1e-3), "unit": "tok/s", "n_gpus": 1, "steps": K, "warmup": W, "ms_per_step": ms / K,
             "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f16 operand tiles (dequantised Q8_0 weights, quantised activations), f32 accumulate",
             "data": "synthetic",
@@ -518,10 +556,10 @@ def run_prefill(args, rank, world, local_rank):
                        "flop_per_step": flops},
             "e2e": {"value": b * K / (e2e_ms * 1e-3), "unit": "tok/s", "h2d_bytes_per_step": b * 8, "d2h_bytes_per_step": conf.vocab_size * 4, "ms_per_step": e2e_ms / K},
             "gpu_launches": int(launches),
-            "roofline": {"bound": "tensor", "kernel": "umma_gemm_kernel (prefill_gemm.cu): TMA -> smem ring -> tcgen05.mma kind::f16 -> TMEM -> tcgen05.ld epilogue",
-                         "achieved": tf, "peak": peak_tf, "peak_source": peak_src + " bf16_tflops_sustained", "unit": "TFLOP/s", "frac": tf / peak_tf, "traffic": None,
-                         "note": "whole step (dequantise + quantise + GEMM launches) over the dense FLOPs; the GEMM kernel alone is profiled in profiles/"},
-            "clocks": clocks}
+            "roofline": {"bound": "tensor", "kernel": "wgmma_gemm_kernel (prefill_gemm.cu): TMA -> smem ring -> wgmma m64n64k16 f16 -> register accumulator epilogue",
+                         "achieved": tf, "peak": peak_tf, "peak_source": peak_src + " bf16_tflops", "unit": "TFLOP/s", "frac": tf / peak_tf, "traffic": None,
+                         "note": "whole step (dequantise + quantise + GEMM launches) over the dense FLOPs"},
+            "clocks": clocks, "gpu": gpu_identity(local_rank)}
     print(json.dumps(line))
     dev.close()
 
@@ -539,6 +577,7 @@ def main():
     ap.add_argument("--prefill-tokens", type=int, default=4096)
     ap.add_argument("--no-also", action="store_true", help="skip the second (Q4_0) measurement of the default run")
     ap.add_argument("--multi", default="sharded", choices=["sharded", "replicas"], help="N > 1: shard one token stream (strong scaling, default) or run N independent replicas")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="after the timed steps, write what the last timed step computed as DIR/<name>.npy")
     ap.add_argument("--comm", default="p2p", choices=["p2p", "nccl"], help="exchange transport of the sharded path: one-shot NVLink peer stores (default) or the NCCL baseline")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))

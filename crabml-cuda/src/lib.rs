@@ -1,4 +1,4 @@
-//! CUDA (B200 / sm_100a) backend of crabml's `Tensor` trait.
+//! CUDA (H100 / sm_90a) backend of crabml's `Tensor` trait.
 //!
 //! `CudaTensor` implements `crabml::tensor::Tensor` (crabml-core/src/tensor/api.rs:11-79) on top of the C ABI of
 //! `libcrabml_cuda.so` (`include/crabml_cuda.h`): quantized GGUF blocks stay quantized on the device, the decode

@@ -1,4 +1,4 @@
-"""crabml_b200 -- B200-native CUDA backend for crabml's quantized decode path.
+"""crabml_b200 -- H100-native CUDA backend for crabml's quantized decode path.
 
 The product is the C-ABI shared library (include/crabml_cuda.h -> crabml_b200/lib/libcrabml_cuda.so).
 This Python package is a thin ctypes binding used by tests/ and bench.py; it mirrors the reference's

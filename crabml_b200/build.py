@@ -1,4 +1,4 @@
-"""Builds libcrabml_cuda.so (sm_100a only) in-tree with nvcc.  Used by __graft_entry__.build()."""
+"""Builds libcrabml_cuda.so (sm_90a only) in-tree with nvcc.  Used by __graft_entry__.build()."""
 from __future__ import annotations
 
 import glob
@@ -11,7 +11,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "lib", "libcrabml_cuda.so")
 
 NVCC_FLAGS = [
-    "-O3", "-std=c++17", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo",
+    "-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
     "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden",
     # parity: no FMA contraction, IEEE div/sqrt, no flush-to-zero (the reference is plain f32 Rust)
     "-fmad=false", "-prec-div=true", "-prec-sqrt=true", "-ftz=false",

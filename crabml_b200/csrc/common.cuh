@@ -1,5 +1,5 @@
 // common.cuh -- internal declarations shared by the CUDA translation units of libcrabml_cuda.
-// B200 (sm_100a) only.  No CPU fallback anywhere in this library.
+// H100 (sm_90a) only.  No CPU fallback anywhere in this library.
 #pragma once
 
 #include <cuda_fp16.h>
@@ -102,7 +102,7 @@ struct cc_device {
     struct LazyState* lz = nullptr;   // non-null in lazy mode (lazy.cu)
     std::string last_error;
     uint64_t launches = 0;
-    int sm_count = 148;
+    int sm_count = 132;          // H100 SXM; replaced by the device's count at creation
 
     // f16 LUTs (cpu_device.rs:108-124), computed on the host with libm and uploaded
     uint16_t* exp_lut = nullptr;
@@ -214,7 +214,7 @@ int cc_launch_act_to_blocks(cc_device* dev, const void* scratch, int64_t n, int 
 int cc_launch_matvec(cc_device* dev, const cc_buf* w, const void* act_scratch, const float* x_f32,
                      float* out, int64_t m, int64_t k, int64_t b);
 
-// ---- prefill_gemm.cu: batched matmul_vec on the tensor cores (TMA + tcgen05.mma, f16 operand tiles, f32 TMEM accumulator) ----
+// ---- prefill_gemm.cu: batched matmul_vec on the tensor cores (TMA + wgmma, f16 operand tiles, f32 register accumulator) ----
 bool cc_prefill_supported(int wtype, int64_t m, int64_t k, int64_t b);
 int cc_launch_prefill_matmul(cc_device* dev, const cc_buf* w, const void* act, const float* x_f32, float* out, int64_t m, int64_t k, int64_t b);
 void cc_prefill_release(cc_device* dev);

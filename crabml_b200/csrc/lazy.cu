@@ -1,7 +1,7 @@
 // lazy.cu -- lazy mode: record the trait calls of one forward(), fuse, replay as a CUDA graph.
 //
 // The reference's Tensor API is eager: ~31 calls per layer, ~1000 per token (SURVEY §3.2), each a separate launch in
-// eager mode.  profiles/r01c shows that per-launch overhead, not kernel bodies, is what caps decode.  In lazy mode the
+// eager mode.  Per-launch overhead, not kernel bodies, is what caps decode.  In lazy mode the
 // SAME C-ABI calls only append to a queue (after the same argument checks); the queue is executed at the first call that
 // needs a result on the host (export / debug tap / synchronize -- the reference synchronises only there too, llama2.rs:209):
 //   1. fuse: runs of ops that match the Llama decode layer (llama2.rs:226-269, 527-638) are replaced by the kernels of

@@ -1,11 +1,11 @@
 // matvec_stream.cu -- the streaming matvec for the decode hot path (b = 1).
 //
-// History (profiles/):
+// History:
 //   r01a  matvec.cu (warp per row, 4 loads in flight, activation staged before the first weight load, 1.33 waves):
-//         latency bound, 38 % of DRAM peak.
+//         latency bound.
 //   r01b  first persistent version with a per-group register ring and the Q8_0 quantisation of x fused into every
 //         CTA's prologue: 171 instructions per 1 KB group and 2.3 M redundant prologue instructions -> issue bound
-//         (IPC 1.5 with 3.7 warps / scheduler), 27 % of DRAM peak.  Lesson: this kernel must be ~20 instructions per
+//         (low IPC with few warps per scheduler).  Lesson: this kernel must be ~20 instructions per
 //         group, and x is quantised ONCE (quantize.cu / the producer's epilogue), not once per SM.
 //   this  persistent grid (2 CTAs x 8 warps per SM), rows dealt round-robin to warps; the weight stream of a warp is
 //         cut into SEGMENTS of 4 groups (4 x 32 blocks = 4096 weights = 4 KB of Q8_0) that are double-buffered in

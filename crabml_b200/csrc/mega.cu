@@ -4,17 +4,16 @@
 // MK_F_RING, or a phase table whose working area leaves the ring fewer than 12 slots) and the A/B baseline.  The phase bodies both
 // kernels share live in mega_phases.cuh; the host side at the bottom of this file serves both.
 //
-// Why: profiles/r01c -- on B200 a kernel boundary costs ~4-5 us for a full-GPU streaming kernel (drain, launch latency,
-// ramp-up) and ~2-3 us for a tiny one; a fused Llama-2-7B token still has ~260 of them (~1 ms), as much as the 1.05 ms the
-// weights need at HBM speed.  Here the whole token is ONE launch of one 512-thread CTA per SM that walks a table of
-// phases (built by lazy.cu from the recorded trait calls) separated by grid-wide barriers (2.15 us each, measured):
+// Why: a kernel boundary costs a few us for a full-GPU streaming kernel (drain, launch latency,
+// ramp-up); a fused Llama-2-7B token still has ~260 of them, of the order of the time the weights need at HBM speed.  Here the whole token is ONE launch of one 512-thread CTA per SM that walks a table of
+// phases (built by lazy.cu from the recorded trait calls) separated by grid-wide barriers:
 //     MATVEC  streaming matvec over 1-3 matrices + epilogue, optionally with a fused prologue ([dup] + rms_norm * w + Q8_0
 //             quantisation of the input row, recomputed by every CTA) and, on the sharded path, the exchange with the other GPUs
 //     NORMQ   the same normalise + quantise as a phase of its own (only when the f32 row must be materialised)
 //     ATTN    rope + KV append + attention + output quantise    (one CTA per head, K/V chunks through a TMA pipeline)
 //     ROWS    copy_rows_from (embedding row dequantisation)
 //     REDUCE / GATHER   second half of an exchange when it cannot fold into the next MATVEC prologue
-// Measurements and the per-phase time breakdown: profiles/r01f_megakernel_ncu.md.
+// The per-phase time breakdown: tools/mega_profile.py.
 // Data written by one CTA and read by another in a later phase is always read with ld.global.cg (L2), never through
 // the non-coherent L1.  All CTAs execute the same number of barriers.
 #define MK_SYNC() __syncthreads()
@@ -59,8 +58,7 @@ __device__ void phase_matvec(const MkPhase& ph, uint8_t* smem, float* s_w, bool 
     MkSeg& buf1 = P.buf1;
     if (ph.x) {
         // Fused prologue: [rms_norm * w] + Q8_0 quantisation of x, computed by EVERY CTA straight into its shared memory
-        // (redundant across SMs, ~1.5 us of issue time) -- cheaper than a separate NORMQ phase, which costs a grid barrier
-        // (~2.1 us) plus its own latency chain.  The weight segments requested by matvec_prefetch are in flight meanwhile.
+        // (redundant across SMs) -- cheaper than a separate NORMQ phase, which costs a grid barrier plus its own latency chain.  The weight segments requested by matvec_prefetch are in flight meanwhile.
         const int n = k;
         const int warp = threadIdx.x >> 5;
         float* s_red = (float*)(smem + (size_t)nbp * 40);                // scratch behind the activation arrays (256 B), then the 2 KB exchange stage
@@ -430,7 +428,7 @@ bool cc_mega_generic_supported(int type, int64_t k) {
 }
 
 // developer A/B switches: CRABML_MEGA_FLAGS replaces the default flag word (see MK_F_* and the L2 budget byte)
-#define MK_DEFAULT_FLAGS (MK_F_LOOK | MK_F_WSTAGE | MK_F_POLLCNT | MK_F_XEARLY | MK_F_RING | MK_F_RPAIR)      // ring + pairs: profiles/r02n (2227 us vs 2386 us per 7B Q8_0 token, same box)      // profiles/r02c: 2407 us vs 2586 us (0x5) on the same box
+#define MK_DEFAULT_FLAGS (MK_F_LOOK | MK_F_WSTAGE | MK_F_POLLCNT | MK_F_XEARLY | MK_F_RING | MK_F_RPAIR)      // ring + pairs: the fastest of the measured flag words
 int cc_mega_flags() {
     static const int f = getenv("CRABML_MEGA_FLAGS") ? (int)strtol(getenv("CRABML_MEGA_FLAGS"), nullptr, 0) : MK_DEFAULT_FLAGS;
     return f;
@@ -457,7 +455,7 @@ int cc_launch_mega(cc_device* dev, const MkPhase* phases_dev, int n_phases, cons
     // is co-resident by construction.  With another tenant on the same GPU (a second process, MPS) a partially scheduled grid
     // cannot finish a barrier: every spin in the kernel is bounded (MkSpin) and ends in CC_ERR_CUDA "megakernel barrier timeout"
     // instead of a hang; CRABML_MEGA_COOP=1 adds the cooperative launch attribute (all-or-nothing placement).  That is opt-in
-    // because a cooperative kernel node costs ~1.3 ms per graph launch on this driver (274 vs 416 tok/s, same call).
+    // because a cooperative kernel node in a CUDA graph is much slower to launch than a plain one.
     cudaLaunchConfig_t cfg;
     memset(&cfg, 0, sizeof(cfg));
     cfg.gridDim = dim3((unsigned)grid); cfg.blockDim = dim3(MK_THREADS); cfg.dynamicSmemBytes = smem; cfg.stream = dev->stream;

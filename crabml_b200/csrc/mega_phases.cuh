@@ -15,7 +15,7 @@
 #error "define MK_SYNC() before including mega_phases.cuh"
 #endif
 
-// one CTA of 16 warps per SM: the grid barrier has 148 participants instead of 296 (its cost is what bounds a phase)
+// one CTA of 16 warps per SM: the grid barrier has one participant per SM instead of two (its cost is what bounds a phase)
 #define MK_THREADS 512
 #define MK_WARPS 16
 #define MK_CTAS_PER_SM 1
@@ -29,8 +29,7 @@ __device__ __forceinline__ unsigned ld_acquire_u32(const unsigned* p) {
 }
 __device__ __forceinline__ void st_release_u32(unsigned* p, unsigned v) { asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory"); }
 
-// Split grid barrier (measured with tools/barrier_floor.py on B200, 148 CTAs: 2.1 us per phase; the two-level
-// acq_rel-atomic version cost 3.1 us, relaxed polling + fence 2.6 us):
+// Split grid barrier (tools/barrier_floor.py times it against a two-level acq_rel-atomic version and relaxed polling + fence):
 //   arrive : bar.sync, then ONE thread does a fire-and-forget red.release.gpu.add on a flat monotonic counter
 //            (the release publishes the CTA's phase output; that thread never issues prefetch loads);
 //   ...      the other warps may already issue the next phase's weight prefetch;
@@ -52,7 +51,7 @@ struct MkSpin {
 // (CTA i) red.release.gpu -> (CTA 0) ld.acquire.gpu ... fence.sys + st.release.sys -> (peer) ld.acquire.sys: release/acquire patterns of
 // different scopes compose (PTX memory model: causality order is transitive over morally strong synchronisation), so a system-scope
 // fence in EVERY CTA is not required (default: off; the 2-GPU parity test runs this way); sysfence = true adds it (it waits for this
-// CTA's NVLink stores to be acknowledged, ~2.5 us per exchange).
+// CTA's NVLink stores to be acknowledged).
 __device__ __forceinline__ void grid_barrier_arrive(unsigned* bar, unsigned nblocks, unsigned gen, bool xgpu = false, bool sysfence = false) {
     MK_SYNC();
     if (threadIdx.x == MK_BAR_THREAD) {
@@ -223,9 +222,9 @@ struct MkNext { StreamArgs mv; int wtype; int norm_n; const float* norm_w; };
 static_assert(sizeof(StreamArgs) % 4 == 0 && sizeof(StreamArgs) / 4 + 4 <= 64, "MkNext fetch layout: 64 threads per look-ahead slot");
 struct MkPipe { MkSeg buf0, buf1; };      // register stages of the weight stream, live across phases and barriers
 
-// (Tried and removed in round 2, profiles/r02a_*, r02b_*: an L2 look-ahead of each warp's coming rows -- cp.async.bulk.prefetch.L2 as
-// well as per-lane prefetch.global.L2 -- made the token 7-10 % SLOWER: a bulk prefetch request occupies its issuing thread for
-// ~9 us per 4 KB, line prefetches cost issue slots at the phase boundary, and the phase bodies already stream at HBM speed.)
+// (Tried and removed in round 2: an L2 look-ahead of each warp's coming rows -- cp.async.bulk.prefetch.L2 as
+// well as per-lane prefetch.global.L2 -- made the token SLOWER: a bulk prefetch request occupies its issuing thread for
+// a long time, line prefetches cost issue slots at the phase boundary, and the phase bodies already stream at HBM speed.)
 
 // geometry of one MATVEC phase for this warp
 struct MkGeo {
@@ -281,8 +280,8 @@ __device__ __forceinline__ MkRowPtr mk_vrow_ptr(const StreamMats& M, const MkGeo
 // shared memory: qs [k] | d [k/256] | bsums [k/16] (TKBase) | reduction scratch | f32 x
 __device__ __forceinline__ int mk_generic_sx_offset(int k) { return ((TKBase::smem_bytes(k) + 15) & ~15) + 256; }
 // __noinline__ (ring kernel): the K-quant row dots are register-hungry; as a called function they get their own allocation instead of pushing spills into
-// the streaming phases of the same kernel (profiles/r02s: every phase of the Q4_0 body was 15-25 % slower in the instantiation that carries
-// the generic code inline: 2335 vs 1938 us per token for a Q6_K classifier that itself costs 50 us more).
+// the streaming phases of the same kernel (every phase of the Q4_0 body was slower in the instantiation that carries
+// the generic code inline).
 // MK_GENERIC_NOINLINE (mega_ring.cu): as a called function with registers of its own.  In mega.cu the phase stays inline and borrows the
 // weight pipe's registers: there the pipe would have to be saved around every call.
 #ifndef MK_GENERIC_NOINLINE
@@ -662,7 +661,7 @@ static __device__ void phase_reduce(const MkPhase& ph, const CommDev& comm, unsi
 #define MK_F_WSTAGE 4
 #define MK_F_POLLCNT 8
 #define MK_F_SYSFENCE 256      // exchange phases: a system-scope fence in EVERY CTA before its arrival (not needed, see grid_barrier_arrive;
-                               // profiles/r02j: 2351 us vs 2265 us per token at N = 2)
+                               // measured faster at N = 2)
 #define MK_F_TESTSTALL 128     // test hook: the last CTA leaves before barrier 2 -> every other CTA must time out, not hang
 #define MK_F_XEARLY 64         // the f32 row of the next fused prologue is requested (cp.async) right after the barrier opens
 #define MK_F_KVPF 2048         // ring kernel: the producer warps prefetch the attention phase's cached K / V rows into L2 one phase ahead

@@ -1,15 +1,14 @@
 // mega_ring.cu -- the persistent decode kernel with the weight stream decoupled from the compute warps.
 //
-// Why (profiles/r02d, r02g): in mega.cu every warp alternates "issue the loads of a segment" and "consume a segment"; at a phase
-// boundary (slowest warp -> grid barrier -> activation prologue, 6-9 us) no warp issues loads, so only the 2 look-ahead segments per
-// warp (20 MB per GPU, 3 us of HBM time) cover the bubble and HBM idles for the rest: 2.36 ms per Llama-2-7B Q8_0 token against
-// 1.07 ms of pure streaming.  Weights are immutable, so nothing forces the weight stream to follow the phase order of the compute:
+// Why: in mega.cu every warp alternates "issue the loads of a segment" and "consume a segment"; at a phase
+// boundary (slowest warp -> grid barrier -> activation prologue) no warp issues loads, so only the 2 look-ahead segments per
+// warp cover the bubble and HBM idles for the rest.  Weights are immutable, so nothing forces the weight stream to follow the phase order of the compute:
 //   * warps 16-19 of every CTA are PRODUCERS: their threads walk the phase table on their own, ahead of the compute warps, and
 //     issue cp.async.bulk (TMA) copies of row segments (4 groups of 32 blocks: 4096 B of Q8_0 quants + 256 B of f16 scales) into a
 //     ring of shared-memory slots -- as many as fit beside the per-phase working area (~37-47 slots = 160-200 KB per SM, 24-30 MB
 //     per GPU in flight or landed).  It never waits for a barrier or an activation: whenever a slot is free the next segment of
 //     this CTA's rows -- of this phase or any later one -- is already being fetched.
-//   * warps 0-15 are CONSUMERS: same row dealing (row r -> CTA r % 148, rows of a CTA -> its warps round-robin), same per-lane
+//   * warps 0-15 are CONSUMERS: same row dealing (row r -> CTA r % gridDim.x, rows of a CTA -> its warps round-robin), same per-lane
 //     block order, same arithmetic as mega.cu / matvec_stream.cu (bit-identical results), but a segment is read from the ring with
 //     LDS.128 after waiting on the slot's "full" mbarrier, and the slot is handed back through its "empty" mbarrier.  No weight
 //     registers live across phases -> no register pipe, no look-ahead bookkeeping, 96 registers are enough.
@@ -93,12 +92,12 @@ __device__ __forceinline__ int mr_locate(const StreamMats& M, const MrGeo& g, in
 }
 
 // ---- producer warp: runs ahead of everybody ---------------------------------------------------------------------------------------------
-// All 32 lanes issue (a single issuing thread manages ~1 entry per 350 cycles -- profiles/r02m: 1.8 TB/s); lane l owns the entries l, l + 32, ...
+// All 32 lanes issue (a single issuing thread manages only ~1 entry per few hundred cycles); lane l owns the entries l, l + 32, ...
 // of a phase: it decomposes the entry index into (unit, virtual row, segment), waits until the slot's previous tenant has been consumed, arms the
 // slot's "full" barrier with the byte count, issues the two bulk copies (quants, scales) and publishes the entry number in the slot's
 // sequence word.  Consumers check that word before they look at the barrier: an mbarrier parity alone cannot tell "this use has not
 // landed" from "the previous use has not landed" when a warp gets more than one lap ahead (16 warps x 3 segments > 40 slots).
-// (Measured, profiles/r02q: 1 / 2 / 4 / 8 producer warps = 2859 / 2782 / 2262 / 2435 us per token -- a warp's probe-and-issue trip takes ~400
+// (Measured on the earlier target: 4 producer warps were the fastest of 1 / 2 / 4 / 8 -- a warp's probe-and-issue trip takes ~400
 // cycles, so the number of polling warps bounds the refill rate, and at 8 the 80-register cap starts to cost.  Sleeping after a failed probe,
 // SIMT-wide parameter computation, in-order probe loops and fence-free hand-back words changed nothing.)
 __device__ void mr_producer(const MkPhase* __restrict__ phases, int n_phases, const MrRing R, unsigned full0, unsigned done0, unsigned ring0,
@@ -116,8 +115,8 @@ __device__ void mr_producer(const MkPhase* __restrict__ phases, int n_phases, co
         for (int j = 0; j < MR_DESC_PER_LANE; j++) { const int i = lane + 32 * j; nw[j] = (p + 1 < n_phases && i < MR_DESC_WORDS) ? ((const int*)(phases + p + 1))[i] : 0; }
         const MkPhase& ph = s_pd[p & 1];
         if (kvpf && ph.type == MK_ATTN) {
-            // The attention phase streams a head's K and V rows through 48 KB of shared memory: latency x bytes in flight = 32 GB/s per head
-            // (profiles/r02y: +0.04 us per cached position and layer).  The producers reach this table entry while the compute warps are still in
+            // The attention phase streams a head's K and V rows through 48 KB of shared memory: bytes in flight over latency bounds the rate
+            // (the attention phase grows with every cached position and layer).  The producers reach this table entry while the compute warps are still in
             // the qkv phase: they ask L2 for the cached rows [0, kv_len) of every kv head now, so that the phase's bulk copies hit L2.
             // (rows written by earlier launches: stable; the current token's row never goes through the cache on its way to the phase)
             const AttnArgs& a = ph.at;
@@ -238,7 +237,7 @@ __device__ __forceinline__ void mr_seg_lds(MkSeg& S, const uint8_t* sp, int seg,
 
 // Activation quants in shared memory, per group of 32 blocks: the 16-byte first halves of all 32 blocks, then the second halves (the layout of
 // the Q8_0 weight plane) -- lane l reads block 32 g + l with two conflict-free LDS.128 (block-major, 32 bytes apart, is a 2-way bank conflict:
-// 64 instead of 32 shared-memory wavefronts per segment, and the ring's throughput is bounded by shared-memory bandwidth, profiles/r02n)
+// 64 instead of 32 shared-memory wavefronts per segment, and the ring's throughput is bounded by shared-memory bandwidth)
 __device__ __forceinline__ int mr_act_word(int i) {           // i = 4-byte word index in block-major order (block i >> 3, word i & 7)
     const int b = i >> 3, w = i & 7;
     return (b >> 5) * 256 + (w >> 2) * 128 + (b & 31) * 4 + (w & 3);

@@ -1,18 +1,17 @@
 // prefill_gemm.cu -- the dense (prefill) path of matmul_vec: C[b, m] = sum_k W[m, k] * x[b, k] for a BATCH of activation rows
 // (Tensor::matmul_vec with a (b, k) rhs: cpu_tensor.rs:368-386, primitives/matmul_vec.rs:26-78; the prompt walk of
-// llama2.rs:111-139).  With b >= 32 rows the contraction is genuinely dense, so it runs on the 5th-generation tensor cores:
+// llama2.rs:111-139).  With b >= 32 rows the contraction is genuinely dense, so it runs on the Hopper tensor cores (wgmma):
 //
 //   1. dequant_w_f16_kernel : GGUF quant blocks (device plane layout, any of the 11 weight types) -> f16 tile source [m][k], ONCE per
-//      weight (kept beside the quantised planes: 180 GB of HBM hold a 7B model's 14 GB of f16 many times over)
+//      weight (kept beside the quantised planes: a 7B model's 13-14 GB of f16 fit in 80 GB of HBM next to its quantised weights)
 //      (w = f32 dequantised value as BlockQ*::dequantize gives it, rounded once to f16: |q| <= 127 times an f16 scale)
 //   2. act_q8_to_f16_kernel : the activation is quantised to Q8_0 exactly like the decode path (buf_q8_0.rs:87-134) and the
 //      quantised value q * d is what enters the GEMM, so the only deviation from the reference is the f16 rounding of the two
 //      operands (relative 2^-11 each) and the f32 accumulation order
-//   3. umma_gemm_kernel     : TMA (cp.async.bulk.tensor.2d, 128-byte swizzle) stages [128 x 64] / [N x 64] f16 tiles into a
-//      4-deep shared-memory ring; ONE elected thread issues tcgen05.mma.cta_group::1.kind::f16 (M = 128, N = 64..256, K = 16)
-//      with the f32 accumulator in TMEM; tcgen05.commit hands smem slots back to the TMA producer and the finished
-//      accumulator to four epilogue warps, which read it with tcgen05.ld and store C[b][m] (m contiguous across lanes).
-//      Warp roles: 0 TMA producer, 1 MMA issuer, 2 TMEM allocator, 4-7 epilogue.
+//   3. wgmma_gemm_kernel    : TMA (cp.async.bulk.tensor.2d, 128-byte swizzle) stages [128 x 64] / [N x 64] f16 tiles into a
+//      4-deep shared-memory ring; two consumer warpgroups each own 64 weight rows and issue
+//      wgmma.mma_async.m64n64k16.f32.f16.f16 (N / 64 per 16-wide K step) with the f32 accumulator in registers, then store
+//      C[b][m] straight from those registers.  Warpgroup roles: 0 TMA producer (one thread), 1-2 MMA + epilogue.
 // MMA-M is the WEIGHT row dimension (large: 4096 .. 32000), MMA-N the batch dimension.
 // Every mbarrier wait is bounded (trap after ~2 s) so that a descriptor mistake ends in an error, not a hung GPU.
 #include <cuda.h>
@@ -22,11 +21,11 @@
 #include "common.cuh"
 #include "dequant.cuh"
 
-#define PG_BLOCK_M 128
+#define PG_BLOCK_M 128                    // 2 consumer warpgroups x 64 rows
 #define PG_BLOCK_K 64                     // 64 f16 = 128 bytes = one swizzle-128B row
 #define PG_STAGES 4
-#define PG_THREADS 256
-#define PG_UMMA_K 16
+#define PG_THREADS 384                    // 3 warpgroups
+#define PG_MMA_K 16
 
 // ---- PTX helpers ------------------------------------------------------------------------------------------------------------
 __device__ __forceinline__ unsigned pg_smem(const void* p) { return (unsigned)__cvta_generic_to_shared(p); }
@@ -34,6 +33,7 @@ __device__ __forceinline__ void pg_mbar_init(unsigned bar, unsigned count) { asm
 __device__ __forceinline__ void pg_mbar_expect_tx(unsigned bar, unsigned bytes) {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
 }
+__device__ __forceinline__ void pg_mbar_arrive(unsigned bar) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory"); }
 __device__ __forceinline__ void pg_mbar_wait(unsigned bar, unsigned parity) {
     unsigned done = 0;
     for (unsigned it = 0; !done; it++) {
@@ -45,149 +45,110 @@ __device__ __forceinline__ void pg_tma_load_2d(unsigned dst, const void* tmap, u
     asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
                  ::"r"(dst), "l"(tmap), "r"(bar), "r"(x), "r"(y) : "memory");
 }
-__device__ __forceinline__ void pg_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void pg_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-// D[tmem] (+)= A[smem] * B[smem]^T, f16 inputs, f32 accumulate; issued by ONE thread
-__device__ __forceinline__ void pg_umma_f16(unsigned tmem_d, uint64_t desc_a, uint64_t desc_b, unsigned idesc, unsigned accumulate) {
-    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\ntcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n}\n"
-                 ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate) : "memory");
-}
-// all tcgen05 operations issued so far by this thread arrive (once) on the mbarrier when they complete
-__device__ __forceinline__ void pg_umma_commit(unsigned bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
 // shared-memory matrix descriptor of a K-major tile stored as rows of 128 bytes with the 128-byte swizzle (what the TMA box
 // {64 x rows} with CU_TENSOR_MAP_SWIZZLE_128B writes): 8-row groups are 1024 bytes apart (stride byte offset), the leading byte
-// offset is unused for swizzled K-major operands, descriptor version 1 (sm_100), layout type 2 = SWIZZLE_128B.
+// offset is unused for swizzled K-major operands, layout type 1 = SWIZZLE_128B (sm_90 encoding).  Tiles start 1024-aligned, so the
+// base offset is 0.
 __device__ __forceinline__ uint64_t pg_smem_desc(unsigned smem_addr) {
     uint64_t d = 0;
     d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);                  // bits [0, 14): start address >> 4
-    d |= (uint64_t)0 << 16;                                       // bits [16, 30): leading byte offset >> 4
+    d |= (uint64_t)1 << 16;                                       // bits [16, 30): leading byte offset >> 4 (unused)
     d |= (uint64_t)(1024 >> 4) << 32;                             // bits [32, 46): stride byte offset >> 4
-    d |= (uint64_t)1 << 46;                                       // bits [46, 48): descriptor version
-    d |= (uint64_t)2 << 61;                                       // bits [61, 64): SWIZZLE_128B
+    d |= (uint64_t)1 << 62;                                       // bits [62, 64): SWIZZLE_128B
     return d;
 }
-// instruction descriptor of kind::f16: f32 accumulator, f16 A and B, both K-major, dense
-__host__ __device__ constexpr unsigned pg_instr_desc(int umma_m, int umma_n) {
-    return (1u << 4)                          // bits [4, 6): accumulator format, 1 = F32
-           | (0u << 7) | (0u << 10)           // bits [7, 10) / [10, 13): A / B format, 0 = F16
-           | (0u << 15) | (0u << 16)          // A / B major: 0 = K-major
-           | ((unsigned)(umma_n >> 3) << 17)  // bits [17, 23): N >> 3
-           | ((unsigned)(umma_m >> 4) << 24); // bits [24, 29): M >> 4
+__device__ __forceinline__ void pg_wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void pg_wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void pg_wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// D[64 x 64] (+)= A[64 x 16] * B[64 x 16]^T, both K-major in shared memory, f16 inputs, f32 accumulator in registers (the warpgroup's
+// 128 threads hold 32 values each); issued by the whole warpgroup
+__device__ __forceinline__ void pg_wgmma_64x64(float (&d)[32], uint64_t desc_a, uint64_t desc_b, int accumulate) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n}\n"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+                 : "l"(desc_a), "l"(desc_b), "r"(accumulate));
 }
 
 struct PgShared {
-    unsigned long long full[PG_STAGES], empty[PG_STAGES], tmem_full;      // (3 or PG_STAGES slots in use)
-    unsigned tmem_base;
+    unsigned long long full[PG_STAGES], empty[PG_STAGES];
 };
 
-// grid: (ceil(m / (128 * MT)), ceil(b / BLOCK_N)); dynamic smem: 1024-aligned ring of STAGES x (A tile MT x 16 KB + B tile BLOCK_N*128 B)
-// MT = 2: the CTA owns a 256-row weight tile as TWO M = 128 accumulators (2 x BLOCK_N TMEM columns) that share every B tile -- 1.5x
-// fewer operand bytes per FLOP than 128 x 256 tiles, which matters because 148 CTAs pulling 48 KB per 128x256x64 step ask more of L2
-// than it delivers (profiles/r02e: 47 % tensor pipe with MT = 1).
-template <int BLOCK_N, int MT>
-__global__ void __launch_bounds__(PG_THREADS, 1) umma_gemm_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant__ CUtensorMap tmap_x,
-                                                                  float* __restrict__ C, int m, int b, int k) {
+// grid: (ceil(m / 128), ceil(b / BLOCK_N)); dynamic smem: 1024-aligned ring of PG_STAGES x (A tile 16 KB + B tile BLOCK_N * 128 B),
+// at most 4 x 48 KB.  The accumulator of a consumer warpgroup is BLOCK_N / 2 registers per thread (128 at BLOCK_N = 256).
+template <int BLOCK_N>
+__global__ void __launch_bounds__(PG_THREADS, 1) wgmma_gemm_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant__ CUtensorMap tmap_x,
+                                                                   float* __restrict__ C, int m, int b, int k) {
     extern __shared__ __align__(1024) uint8_t pg_smem_raw[];
     __shared__ PgShared sh;
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    constexpr unsigned A_TILE = PG_BLOCK_M * PG_BLOCK_K * 2, A_BYTES = MT * A_TILE, B_BYTES = BLOCK_N * PG_BLOCK_K * 2;
-    constexpr unsigned TMEM_COLS = MT * BLOCK_N < 32 ? 32 : MT * BLOCK_N;     // power of two >= 32 (64 .. 512)
-    constexpr int STAGES = (A_BYTES + B_BYTES) * PG_STAGES <= 200 * 1024 ? PG_STAGES : 3;
+    const int wg = threadIdx.x >> 7, t = threadIdx.x & 127;
+    constexpr unsigned A_BYTES = PG_BLOCK_M * PG_BLOCK_K * 2, B_BYTES = BLOCK_N * PG_BLOCK_K * 2, STAGE = A_BYTES + B_BYTES;
+    constexpr int NJ = BLOCK_N / 64;
     uint8_t* ring = (uint8_t*)(((uintptr_t)pg_smem_raw + 1023) & ~(uintptr_t)1023);
     const int num_kb = k / PG_BLOCK_K;
-    const int m0 = blockIdx.x * PG_BLOCK_M * MT, n0 = blockIdx.y * BLOCK_N;
+    const int m0 = blockIdx.x * PG_BLOCK_M, n0 = blockIdx.y * BLOCK_N;
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_w) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_x) : "memory");
-    }
-    if (warp == 1 && lane == 0) {
-        for (int s = 0; s < STAGES; s++) { pg_mbar_init(pg_smem(&sh.full[s]), 1); pg_mbar_init(pg_smem(&sh.empty[s]), 1); }
-        pg_mbar_init(pg_smem(&sh.tmem_full), 1);
+        for (int s = 0; s < PG_STAGES; s++) { pg_mbar_init(pg_smem(&sh.full[s]), 1); pg_mbar_init(pg_smem(&sh.empty[s]), 2); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 2) {                       // one warp allocates the accumulator columns and writes their base to shared memory
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(pg_smem(&sh.tmem_base)), "n"(TMEM_COLS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    pg_fence_before();
     __syncthreads();
-    pg_fence_after();
-    const unsigned tmem_acc = sh.tmem_base;
 
-    if (warp == 0) {
-        // ===== TMA producer =====
-        if (lane == 0) {
+    if (wg == 0) {
+        // ===== TMA producer: a single thread =====
+        if (t == 0) {
             for (int kb = 0; kb < num_kb; kb++) {
-                const int s = kb % STAGES;
-                const unsigned ph = (unsigned)(kb / STAGES) & 1u;
+                const int s = kb % PG_STAGES;
+                const unsigned ph = (unsigned)(kb / PG_STAGES) & 1u;
                 pg_mbar_wait(pg_smem(&sh.empty[s]), ph ^ 1u);           // slot free (passes at once on the first round)
                 const unsigned full = pg_smem(&sh.full[s]);
-                pg_mbar_expect_tx(full, A_BYTES + B_BYTES);
-                uint8_t* st = ring + (size_t)s * (A_BYTES + B_BYTES);
-#pragma unroll
-                for (int t = 0; t < MT; t++) pg_tma_load_2d(pg_smem(st + t * A_TILE), &tmap_w, full, kb * PG_BLOCK_K, m0 + t * PG_BLOCK_M);
+                pg_mbar_expect_tx(full, STAGE);
+                uint8_t* st = ring + (size_t)s * STAGE;
+                pg_tma_load_2d(pg_smem(st), &tmap_w, full, kb * PG_BLOCK_K, m0);
                 pg_tma_load_2d(pg_smem(st + A_BYTES), &tmap_x, full, kb * PG_BLOCK_K, n0);
             }
         }
-    } else if (warp == 1) {
-        // ===== MMA issuer: a single thread =====
-        if (lane == 0) {
-            constexpr unsigned idesc = pg_instr_desc(PG_BLOCK_M, BLOCK_N);
-            for (int kb = 0; kb < num_kb; kb++) {
-                const int s = kb % STAGES;
-                const unsigned ph = (unsigned)(kb / STAGES) & 1u;
-                pg_mbar_wait(pg_smem(&sh.full[s]), ph);                  // TMA landed this stage
-                pg_fence_after();
-                uint8_t* st = ring + (size_t)s * (A_BYTES + B_BYTES);
-                const uint64_t db = pg_smem_desc(pg_smem(st + A_BYTES));
-#pragma unroll
-                for (int t = 0; t < MT; t++) {
-                    const uint64_t da = pg_smem_desc(pg_smem(st + t * A_TILE));
-#pragma unroll
-                    for (int kk = 0; kk < PG_BLOCK_K / PG_UMMA_K; kk++) {
-                        // advancing K inside the 128-byte swizzle atom = advancing the (pre-swizzle) start address by 32 bytes
-                        const uint64_t adv = (uint64_t)((kk * PG_UMMA_K * 2) >> 4);
-                        pg_umma_f16(tmem_acc + (unsigned)(t * BLOCK_N), da + adv, db + adv, idesc, (kb > 0 || kk > 0) ? 1u : 0u);
-                    }
-                }
-                pg_umma_commit(pg_smem(&sh.empty[s]));                   // frees the slot once these MMAs have read it
-            }
-            pg_umma_commit(pg_smem(&sh.tmem_full));                      // accumulator complete
-        }
-    } else if (warp >= 4) {
-        // ===== epilogue: TMEM -> registers -> C[b][m] =====
-        const int q = warp & 3;                                          // a warp reads the TMEM lanes 32 * (warp % 4) ..
-        pg_mbar_wait(pg_smem(&sh.tmem_full), 0);
-        pg_fence_after();
-#pragma unroll 1
-        for (int cc = 0; cc < MT * BLOCK_N; cc += 32) {
-            const int t = cc / BLOCK_N, c0 = cc - t * BLOCK_N;          // accumulator t holds the weight rows m0 + 128 t ..
-            const int row = m0 + t * PG_BLOCK_M + q * 32 + lane;         // weight row = output column index
-            unsigned v[32];
-            const unsigned taddr = tmem_acc + ((unsigned)(q * 32) << 16) + (unsigned)cc;
-            asm volatile(
-                "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, "
-                "%23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-                : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]),
-                  "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]),
-                  "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-                : "r"(taddr));
-            asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-            if (row < m) {
-#pragma unroll
-                for (int j = 0; j < 32; j++) {
-                    const int bi = n0 + c0 + j;
-                    if (bi < b) C[(size_t)bi * m + row] = __uint_as_float(v[j]);      // lanes = consecutive rows: 128-byte stores
-                }
-            }
-        }
+        return;
     }
-    pg_fence_before();
-    __syncthreads();
-    if (warp == 2) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_acc), "n"(TMEM_COLS) : "memory");
+    // ===== consumers: warpgroup c = wg - 1 owns weight rows m0 + 64 c .. m0 + 64 c + 63 =====
+    const int c = wg - 1;
+    float acc[NJ][32];
+#pragma unroll
+    for (int j = 0; j < NJ; j++)
+#pragma unroll
+        for (int i = 0; i < 32; i++) acc[j][i] = 0.0f;
+    for (int kb = 0; kb < num_kb; kb++) {
+        const int s = kb % PG_STAGES;
+        const unsigned ph = (unsigned)(kb / PG_STAGES) & 1u;
+        pg_mbar_wait(pg_smem(&sh.full[s]), ph);                          // TMA landed this stage
+        uint8_t* st = ring + (size_t)s * STAGE;
+        const uint64_t da = pg_smem_desc(pg_smem(st + c * 64 * 128));
+        const uint64_t db = pg_smem_desc(pg_smem(st + A_BYTES));
+        pg_wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < PG_BLOCK_K / PG_MMA_K; kk++) {
+            // advancing K inside the 128-byte swizzle atom = advancing the (pre-swizzle) start address by 32 bytes
+            const uint64_t adv = (uint64_t)((kk * PG_MMA_K * 2) >> 4);
+#pragma unroll
+            for (int j = 0; j < NJ; j++) pg_wgmma_64x64(acc[j], da + adv, db + (uint64_t)((j * 64 * 128) >> 4) + adv, 1);
+        }
+        pg_wgmma_commit();
+        pg_wgmma_wait<1>();                                              // the MMAs of stage kb - 1 have read their operands
+        if (kb > 0 && t == 0) pg_mbar_arrive(pg_smem(&sh.empty[(kb - 1) % PG_STAGES]));
+    }
+    pg_wgmma_wait<0>();
+    // ===== epilogue: registers -> C[b][m].  wgmma's f32 layout: thread t of the warpgroup holds, for column chunk j and i = 0..31,
+    // row 16 (t / 32) + (t % 32) / 4 + 8 ((i / 2) % 2), column 64 j + 8 (i / 4) + 2 (t % 4) + i % 2.
+    const int r0 = m0 + c * 64 + 16 * (t >> 5) + ((t & 31) >> 2);
+#pragma unroll
+    for (int j = 0; j < NJ; j++)
+#pragma unroll
+        for (int i = 0; i < 32; i++) {
+            const int row = r0 + 8 * ((i >> 1) & 1), bi = n0 + 64 * j + 8 * (i >> 2) + 2 * (t & 3) + (i & 1);
+            if (row < m && bi < b) C[(size_t)bi * m + row] = acc[j][i];
+        }
 }
 
 // ---- operand preparation ---------------------------------------------------------------------------------------------------------
@@ -286,20 +247,18 @@ bool cc_prefill_supported(int wtype, int64_t m, int64_t k, int64_t b) {
     return b >= min_b && k % PG_BLOCK_K == 0 && k >= PG_BLOCK_K && m >= 1 && (at == CC_Q8_0 || at == CC_Q8_K);
 }
 
-template <int BLOCK_N, int MT>
+template <int BLOCK_N>
 static int pg_launch(cc_device* dev, const CUtensorMap& tw, const CUtensorMap& tx, float* out, int64_t m, int64_t b, int64_t k) {
-    const size_t stage = (size_t)MT * PG_BLOCK_M * PG_BLOCK_K * 2 + (size_t)BLOCK_N * PG_BLOCK_K * 2;
-    const int stages = stage * PG_STAGES <= 200 * 1024 ? PG_STAGES : 3;
-    const size_t smem = (size_t)stages * stage + 1024;
-    CC_CUDA(dev, cudaFuncSetAttribute(umma_gemm_kernel<BLOCK_N, MT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    dim3 grid((unsigned)((m + PG_BLOCK_M * MT - 1) / (PG_BLOCK_M * MT)), (unsigned)((b + BLOCK_N - 1) / BLOCK_N));
-    umma_gemm_kernel<BLOCK_N, MT><<<grid, PG_THREADS, smem, dev->stream>>>(tw, tx, out, (int)m, (int)b, (int)k);
+    const size_t smem = (size_t)PG_STAGES * ((size_t)PG_BLOCK_M * PG_BLOCK_K * 2 + (size_t)BLOCK_N * PG_BLOCK_K * 2) + 1024;
+    CC_CUDA(dev, cudaFuncSetAttribute(wgmma_gemm_kernel<BLOCK_N>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    dim3 grid((unsigned)((m + PG_BLOCK_M - 1) / PG_BLOCK_M), (unsigned)((b + BLOCK_N - 1) / BLOCK_N));
+    wgmma_gemm_kernel<BLOCK_N><<<grid, PG_THREADS, smem, dev->stream>>>(tw, tx, out, (int)m, (int)b, (int)k);
     CC_LAUNCH_CHECK(dev);
     return CC_OK;
 }
 
-// Dequantised weights are kept: with 180 GB of HBM a 7B model's f16 tile source (2 bytes per weight, 13-14 GB) fits many times over,
-// and dequantising 58 MB per matrix on every call costs as much as the GEMM itself (profiles/r02e).  CRABML_PREFILL_NOCACHE=1 keeps
+// Dequantised weights are kept: with 80 GB of HBM a 7B model's f16 tile source (2 bytes per weight, 13-14 GB) fits beside its
+// quantised weights, and dequantising 58 MB per matrix on every call costs as much as the GEMM itself.  CRABML_PREFILL_NOCACHE=1 keeps
 // the round-trip through one reusable scratch buffer instead (memory-constrained deployments).
 static int pg_weight_f16(cc_device* dev, const cc_buf* w, int64_t m, int64_t k, PgScratch* s, const void** out) {
     static const bool nocache = getenv("CRABML_PREFILL_NOCACHE") != nullptr;
@@ -342,9 +301,7 @@ int cc_launch_prefill_matmul(cc_device* dev, const cc_buf* w, const void* act_q8
     if (rc) return rc;
     rc = pg_make_tmap(dev, &tx, s->x, b, k, block_n);
     if (rc) return rc;
-    static const bool one_tile = getenv("CRABML_PREFILL_MT1") != nullptr;          // developer A/B: 128-row CTA tiles
-    const bool mt2 = !one_tile && m >= 512;
-    if (block_n == 256) return mt2 ? pg_launch<256, 2>(dev, tw, tx, out, m, b, k) : pg_launch<256, 1>(dev, tw, tx, out, m, b, k);
-    if (block_n == 128) return mt2 ? pg_launch<128, 2>(dev, tw, tx, out, m, b, k) : pg_launch<128, 1>(dev, tw, tx, out, m, b, k);
-    return mt2 ? pg_launch<64, 2>(dev, tw, tx, out, m, b, k) : pg_launch<64, 1>(dev, tw, tx, out, m, b, k);
+    if (block_n == 256) return pg_launch<256>(dev, tw, tx, out, m, b, k);
+    if (block_n == 128) return pg_launch<128>(dev, tw, tx, out, m, b, k);
+    return pg_launch<64>(dev, tw, tx, out, m, b, k);
 }

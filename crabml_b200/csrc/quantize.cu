@@ -133,7 +133,7 @@ __global__ void act_to_blocks_kernel(int t, const void* scratch, int64_t n, uint
         if (b >= n / 32) return;
         uint8_t* o = out + b * 34;
         // 16-bit store on purpose: ptxas 12.9 folds `cvt.rn.f16.f32` + a truncating byte store into a
-        // NUMERIC F2I.U8.F16 (observed on sm_100a), so never narrow f16 bits with `& 0xFF`.
+        // NUMERIC F2I.U8.F16 (observed with ptxas 12.9 for sm_100a), so never narrow f16 bits with `& 0xFF`.
         *reinterpret_cast<__half*>(o) = __float2half_rn(a0.d[b]);
         for (int i = 0; i < 32; i++) o[2 + i] = (uint8_t)a0.qs[b * 32 + i];
     } else if (t == CC_Q8_1) {

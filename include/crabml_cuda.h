@@ -1,5 +1,5 @@
 /*
- * crabml_cuda.h -- C ABI of the B200-native CUDA backend for crabml's quantized tensor-op path.
+ * crabml_cuda.h -- C ABI of the H100-native CUDA backend for crabml's quantized tensor-op path.
  *
  * This is the drop-in boundary: one entry point per method of the reference's `Tensor` trait
  * (crabml-core/src/tensor/api.rs:11-79).  A Rust `crabml-cuda` crate binds these with

@@ -9,17 +9,14 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100; run with -m gpu)")
 
 
 def find_fixture(name):
-    """GGUF fixtures are the reference's testdata; they are copied (git-ignored) into
-    oracle/_ref/testdata by __graft_entry__.build() so that they travel to the GPU box."""
-    for d in (os.path.join(ROOT, "oracle", "_ref", "testdata"), "/root/reference/testdata"):
-        p = os.path.join(d, name)
-        if os.path.exists(p):
-            return p
-    return None
+    """GGUF fixtures are the upstream project's test models; __graft_entry__.build() copies them (git-ignored) into
+    oracle/_ref/testdata (oracle/fixtures.py)."""
+    p = os.path.join(ROOT, "oracle", "_ref", "testdata", name)
+    return p if os.path.exists(p) else None
 
 
 @pytest.fixture
@@ -27,6 +24,6 @@ def fixture_path():
     def _get(name):
         p = find_fixture(name)
         if p is None:
-            pytest.skip(f"fixture {name} not available (run __graft_entry__.build() where /root/reference exists)")
+            pytest.skip(f"fixture {name} not available (run __graft_entry__.build() with an upstream crabml checkout, see oracle/fixtures.py)")
         return p
     return _get

@@ -1,7 +1,7 @@
 """Regenerates tests/golden/*_logits.npz from the reference's GGUF fixtures with the CPU oracle.
 
-Run where /root/reference exists:  python tests/golden/make_golden.py
-The reference (nightly Rust) cannot be executed in this image; these vectors are outputs of the
+Run after __graft_entry__.build() has copied the fixtures (oracle/fixtures.py):  python tests/golden/make_golden.py
+The reference (nightly Rust) is not built here; these vectors are outputs of the
 oracle, which is itself pinned by the reference's KATs and golden strings (tests/test_oracle_*).
 """
 import os

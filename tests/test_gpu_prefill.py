@@ -1,4 +1,4 @@
-"""The dense (prefill) path of matmul_vec: (m, k) @ (b, k) for b >= 32 rows runs as TMA + tcgen05.mma tiles
+"""The dense (prefill) path of matmul_vec: (m, k) @ (b, k) for b >= 32 rows runs as TMA + wgmma tiles
 (csrc/prefill_gemm.cu).  Reference behaviour: the batched rhs of primitives/matmul_vec.rs:6-8,26-78 (every output element
 is vec_dot(W row, Q8_0-quantised activation row)).
 
@@ -75,8 +75,8 @@ def test_prefill_dense_7b_shapes(gdev, t):
 
 
 def test_prefill_dense_256_row_cta_tiles(gdev):
-    # m >= 512: a CTA owns 256 weight rows as two M = 128 accumulators sharing every activation tile; ragged second tile (640 = 2 x 256
-    # + 128, 1000 = 3 x 256 + 232) and all three N tiles
+    # several 128-row CTA tiles (one 64-row half per consumer warpgroup) with a ragged last tile (1000 = 7 x 128 + 104) and all three
+    # N tiles (64, 128, 256 batch rows)
     run_dense(gdev, oc.Q8_0, 640, 512, 64, seed=81)
     run_dense(gdev, oc.Q8_0, 1000, 1024, 130, seed=82)
     run_dense(gdev, oc.Q4_0, 1024, 2048, 300, seed=83)

@@ -8,7 +8,7 @@ import itertools
 import pytest
 
 MK_SEG = 4
-GRID = 148
+GRID = 132                     # one CTA per SM of an H100 SXM
 
 
 def geo(m, n_mats, k, epilogue, cta, grid=GRID):

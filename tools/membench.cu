@@ -1,7 +1,8 @@
-// membench.cu -- what read bandwidth can a streaming kernel reach on this B200, and with which shape?
-// (developer tool; informs matvec_stream.cu).  Build: nvcc -O3 -gencode arch=compute_100a,code=sm_100a -o tools/build/membench tools/membench.cu
+// membench.cu -- what read bandwidth can a streaming kernel reach on this H100, and with which shape?
+// (developer tool; informs matvec_stream.cu).  Build: nvcc -O3 -gencode arch=compute_90a,code=sm_90a -o tools/build/membench tools/membench.cu
 #include <cstdio>
 #include <cstdint>
+#include <vector>
 #include <cuda_runtime.h>
 
 __device__ __forceinline__ int4 ld_nc(const int4* p) {
@@ -134,7 +135,8 @@ int main(int argc, char** argv) {
     cudaMalloc(&buf, bytes); cudaMalloc(&out, 4);
     cudaMemset(buf, 1, bytes);
     size_t n = bytes / 16;
-    int sms = 148;
+    int sms = 0;
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
     printf("buffer %zu MB\n", bytes >> 20);
 #define RUN_A(U, NC, CPS, T) { float ms = timeit([&] { k_gridstride<U, NC><<<sms * CPS, T>>>(buf, n, out); }); \
     printf("A gridstride U=%2d nc=%d ctas/sm=%d threads=%4d : %7.1f GB/s\n", U, NC, CPS, T, bytes / ms / 1e6); }
@@ -163,7 +165,7 @@ int main(int argc, char** argv) {
     // bulk L2 prefetch, wait, read: per-CTA max of (read time); fresh region every run (rotating through the big buffer)
     {
         unsigned long long* st; cudaMalloc(&st, sms * 4 * 8);
-        unsigned long long h[148 * 4];
+        std::vector<unsigned long long> h(sms * 4);
         int rot = 0;
         for (size_t mb : {16, 48, 96})
             for (int pf = 0; pf < 2; pf++)
@@ -175,7 +177,7 @@ int main(int argc, char** argv) {
                         const int4* base = buf + (size_t)rot * ((size_t)100 << 20) / 16;
                         k_prefetch_then_read<<<sms, 512>>>(base, bytes_r, chunk, wait_us * 1000, pf, out, st);
                         cudaDeviceSynchronize();
-                        cudaMemcpy(h, st, sizeof(h), cudaMemcpyDeviceToHost);
+                        cudaMemcpy(h.data(), st, h.size() * sizeof(h[0]), cudaMemcpyDeviceToHost);
                         unsigned long long t0 = ~0ull, tpf = 0, t2 = ~0ull, t3 = 0;
                         for (int b = 0; b < sms; b++) { if (h[b*4] < t0) t0 = h[b*4]; if (h[b*4+1] > tpf) tpf = h[b*4+1]; if (h[b*4+2] < t2) t2 = h[b*4+2]; if (h[b*4+3] > t3) t3 = h[b*4+3]; }
                         printf("D %3zu MB pf=%d chunk=%5u wait=%2u us: issue %6.2f us, read %7.2f us = %7.1f GB/s, total %7.2f us\n", mb, pf, chunk, wait_us,

@@ -1,6 +1,6 @@
 // ringbench.cu -- can a TMA-fed shared-memory ring (one producer warp, 16 consumer warps per SM: the structure of mega_ring.cu) stream
-// HBM at full speed, and with which slot size / depth / number of issuing lanes?  Developer tool (profiles/r02n_ringbench.txt).
-// Build: nvcc -O3 -gencode arch=compute_100a,code=sm_100a -o tools/build/ringbench tools/ringbench.cu
+// HBM at full speed, and with which slot size / depth / number of issuing lanes?  Developer tool.
+// Build: nvcc -O3 -gencode arch=compute_90a,code=sm_90a -o tools/build/ringbench tools/ringbench.cu
 #include <cstdio>
 #include <cstdint>
 #include <cstdlib>
@@ -49,7 +49,7 @@ __global__ void __launch_bounds__(544, 1) k_ring(const uint8_t* __restrict__ in,
                 const unsigned fb = full0 + 8u * slot, dst = ring0 + slot * (unsigned)slot_bytes;
                 const uint8_t* src = base + (size_t)e * ent_bytes;
                 expect_tx(fb, (unsigned)ent_bytes);
-                if (pattern == 1) {        // mega_ring.cu's addresses: CTA c takes the 4 KB rows c, c + 148, ... of a matrix; their 256-byte scale rows live in another plane
+                if (pattern == 1) {        // mega_ring.cu's addresses: CTA c takes the 4 KB rows c, c + gridDim.x, ... of a matrix; their 256-byte scale rows live in another plane
                     const size_t idx = (size_t)e * gridDim.x + blockIdx.x;
                     bulk_g2s(dst, in + idx * 4096, 4096u, fb);
                     bulk_g2s(dst + 4096, in + ((size_t)5 << 30) + idx * 256, 256u, fb);
@@ -101,6 +101,8 @@ int main() {
     uint8_t* in; int* out;
     cudaMalloc(&in, total); cudaMalloc(&out, 4);
     cudaMemset(in, 1, total);
+    int sms = 0;
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
     cudaFuncSetAttribute(k_ring, cudaFuncAttributeMaxDynamicSharedMemorySize, 225 * 1024);
     cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);
     struct Cfg { int ent, ring_kb, copies, lanes, work, pattern; };
@@ -110,20 +112,20 @@ int main() {
     for (const Cfg& c : cfgs) {
         const int slot_bytes = (c.ent + 127) & ~127;
         int nslots = c.ring_kb * 1024 / slot_bytes; if (nslots > MAX_SLOTS) nslots = MAX_SLOTS;
-        const size_t per_cta = (c.pattern ? ((size_t)5 << 30) : total) / 148 / 256 * 256;
+        const size_t per_cta = (c.pattern ? ((size_t)5 << 30) : total) / sms / 256 * 256;
         const int n_ent = (int)(per_cta / (c.pattern ? 4096 : c.ent));
         const size_t smem = (size_t)nslots * slot_bytes + 4608;
         float best = 1e30f;
         for (int rep = 0; rep < 3; rep++) {
             cudaEventRecord(e0);
-            k_ring<<<148, 544, smem>>>(in, per_cta, n_ent, c.ent, slot_bytes, nslots, c.copies, c.lanes, c.work, c.pattern, out);
+            k_ring<<<sms, 544, smem>>>(in, per_cta, n_ent, c.ent, slot_bytes, nslots, c.copies, c.lanes, c.work, c.pattern, out);
             cudaEventRecord(e1);
             cudaError_t err = cudaEventSynchronize(e1);
             if (err != cudaSuccess) { printf("error: %s\n", cudaGetErrorString(err)); return 1; }
             float ms; cudaEventElapsedTime(&ms, e0, e1);
             if (ms < best) best = ms;
         }
-        const double bytes = (double)n_ent * c.ent * 148;
+        const double bytes = (double)n_ent * c.ent * sms;
         printf("entry %5d B  slots %3d (%3d KB)  copies %d  lanes %2d  work %d  pattern %d : %8.1f GB/s  (%.3f ms)\n", c.ent, nslots, (int)(smem / 1024), c.copies, c.lanes, c.work, c.pattern, bytes / best / 1e6, best);
         fflush(stdout);
     }
