@@ -23,6 +23,7 @@
 #define MR_PRODUCER_WARPS 4        // 20 warps: five per SM sub-partition, still 96 registers per thread
 #define MR_THREADS (MK_THREADS + 32 * MR_PRODUCER_WARPS)
 #define MR_MAX_SLOTS 112
+#define MR_Q8_SLOTS 24             // ring depth for Q8_0 entries (cc_launch_mega_ring)
 #define MR_DESC_WORDS ((int)(sizeof(MkPhase) / 4))
 #define MR_DESC_PER_LANE ((MR_DESC_WORDS + 31) / 32)
 
@@ -665,9 +666,12 @@ int cc_launch_mega_ring(cc_device* dev, const MkPhase* phases_dev, int n_phases,
     const size_t ring_off = (wtop + smem_wstage + 127) & ~(size_t)127;
     const size_t cap = 227 * 1024 - fa.sharedSizeBytes;
     CC_REQUIRE(dev, ring_off + 4 * (size_t)slot_bytes <= cap, "megakernel: the phases leave no room for the weight ring (%zu bytes of working area)", ring_off);
-    int nslots = (int)((cap - ring_off) / (size_t)slot_bytes);
-    if (nslots > MR_MAX_SLOTS) nslots = MR_MAX_SLOTS;
-    if (const char* e = getenv("CRABML_RING_SLOTS")) { const int v = atoi(e); if (v >= 2 && v < nslots) nslots = v; }      // developer A/B
+    const int fit = std::min((int)((cap - ring_off) / (size_t)slot_bytes), MR_MAX_SLOTS);
+    // Ring depth: a Q8_0 ring (4352-byte slots) is faster SHALLOW -- 24 slots = 104 KB per SM decode a Llama-2-7B token in 3.88 ms
+    // against 4.04 ms with the ~40 that fit, and 20 / 16 / 12 slots are slower again (NVIDIA H100 80GB HBM3, 400 W).  The Q4_0 consumer is
+    // ALU-bound and keeps every slot that fits: a 55 KB ring (24 of its slots) cost it 2-4 %, 46 KB 9 %.
+    int nslots = slot_bytes >= 4352 ? std::min(fit, MR_Q8_SLOTS) : fit;
+    if (const char* e = getenv("CRABML_RING_SLOTS")) { const int v = atoi(e); if (v >= 2 && v <= fit) nslots = v; }      // developer A/B
     const size_t smem = ring_off + (size_t)nslots * slot_bytes;
     CC_CUDA(dev, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     int max_ctas_per_sm = 0;

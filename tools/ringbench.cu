@@ -1,4 +1,4 @@
-// ringbench.cu -- can a TMA-fed shared-memory ring (one producer warp, 16 consumer warps per SM: the structure of mega_ring.cu) stream
+// ringbench.cu -- can a TMA-fed shared-memory ring (up to 4 producer warps, 16 consumer warps per SM: the structure of mega_ring.cu) stream
 // HBM at full speed, and with which slot size / depth / number of issuing lanes?  Developer tool.
 // Build: nvcc -O3 -gencode arch=compute_90a,code=sm_90a -o tools/build/ringbench tools/ringbench.cu
 #include <cstdio>
@@ -25,9 +25,9 @@ __device__ __forceinline__ unsigned ld_acquire(unsigned addr) {
 }
 
 #define MAX_SLOTS 128
-// every CTA streams `n_ent` entries of `ent_bytes` (contiguous region per CTA); copies = 1: one bulk copy per entry, 2: main part + a 256-byte tail
-// (the f16 scale plane of mega_ring.cu); lanes: issuing lanes of the producer warp
-__global__ void __launch_bounds__(544, 1) k_ring(const uint8_t* __restrict__ in, size_t cta_stride, int n_ent, int ent_bytes, int slot_bytes, int nslots, int copies,
+// every CTA streams `n_ent` entries of `ent_bytes` (contiguous region per CTA); copies = 1: one bulk copy per entry, 2: main part + a tail of
+// 256 bytes per 4352 (the f16 scale plane of mega_ring.cu); lanes: issuing threads of the producer warps (threads 512 ..)
+__global__ void __launch_bounds__(640, 1) k_ring(const uint8_t* __restrict__ in, size_t cta_stride, int n_ent, int ent_bytes, int slot_bytes, int nslots, int copies,
                                                  int lanes, int work, int pattern, int* out) {
     extern __shared__ __align__(128) uint8_t smem[];
     __shared__ __align__(8) unsigned long long s_full[MAX_SLOTS];
@@ -40,9 +40,10 @@ __global__ void __launch_bounds__(544, 1) k_ring(const uint8_t* __restrict__ in,
     __syncthreads();
     const uint8_t* base = in + (size_t)blockIdx.x * cta_stride;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    if (warp == 16) {
-        if (lane >= lanes) return;
-        int j = lane;
+    if (warp >= 16) {
+        const int pt = (int)threadIdx.x - 512;
+        if (pt >= lanes) return;
+        int j = pt;
         while (j < n_ent) {
             const unsigned e = (unsigned)j, slot = e % (unsigned)nslots, use = e / (unsigned)nslots;
             if (!use || ld_acquire(done0 + 4u * slot) == e - (unsigned)nslots + 1u) {
@@ -53,7 +54,10 @@ __global__ void __launch_bounds__(544, 1) k_ring(const uint8_t* __restrict__ in,
                     const size_t idx = (size_t)e * gridDim.x + blockIdx.x;
                     bulk_g2s(dst, in + idx * 4096, 4096u, fb);
                     bulk_g2s(dst + 4096, in + ((size_t)5 << 30) + idx * 256, 256u, fb);
-                } else if (copies == 2) { bulk_g2s(dst, src, (unsigned)ent_bytes - 256u, fb); bulk_g2s(dst + ent_bytes - 256, src + ent_bytes - 256, 256u, fb); }
+                } else if (copies == 2) {
+                    const unsigned tail = (unsigned)(ent_bytes / 17) & ~15u;
+                    bulk_g2s(dst, src, (unsigned)ent_bytes - tail, fb); bulk_g2s(dst + ent_bytes - tail, src + ent_bytes - tail, tail, fb);
+                }
                 else bulk_g2s(dst, src, (unsigned)ent_bytes, fb);
                 __threadfence_block();
                 ((volatile unsigned*)s_seq)[slot] = e + 1u;
@@ -63,8 +67,9 @@ __global__ void __launch_bounds__(544, 1) k_ring(const uint8_t* __restrict__ in,
         return;
     }
     int acc = 0;
-    // work 1 / 2: the arithmetic of mega_ring.cu's consumer on a 4352-byte entry (8 weight LDS.128 + 4 scales, 8 activation LDS.128, 32 dp4a,
-    // f32 scale-accumulate); activation layout 1 = block-major (lane stride 32 B: 2-way bank conflicts), 2 = half-split (conflict-free)
+    // work 1 / 2: the arithmetic of mega_ring.cu's consumer on every 4352 bytes of an entry (8 weight LDS.128 + 4 scales, 8 activation LDS.128,
+    // 32 dp4a, f32 scale-accumulate; an entry of R such rows holds R x 4096 B of quants, then R x 256 B of scales); activation layout
+    // 1 = block-major (lane stride 32 B: 2-way bank conflicts), 2 = half-split (conflict-free)
     uint8_t* act = smem + (size_t)nslots * slot_bytes;         // 4096 B quants + 512 B scales
     if (work) { for (int i = threadIdx.x; i < 4608 / 4; i += 512) ((int*)act)[i] = i * 2654435761u; asm volatile("bar.sync 1, 512;" ::: "memory"); }
     float facc = 0.0f;
@@ -74,18 +79,21 @@ __global__ void __launch_bounds__(544, 1) k_ring(const uint8_t* __restrict__ in,
         const int4* sp = (const int4*)(smem + (size_t)slot * slot_bytes);
         if (!work) { for (int i = lane; i < ent_bytes / 16; i += 32) { const int4 v = sp[i]; acc += v.x ^ v.y ^ v.z ^ v.w; } }
         else {
-            const uint8_t* q = (const uint8_t*)sp + lane * 16;
-            const uint16_t* d = (const uint16_t*)((const uint8_t*)sp + 4096) + lane;
+            const int rows = ent_bytes / 4352 > 0 ? ent_bytes / 4352 : 1;
             const float* ad = (const float*)(act + 4096) + lane;
             float part = 0.0f;
+            for (int r = 0; r < rows; r++) {
+                const uint8_t* q = (const uint8_t*)sp + r * 4096 + lane * 16;
+                const uint16_t* d = (const uint16_t*)((const uint8_t*)sp + rows * 4096 + r * 256) + lane;
 #pragma unroll
-            for (int g = 0; g < 4; g++) {
-                const int4 wa = *(const int4*)(q + g * 1024), wb = *(const int4*)(q + g * 1024 + 512);
-                int4 aa, ab;
-                if (work == 1) { aa = *(const int4*)(act + g * 1024 + lane * 32); ab = *(const int4*)(act + g * 1024 + lane * 32 + 16); }
-                else { aa = *(const int4*)(act + g * 1024 + lane * 16); ab = *(const int4*)(act + g * 1024 + 512 + lane * 16); }
-                int si = __dp4a(wa.x, aa.x, __dp4a(wa.y, aa.y, __dp4a(wa.z, aa.z, __dp4a(wa.w, aa.w, 0)))) + __dp4a(wb.x, ab.x, __dp4a(wb.y, ab.y, __dp4a(wb.z, ab.z, __dp4a(wb.w, ab.w, 0))));
-                part += (float)si * __half2float(__ushort_as_half(d[g * 32])) * ad[g * 32];
+                for (int g = 0; g < 4; g++) {
+                    const int4 wa = *(const int4*)(q + g * 1024), wb = *(const int4*)(q + g * 1024 + 512);
+                    int4 aa, ab;
+                    if (work == 1) { aa = *(const int4*)(act + g * 1024 + lane * 32); ab = *(const int4*)(act + g * 1024 + lane * 32 + 16); }
+                    else { aa = *(const int4*)(act + g * 1024 + lane * 16); ab = *(const int4*)(act + g * 1024 + 512 + lane * 16); }
+                    int si = __dp4a(wa.x, aa.x, __dp4a(wa.y, aa.y, __dp4a(wa.z, aa.z, __dp4a(wa.w, aa.w, 0)))) + __dp4a(wb.x, ab.x, __dp4a(wb.y, ab.y, __dp4a(wb.z, ab.z, __dp4a(wb.w, ab.w, 0))));
+                    part += (float)si * __half2float(__ushort_as_half(d[g * 32])) * ad[g * 32];
+                }
             }
             facc += part;
             acc += __float_as_int(part) & 1;
@@ -105,9 +113,18 @@ int main() {
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
     cudaFuncSetAttribute(k_ring, cudaFuncAttributeMaxDynamicSharedMemorySize, 225 * 1024);
     cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);
+    // ring_kb: ring bytes in KB (slots = ring_kb * 1024 / slot size); lanes 128 = 4 producer warps (mega_ring.cu), 32 = one
     struct Cfg { int ent, ring_kb, copies, lanes, work, pattern; };
     const Cfg cfgs[] = {
-        {4352, 160, 2, 32, 2, 0}, {4352, 160, 2, 32, 2, 1}, {4352, 160, 2, 32, 0, 1}, {4352, 160, 2, 8, 2, 1}, {4352, 120, 2, 32, 2, 1}, {4352, 80, 2, 32, 2, 1}, {4352, 160, 2, 32, 2, 0},
+        // the ring kernel today: 4352-byte Q8_0 entries (4096 B quants + 256 B scales, two copies), ~40 slots, 4 producer warps
+        {4352, 174, 2, 128, 2, 1}, {4352, 174, 2, 128, 2, 0}, {4352, 174, 2, 128, 0, 0}, {4352, 174, 2, 32, 2, 0},
+        // one copy per entry: 4.3, 8.7 and 17 KB, at ~174 KB and ~200 KB of ring
+        {4352, 174, 1, 128, 2, 0}, {8704, 174, 1, 128, 2, 0}, {17408, 174, 1, 128, 2, 0},
+        {4352, 200, 1, 128, 2, 0}, {8704, 204, 1, 128, 2, 0}, {17408, 204, 1, 128, 2, 0},
+        // two copies per entry (quants + scales) at 8.7 / 17 KB: a row pair / quad in one slot
+        {8704, 174, 2, 128, 2, 0}, {8704, 204, 2, 128, 2, 0}, {17408, 204, 2, 128, 2, 0}, {8704, 204, 2, 64, 2, 0}, {8704, 204, 2, 32, 2, 0},
+        // Q4_0 entries (2048 B quants + 256 B scales per row): 1, 2 and 4 rows per slot, two copies, read only
+        {2304, 174, 2, 128, 0, 0}, {4608, 174, 2, 128, 0, 0}, {4608, 204, 2, 128, 0, 0}, {9216, 204, 2, 128, 0, 0},
     };
     for (const Cfg& c : cfgs) {
         const int slot_bytes = (c.ent + 127) & ~127;
@@ -118,7 +135,7 @@ int main() {
         float best = 1e30f;
         for (int rep = 0; rep < 3; rep++) {
             cudaEventRecord(e0);
-            k_ring<<<sms, 544, smem>>>(in, per_cta, n_ent, c.ent, slot_bytes, nslots, c.copies, c.lanes, c.work, c.pattern, out);
+            k_ring<<<sms, 640, smem>>>(in, per_cta, n_ent, c.ent, slot_bytes, nslots, c.copies, c.lanes, c.work, c.pattern, out);
             cudaEventRecord(e1);
             cudaError_t err = cudaEventSynchronize(e1);
             if (err != cudaSuccess) { printf("error: %s\n", cudaGetErrorString(err)); return 1; }
@@ -126,7 +143,7 @@ int main() {
             if (ms < best) best = ms;
         }
         const double bytes = (double)n_ent * c.ent * sms;
-        printf("entry %5d B  slots %3d (%3d KB)  copies %d  lanes %2d  work %d  pattern %d : %8.1f GB/s  (%.3f ms)\n", c.ent, nslots, (int)(smem / 1024), c.copies, c.lanes, c.work, c.pattern, bytes / best / 1e6, best);
+        printf("entry %5d B  slots %3d (%3d KB)  copies %d  lanes %3d  work %d  pattern %d : %8.1f GB/s  (%.3f ms)\n", c.ent, nslots, (int)(smem / 1024), c.copies, c.lanes, c.work, c.pattern, bytes / best / 1e6, best);
         fflush(stdout);
     }
     return 0;
