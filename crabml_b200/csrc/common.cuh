@@ -302,6 +302,7 @@ int cc_launch_mega_ring(cc_device* dev, const MkPhase* phases_dev, int n_phases,
 int cc_check_async_error(cc_device* dev);     // after a stream synchronize: did a persistent kernel give up on a barrier?
 int cc_launch_normq(cc_device* dev, float* x, float* orig, const float* norm_w, float eps, int64_t n, void* act_scratch, bool write_back);
 int cc_launch_attn_decode(cc_device* dev, const AttnArgs& a);
+bool cc_attn_decode_fits(int64_t hd, int64_t max_len);      // can the single-pass attention kernel hold the score row of this cache?
 struct LazyState;
 LazyState* cc_lazy_create(cc_device* dev);
 void cc_lazy_destroy(cc_device* dev);

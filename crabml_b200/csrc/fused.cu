@@ -224,9 +224,14 @@ int cc_launch_normq(cc_device* dev, float* x, float* orig, const float* norm_w, 
     return CC_OK;
 }
 
+// q, k, v of the head and the whole score row live in shared memory: max_len <= 50 808 positions at head_dim 128
+#define AT_SMEM_MAX (200 * 1024)
+static size_t attn_decode_smem(int64_t hd, int64_t max_len) { return (size_t)(3 * hd + max_len + 8) * sizeof(float); }
+bool cc_attn_decode_fits(int64_t hd, int64_t max_len) { return attn_decode_smem(hd, max_len) <= AT_SMEM_MAX; }
+
 int cc_launch_attn_decode(cc_device* dev, const AttnArgs& a) {
-    size_t smem = (size_t)(3 * a.hd + a.max_len + 8) * sizeof(float);
-    CC_REQUIRE(dev, smem <= 200 * 1024, "attention: context %d too long for the single-pass kernel", a.max_len);
+    const size_t smem = attn_decode_smem(a.hd, a.max_len);
+    CC_REQUIRE(dev, smem <= AT_SMEM_MAX, "attention: context %d too long for the single-pass kernel", a.max_len);
     ActQ8_0 act = cc_act_q8_0(a.act_scratch, (int64_t)a.n_heads * a.hd);
     if (!a.act_scratch) act.qs = nullptr;
     cudaError_t e;

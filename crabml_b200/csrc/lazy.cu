@@ -387,6 +387,8 @@ struct Fuser {
         if (ct.a.buf != qb || sc.a.buf != ct.out || b1.a.buf != ct.out || b1.b.buf != kc || sm.a.buf != b1.out || b2.a.buf != b1.out || b2.b.buf != vc) return 0;
         if (b1.b.shape[2] != kv_len + 1 || b1.b.strides[1] != 1 || b2.b.shape[1] != kv_len + 1 || b2.b.strides[2] != 1) return 0;
         if (kv_len + 1 > seq_stride / hd) return 0;
+        // a cache longer than the single-pass kernel's score row (50 808 positions at head_dim 128): the ops run as their eager kernels
+        if (!cc_attn_decode_fits(hd, seq_stride / hd)) return 0;
         // intermediates must not be observable afterwards
         if (!dead_after(ct.out, i + 9) || !dead_after(b1.out, i + 9) || !dead_after(qb, i + 9) || !dead_after(kb, i + 9) || !dead_after(vb, i + 9)) return 0;
         const int64_t pos = rq.i0, rope_dim = rq.rows[0];
@@ -661,7 +663,11 @@ int cc_lazy_flush(cc_device* dev) {
             cudaGraph_t graph = nullptr;
             GraphEntry ge;
             bool use_mega = dev->mega && P.mega_ok && !P.phases.empty();
-            if (use_mega) {       // a phase whose working area cannot fit beside anything (e.g. the score row of a 32 K-token context): CUDA-graph mode
+            // a phase whose working area cannot fit beside anything: CUDA-graph mode.  The register kernel's attention area (three 64-row
+            // chunk buffers + the score row) decides this for both persistent kernels: at head_dim 128, max_len 32 105 and up, and 28 009
+            // and up beside a Llama-2-7B norm + qkv phase (its 16 KB of norm weights are staged too).  Past 50 808 positions the fuser
+            // leaves attention to the per-op kernels (try_attention).
+            if (use_mega) {
                 size_t work = 0, wst = 0;
                 for (auto& ph : P.phases) {
                     work = std::max(work, cc_mega_smem_for_phase(ph));

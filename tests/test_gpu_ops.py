@@ -86,13 +86,30 @@ def test_softmax_silu_kats(gdev):
     np.testing.assert_allclose(t.to_vec(), [0.7310586, 1.761594, 2.8577225, 3.928055, 4.9665356, 5.9851646], rtol=2e-3)
 
 
-@pytest.mark.parametrize("shape", [[32, 1, 1], [6, 1, 37], [32, 1, 257], [4, 3, 2048], [8, 100]])
+@pytest.mark.parametrize("shape", [[32, 1, 1], [6, 1, 37], [32, 1, 257], [4, 3, 2048], [8, 100], [3, 1, 4097]])
 def test_softmax_vs_oracle(gdev, odev, shape):
     rng = np.random.default_rng(6)
     g, o = both(rng.standard_normal(int(np.prod(shape))) * 4, shape, gdev, odev)
     ax = len(shape) - 1
     # identical LUT exps; only the order of the f32 sum differs (tree vs sequential)
     np.testing.assert_allclose(g.softmax_inplace(ax).export(), o.softmax_inplace(ax).export(), rtol=5e-6, atol=0)
+
+
+def test_softmax_long_rows_vs_f64_and_oracle(gdev, odev):
+    """Rows of 40 001.  The exps are the same LUT values on both sides, so the f32 sum alone differs.  The oracle sums sequentially (the
+    reference's order, softmax.rs:39-54), which drifts by about 5e-5 relative at this length; the kernel's 512-thread tree stays within
+    5e-6 of the f64 sum of the same exps.  So the kernel is held to 5e-6 of that f64 normalisation, and to the oracle within 5e-6 plus the
+    oracle's own distance from it."""
+    rng = np.random.default_rng(6)
+    x = (rng.standard_normal(2 * 40001) * 4).astype(np.float32)
+    g, o = both(x, [2, 40001], gdev, odev)
+    got, want_o = g.softmax_inplace(1).export().reshape(2, -1), o.softmax_inplace(1).export().reshape(2, -1)
+    rows = x.reshape(2, -1)
+    e = oc.f16_to_f32(oc.exp_lut()[oc.f32_to_f16(rows - rows.max(axis=1, keepdims=True)).astype(np.int64)]).astype(np.float64)
+    want = e / e.sum(axis=1, keepdims=True)
+    np.testing.assert_allclose(got, want, rtol=5e-6, atol=0)
+    drift = float(np.abs(want_o / np.where(want > 0, want, 1) - 1)[want > 0].max())
+    np.testing.assert_allclose(got, want_o, rtol=5e-6 + drift, atol=0)
 
 
 def test_silu_gelu_bit_exact(gdev, odev):
@@ -175,7 +192,8 @@ def test_concatenate_kv_cache(gdev, odev, kv_dtype):
 
 
 @pytest.mark.parametrize("kv_dtype", [oc.F32, oc.F16])
-@pytest.mark.parametrize("heads,kv_heads,hd,seq", [(6, 6, 48, 1), (6, 6, 48, 17), (32, 32, 128, 100), (8, 4, 16, 33), (32, 8, 128, 64)])
+@pytest.mark.parametrize("heads,kv_heads,hd,seq", [(6, 6, 48, 1), (6, 6, 48, 17), (32, 32, 128, 100), (8, 4, 16, 33), (32, 8, 128, 64),
+                                                    (32, 32, 128, 1000), (32, 8, 128, 1000), (32, 32, 128, 4096), (32, 8, 128, 4096)])
 def test_batch_matmul_attention_shapes(gdev, odev, kv_dtype, heads, kv_heads, hd, seq):
     """QK^T (B = K cache transposed, stride_k == 1) and PV (B = V cache, stride_n == 1), incl. the
     GQA head mapping: bi % bb for F32 caches (batch_matmul.rs:63), bi / (ab/bb) for F16 (:89-91)."""

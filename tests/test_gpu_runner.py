@@ -208,22 +208,56 @@ def test_both_persistent_kernels_bit_identical_on_7b_shapes(tmp_path, wt, ct):
 @pytest.mark.parametrize("f16_kv", [False, True])
 def test_execution_modes_bit_identical_on_fixture(fixture_path, fname, f16_kv):
     """eager / CUDA-graph / megakernel on the reference's own GGUF fixtures (head_dim 48: unquantised attention output path,
-    rows of 288 and 768: ragged last group), 24 positions so the softmax spans more than one warp."""
+    rows of 288 and 768: ragged last group), 250 positions: the megakernel's attention phase streams up to 8 chunks of 32 (f32) or 4 of
+    64 (f16) cache rows per head through its 3 buffers, so every buffer is refilled many times."""
     from crabml_b200 import runner as R
     path = fixture_path(fname)
-    seq = (PROMPT_IDS + CASES[0][2])[:21] + [5, 6, 7]
+    seq = (PROMPT_IDS + CASES[0][2])[:21] + [5, 6, 7] + [int(t) for t in np.random.default_rng(3).integers(1, 32000, 226)]
     res = {}
     for lazy in (0, 1, 2):
         dev = make_device(lazy=lazy)
         try:
             conf, w, _ = R.load_gguf(path, dev)
-            r = R.LlamaRunner(dev, conf, w, 64, f16_kv=f16_kv)
+            r = R.LlamaRunner(dev, conf, w, 256, f16_kv=f16_kv)
             res[lazy] = np.stack([r.forward([t], p).copy() for p, t in enumerate(seq)])
+            if lazy == 2:
+                assert dev.mega_variant() == 2, "expected the ring kernel"
             r.close()
         finally:
             dev.close()
     for mode in (1, 2):
         np.testing.assert_array_equal(res[mode].view(np.uint32), res[0].view(np.uint32), err_msg=f"lazy={mode} vs eager")
+
+
+@pytest.mark.parametrize("n_kv,hidden", [(32, 11008), (8, 14336)], ids=["llama2-7b", "mistral-7b"])
+def test_execution_modes_bit_identical_over_200_positions_on_7b_shapes(n_kv, hidden):
+    """One Q8_0 layer of Llama-2-7B (and of Mistral-7B: 8 kv heads) decoding positions 0-199: this covers bench.py's window (positions
+    36-68) and many refills of the megakernel's three attention buffers.  Eager kernels, CUDA graph and ring megakernel logits are
+    bit-identical at positions around every chunk boundary (logits are not exported elsewhere, to keep the run short)."""
+    from crabml_b200 import runner as R
+    conf = R.LlamaConfig(32, n_kv, 1, 4096, hidden, 256, 32000, 1e-5, 128)
+    toks = [int(t) for t in np.random.default_rng(11).integers(1, 32000, 200)]
+    check = [0, 1, 31, 32, 33, 36, 50, 63, 64, 65, 68, 95, 96, 97, 127, 128, 129, 191, 192, 193, 199]
+    res = {}
+    for lazy in (0, 1, 2):
+        dev = make_device(lazy=lazy)
+        try:
+            w = R.synthetic_weights(dev, conf, oc.Q8_0, oc.Q8_0, seed=0x7B)
+            r = R.LlamaRunner(dev, conf, w, 256)
+            res[lazy] = {}
+            for p, t in enumerate(toks):
+                lg = r.forward([t], p, export=p in check)
+                if p in check:
+                    res[lazy][p] = lg.copy()
+            if lazy == 2:
+                assert dev.mega_variant() == 2, "expected the ring kernel"
+            r.close()
+        finally:
+            dev.close()
+    for p in check:
+        assert np.isfinite(res[0][p]).all() and np.abs(res[0][p]).max() > 1e-3
+        for mode in (1, 2):
+            np.testing.assert_array_equal(res[mode][p].view(np.uint32), res[0][p].view(np.uint32), err_msg=f"lazy={mode} vs eager, pos {p}")
 
 
 @pytest.mark.parametrize("mode", [0, 1, 2])
