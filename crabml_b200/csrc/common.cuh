@@ -216,7 +216,7 @@ int cc_launch_matvec(cc_device* dev, const cc_buf* w, const void* act_scratch, c
 
 // ---- prefill_gemm.cu: batched matmul_vec on the tensor cores (TMA + wgmma, f16 operand tiles, f32 register accumulator) ----
 bool cc_prefill_supported(int wtype, int64_t m, int64_t k, int64_t b);
-int cc_launch_prefill_matmul(cc_device* dev, const cc_buf* w, const void* act, const float* x_f32, float* out, int64_t m, int64_t k, int64_t b);
+int cc_launch_prefill_matmul(cc_device* dev, const cc_buf* w, const void* act_q8_k, const float* x_f32, float* out, int64_t m, int64_t k, int64_t b);
 void cc_prefill_release(cc_device* dev);
 
 // ---- ops.cu --------------------------------------------------------------------------------------

@@ -5,9 +5,12 @@
 //   1. dequant_w_f16_kernel : GGUF quant blocks (device plane layout, any of the 11 weight types) -> f16 tile source [m][k], ONCE per
 //      weight (kept beside the quantised planes: a 7B model's 13-14 GB of f16 fit in 80 GB of HBM next to its quantised weights)
 //      (w = f32 dequantised value as BlockQ*::dequantize gives it, rounded once to f16: |q| <= 127 times an f16 scale)
-//   2. act_q8_to_f16_kernel : the activation is quantised to Q8_0 exactly like the decode path (buf_q8_0.rs:87-134) and the
-//      quantised value q * d is what enters the GEMM, so the only deviation from the reference is the f16 rounding of the two
-//      operands (relative 2^-11 each) and the f32 accumulation order
+//   2. act_f32_to_q8f16_kernel / act_q8k_to_f16_kernel : the activation is quantised exactly like the decode path, to Q8_0
+//      (buf_q8_0.rs:87-134) or, for K-quant weights, to Q8_K (buf_q8_k.rs:84-131), and the quantised value q * d is what enters the
+//      GEMM, so the only deviation from the reference is the f16 rounding of the two operands (relative 2^-11 each) and the f32
+//      accumulation order.  A row whose largest |q * d| reaches 2^15 would overflow f16 (127 * f16(65504 / 127) rounds to +inf);
+//      it enters scaled by a power of two 2^-e (the smallest e that brings it below 2^15), and the epilogue multiplies its outputs
+//      by 2^e.  Rows in range have e = 0: the multiply by 1.0f is exact and changes no bit
 //   3. wgmma_gemm_kernel    : TMA (cp.async.bulk.tensor.2d, 128-byte swizzle) stages [128 x 64] / [N x 64] f16 tiles into a
 //      4-deep shared-memory ring; two consumer warpgroups each own 64 weight rows and issue
 //      wgmma.mma_async.m64n64k16.f32.f16.f16 (N / 64 per 16-wide K step) with the f32 accumulator in registers, then store
@@ -76,9 +79,10 @@ struct PgShared {
 
 // grid: (ceil(m / 128), ceil(b / BLOCK_N)); dynamic smem: 1024-aligned ring of PG_STAGES x (A tile 16 KB + B tile BLOCK_N * 128 B),
 // at most 4 x 48 KB.  The accumulator of a consumer warpgroup is BLOCK_N / 2 registers per thread (128 at BLOCK_N = 256).
+// row_scale[b]: 2^e of each activation row (the inverse of the scale its f16 operand was taken at; 1.0 for rows in f16 range).
 template <int BLOCK_N>
 __global__ void __launch_bounds__(PG_THREADS, 1) wgmma_gemm_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant__ CUtensorMap tmap_x,
-                                                                   float* __restrict__ C, int m, int b, int k) {
+                                                                   const float* __restrict__ row_scale, float* __restrict__ C, int m, int b, int k) {
     extern __shared__ __align__(1024) uint8_t pg_smem_raw[];
     __shared__ PgShared sh;
     const int wg = threadIdx.x >> 7, t = threadIdx.x & 127;
@@ -147,7 +151,7 @@ __global__ void __launch_bounds__(PG_THREADS, 1) wgmma_gemm_kernel(const __grid_
 #pragma unroll
         for (int i = 0; i < 32; i++) {
             const int row = r0 + 8 * ((i >> 1) & 1), bi = n0 + 64 * j + 8 * (i >> 2) + 2 * (t & 3) + (i & 1);
-            if (row < m && bi < b) C[(size_t)bi * m + row] = acc[j][i];
+            if (row < m && bi < b) C[(size_t)bi * m + row] = acc[j][i] * row_scale[bi];
         }
 }
 
@@ -162,34 +166,92 @@ __global__ void dequant_w_f16_kernel(int dtype, DeqPlanes planes, int64_t nelems
     else { a = dequant_elem(dtype, planes, i); b2 = dequant_elem(dtype, planes, i + 1); }
     *(__half2*)(out + i) = __halves2half2(__float2half_rn(a), __float2half_rn(b2));
 }
-// activation: Q8_0 SoA (qs, f32(f16 d)) -> f16(q * d) [b][k]
-__global__ void act_q8_to_f16_kernel(ActQ8_0 act, int64_t nelems, __half* __restrict__ out) {
-    const int64_t i = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) * 2;
-    if (i >= nelems) return;
-    const float d = act.d[i >> 5];
-    *(__half2*)(out + i) = __halves2half2(__float2half_rn((float)act.qs[i] * d), __float2half_rn((float)act.qs[i + 1] * d));
+// Activation rows -> f16 GEMM operand, one CTA of PG_ACT_THREADS per batch row.  The row is converted as if in f16 range and its
+// largest |q * d| is reduced on the way; only a row at or above 2^15 is converted a second time, at 2^-e (pg_row_exp), so an in-range
+// row is read once, as before.  row_scale[row] = 2^e undoes the scale in the GEMM's epilogue.
+#define PG_ACT_THREADS 256
+// the smallest e >= 0 with amax * 2^-e < 2^15 (amax = f * 2^x, f in [0.5, 1): e = x - 15); 0 for non-finite amax, which no scale helps
+__device__ __forceinline__ int pg_row_exp(float amax) {
+    int x = 0;
+    if (amax >= 32768.0f && amax <= 3.402823466e38f) { frexpf(amax, &x); x -= 15; }
+    return x;
+}
+__device__ __forceinline__ float pg_cta_max(float v) {
+    __shared__ float red[PG_ACT_THREADS / 32];
+    v = warp_max(v);
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+    __syncthreads();
+    v = red[0];
+#pragma unroll
+    for (int i = 1; i < PG_ACT_THREADS / 32; i++) v = fmaxf(v, red[i]);
+    return v;
+}
+__device__ __forceinline__ uint2 pg_pack4_f16(float a0, float a1, float a2, float a3, float s) {
+    __half2 h0 = __halves2half2(__float2half_rn(a0 * s), __float2half_rn(a1 * s)), h1 = __halves2half2(__float2half_rn(a2 * s), __float2half_rn(a3 * s));
+    return make_uint2(*(unsigned*)&h0, *(unsigned*)&h1);
 }
 
-// activation of the K-quant weights: Q8_K SoA (qs, f32 d per 256) -> f16(q * d) [b][k]   (buf_q8_k.rs:84-131)
-__global__ void act_q8k_to_f16_kernel(ActQ8_K act, int64_t nelems, __half* __restrict__ out) {
-    const int64_t i = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) * 2;
-    if (i >= nelems) return;
-    const float d = act.d[i >> 8];
-    *(__half2*)(out + i) = __halves2half2(__float2half_rn((float)act.qs[i] * d), __float2half_rn((float)act.qs[i + 1] * d));
-}
-
-// f32 activation rows -> f16(q * d) in ONE pass (what quantize_q8_0_kernel + act_q8_to_f16_kernel produce together, same arithmetic:
-// d = max|x| / 127, q = trunc(x / d), stored scale f32(f16(d)); buf_q8_0.rs:87-134): one warp per 32-element block
-__global__ void act_f32_to_q8f16_kernel(const float* __restrict__ x, int64_t nblocks, __half* __restrict__ out) {
-    const int64_t b = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-    const int lane = threadIdx.x & 31;
-    if (b >= nblocks) return;
-    const float v = x[b * 32 + lane];
-    const float amax = warp_max(fabsf(v));
+// Q8_0 partners: f32 activation rows -> f16(q * d), quantised on the way (what quantize_q8_0_kernel computes, same arithmetic:
+// d = max|x| / 127, q = trunc(x / d), stored scale f32(f16(d)); buf_q8_0.rs:87-134).  A lane takes 4 elements, 8 lanes one 32-element
+// block.  k % 64 == 0, so the bound check is uniform across each 8-lane group.
+__device__ __forceinline__ void pg_q8_0_4(const float4* __restrict__ xr, int i, bool ok, float (&a)[4]) {
+    const float4 v = ok ? xr[i] : make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+    float amax = fmaxf(fmaxf(fabsf(v.x), fabsf(v.y)), fmaxf(fabsf(v.z), fabsf(v.w)));
+#pragma unroll
+    for (int o = 1; o < 8; o <<= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
     const float d = amax / 127.0f;
-    const int q = __float2int_rz(v / d);                       // NaN (0 / 0) -> 0
     const float d16 = __half2float(__float2half_rn(d));
-    out[b * 32 + lane] = __float2half_rn((float)(int)(int8_t)q * d16);
+    const float vv[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+    for (int j = 0; j < 4; j++) a[j] = (float)(int)(int8_t)__float2int_rz(vv[j] / d) * d16;        // NaN (0 / 0) -> 0
+}
+__global__ void __launch_bounds__(PG_ACT_THREADS) act_f32_to_q8f16_kernel(const float* __restrict__ x, int k, __half* __restrict__ out, float* __restrict__ row_scale) {
+    const int n4 = k / 4, lane = threadIdx.x & 31, w0 = (threadIdx.x >> 5) * 32;
+    const float4* xr = (const float4*)(x + (size_t)blockIdx.x * k);
+    uint2* orow = (uint2*)(out + (size_t)blockIdx.x * k);
+    float vmax = 0.0f;
+    for (int base = w0; base < n4; base += PG_ACT_THREADS) {
+        const int i = base + lane;
+        float a[4];
+        pg_q8_0_4(xr, i, i < n4, a);
+        if (i < n4) orow[i] = pg_pack4_f16(a[0], a[1], a[2], a[3], 1.0f);
+        vmax = fmaxf(vmax, fmaxf(fmaxf(fabsf(a[0]), fabsf(a[1])), fmaxf(fabsf(a[2]), fabsf(a[3]))));
+    }
+    const int e = pg_row_exp(pg_cta_max(vmax));
+    if (threadIdx.x == 0) row_scale[blockIdx.x] = ldexpf(1.0f, e);
+    if (e == 0) return;
+    const float s = ldexpf(1.0f, -e);
+    for (int base = w0; base < n4; base += PG_ACT_THREADS) {
+        const int i = base + lane;
+        float a[4];
+        pg_q8_0_4(xr, i, i < n4, a);
+        if (i < n4) orow[i] = pg_pack4_f16(a[0], a[1], a[2], a[3], s);
+    }
+}
+
+// K-quant partners: Q8_K SoA (qs, f32 d per 256; buf_q8_k.rs:84-131) -> f16(q * d); a thread takes 4 quants per step
+__global__ void __launch_bounds__(PG_ACT_THREADS) act_q8k_to_f16_kernel(ActQ8_K act, int k, __half* __restrict__ out, float* __restrict__ row_scale) {
+    const int n4 = k / 4;
+    const char4* qr = (const char4*)(act.qs + (size_t)blockIdx.x * k);
+    const float* dr = act.d + (size_t)blockIdx.x * (k / 256);
+    uint2* orow = (uint2*)(out + (size_t)blockIdx.x * k);
+    float vmax = 0.0f;
+    for (int i = threadIdx.x; i < n4; i += PG_ACT_THREADS) {
+        const char4 q = qr[i];
+        const float d = dr[i >> 6];
+        const float a0 = (float)q.x * d, a1 = (float)q.y * d, a2 = (float)q.z * d, a3 = (float)q.w * d;
+        orow[i] = pg_pack4_f16(a0, a1, a2, a3, 1.0f);
+        vmax = fmaxf(vmax, fmaxf(fmaxf(fabsf(a0), fabsf(a1)), fmaxf(fabsf(a2), fabsf(a3))));
+    }
+    const int e = pg_row_exp(pg_cta_max(vmax));
+    if (threadIdx.x == 0) row_scale[blockIdx.x] = ldexpf(1.0f, e);
+    if (e == 0) return;
+    const float s = ldexpf(1.0f, -e);
+    for (int i = threadIdx.x; i < n4; i += PG_ACT_THREADS) {
+        const char4 q = qr[i];
+        const float d = dr[i >> 6];
+        orow[i] = pg_pack4_f16((float)q.x * d, (float)q.y * d, (float)q.z * d, (float)q.w * d, s);
+    }
 }
 
 // ---- host side ------------------------------------------------------------------------------------------------------------------------
@@ -248,11 +310,11 @@ bool cc_prefill_supported(int wtype, int64_t m, int64_t k, int64_t b) {
 }
 
 template <int BLOCK_N>
-static int pg_launch(cc_device* dev, const CUtensorMap& tw, const CUtensorMap& tx, float* out, int64_t m, int64_t b, int64_t k) {
+static int pg_launch(cc_device* dev, const CUtensorMap& tw, const CUtensorMap& tx, const float* row_scale, float* out, int64_t m, int64_t b, int64_t k) {
     const size_t smem = (size_t)PG_STAGES * ((size_t)PG_BLOCK_M * PG_BLOCK_K * 2 + (size_t)BLOCK_N * PG_BLOCK_K * 2) + 1024;
     CC_CUDA(dev, cudaFuncSetAttribute(wgmma_gemm_kernel<BLOCK_N>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     dim3 grid((unsigned)((m + PG_BLOCK_M - 1) / PG_BLOCK_M), (unsigned)((b + BLOCK_N - 1) / BLOCK_N));
-    wgmma_gemm_kernel<BLOCK_N><<<grid, PG_THREADS, smem, dev->stream>>>(tw, tx, out, (int)m, (int)b, (int)k);
+    wgmma_gemm_kernel<BLOCK_N><<<grid, PG_THREADS, smem, dev->stream>>>(tw, tx, row_scale, out, (int)m, (int)b, (int)k);
     CC_LAUNCH_CHECK(dev);
     return CC_OK;
 }
@@ -279,29 +341,29 @@ static int pg_weight_f16(cc_device* dev, const cc_buf* w, int64_t m, int64_t k, 
     return CC_OK;
 }
 
-// act: the quantisation of the (b, k) activation to the weight's partner type, Q8_0 or Q8_K (quantize.cu layout) -- or, for Q8_0
-// partners, x_f32: the f32 activation itself, quantised on the way to f16 (the caller then skips its own quantise launch); out: f32 [b][m]
-int cc_launch_prefill_matmul(cc_device* dev, const cc_buf* w, const void* act_q8_0, const float* x_f32, float* out, int64_t m, int64_t k, int64_t b) {
+// act_q8_k: for K-quant weights, the (b, k) activation quantised to Q8_K (quantize.cu layout); x_f32: for Q8_0 partners, the f32
+// activation itself, quantised on the way to f16 (the caller skips its own quantise launch); out: f32 [b][m]
+int cc_launch_prefill_matmul(cc_device* dev, const cc_buf* w, const void* act_q8_k, const float* x_f32, float* out, int64_t m, int64_t k, int64_t b) {
+    const int at = cc_partner_type(w->dtype);
+    if (at == CC_Q8_0 && !x_f32) return cc_fail(dev, CC_ERR_ARG, "prefill: a Q8_0-partner weight needs the f32 activation");
     PgScratch* s = pg_scratch(dev);
     const void* wf16 = nullptr;
     int rc = pg_weight_f16(dev, w, m, k, s, &wf16);
     if (rc) return rc;
-    rc = pg_ensure(dev, &s->x, &s->x_bytes, (size_t)b * k * 2);
+    // x scratch: the f16 operand [b][k], then the f32 row scales [b] (b * k * 2 is a multiple of 128 bytes)
+    rc = pg_ensure(dev, &s->x, &s->x_bytes, (size_t)b * k * 2 + (size_t)b * 4);
     if (rc) return rc;
-    {
-        const int64_t na = b * k;
-        if (cc_partner_type(w->dtype) == CC_Q8_K) act_q8k_to_f16_kernel<<<(unsigned)((na / 2 + 255) / 256), 256, 0, dev->stream>>>(cc_act_q8_k((void*)act_q8_0, na), na, (__half*)s->x);
-        else if (x_f32) act_f32_to_q8f16_kernel<<<(unsigned)((na / 32 + 7) / 8), 256, 0, dev->stream>>>(x_f32, na / 32, (__half*)s->x);      // quantise + f16 in one pass
-        else act_q8_to_f16_kernel<<<(unsigned)((na / 2 + 255) / 256), 256, 0, dev->stream>>>(cc_act_q8_0((void*)act_q8_0, na), na, (__half*)s->x);
-        CC_LAUNCH_CHECK(dev);
-    }
+    float* row_scale = (float*)((uint8_t*)s->x + (size_t)b * k * 2);
+    if (at == CC_Q8_K) act_q8k_to_f16_kernel<<<(unsigned)b, PG_ACT_THREADS, 0, dev->stream>>>(cc_act_q8_k((void*)act_q8_k, b * k), (int)k, (__half*)s->x, row_scale);
+    else act_f32_to_q8f16_kernel<<<(unsigned)b, PG_ACT_THREADS, 0, dev->stream>>>(x_f32, (int)k, (__half*)s->x, row_scale);
+    CC_LAUNCH_CHECK(dev);
     const int block_n = b >= 192 ? 256 : b >= 96 ? 128 : 64;
     CUtensorMap tw, tx;
     rc = pg_make_tmap(dev, &tw, wf16, m, k, PG_BLOCK_M);
     if (rc) return rc;
     rc = pg_make_tmap(dev, &tx, s->x, b, k, block_n);
     if (rc) return rc;
-    if (block_n == 256) return pg_launch<256>(dev, tw, tx, out, m, b, k);
-    if (block_n == 128) return pg_launch<128>(dev, tw, tx, out, m, b, k);
-    return pg_launch<64>(dev, tw, tx, out, m, b, k);
+    if (block_n == 256) return pg_launch<256>(dev, tw, tx, row_scale, out, m, b, k);
+    if (block_n == 128) return pg_launch<128>(dev, tw, tx, row_scale, out, m, b, k);
+    return pg_launch<64>(dev, tw, tx, row_scale, out, m, b, k);
 }
