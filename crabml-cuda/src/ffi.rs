@@ -129,6 +129,16 @@ extern "C" {
     // ---- greedy decoding without a host round trip per token (extension) ----
     pub fn cc_argmax_to_slot(dev: *mut cc_device, x: *const cc_view, slot: i32, hist_index: i64) -> c_int;
     pub fn cc_copy_rows_from_slot(dev: *mut cc_device, dst: *const cc_view, src: *const cc_view, slot: i32) -> c_int;
+    pub fn cc_sample_to_slot(
+        dev: *mut cc_device,
+        x: *const cc_view,
+        temperature: f32,
+        topp: f32,
+        seed: u64,
+        coin_index: i64,
+        slot: i32,
+        hist_index: i64,
+    ) -> c_int;
     pub fn cc_slot_set(dev: *mut cc_device, slot: i32, value: i64) -> c_int;
     pub fn cc_read_history(dev: *mut cc_device, first: i64, count: i64, out: *mut i64) -> c_int;
     pub fn cc_tensor_export_f32_async(dev: *mut cc_device, src: *const cc_view, dst: *mut f32, n: usize) -> c_int;

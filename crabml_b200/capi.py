@@ -140,6 +140,8 @@ def load_library(build_if_missing: bool = True):
         "ccr_runner_generate_greedy": (i32, [vp, C.POINTER(i64), i32, i32, i64, C.POINTER(i64), C.POINTER(i32)]),
         "ccr_runner_generate_greedy_ex": (i32, [vp, C.POINTER(i64), i32, i32, i64, C.POINTER(i64), C.POINTER(i32), vp]),
         "cc_argmax_to_slot": (i32, [vp, pv, i32, i64]),
+        "cc_sample_to_slot": (i32, [vp, pv, f32, f32, u64, i64, i32, i64]),
+        "ccr_runner_generate_ex": (i32, [vp, C.POINTER(i64), i32, i32, i64, f32, f32, u64, C.POINTER(i64), C.POINTER(i32), vp]),
         "cc_copy_rows_from_slot": (i32, [vp, pv, pv, i32]),
         "cc_slot_set": (i32, [vp, i32, i64]),
         "cc_read_history": (i32, [vp, i64, i64, C.POINTER(i64)]),

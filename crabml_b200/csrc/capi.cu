@@ -1,7 +1,7 @@
 // capi.cu -- extern "C" entry points: argument checks mirroring CpuTensor (cpu_tensor.rs:126-446) + launches.
 #include <string.h>
 
-#include "common.cuh"
+#include "sample_dev.cuh"
 
 // ---- strider helpers (tensor/strider.rs) ------------------------------------------------------------------
 static int64_t view_len(const cc_view* v) {
@@ -50,7 +50,7 @@ static bool view_in_bounds(const cc_view* v) {
                    "%s: view [%lld, %lld] does not match the quantized matrix [%lld, %lld]", what, (long long)(v)->shape[0],   \
                    (long long)((v)->ndim == 2 ? (v)->shape[1] : 0), (long long)(v)->buf->rows, (long long)(v)->buf->cols)
 // lazy mode (lazy.cu): after the same argument checks as eager mode the op is queued instead of launched
-enum { L_COPY_ROWS, L_DUP, L_RMS_NORM, L_MUL, L_ADD, L_SCALE, L_MATVEC, L_ROPE, L_CONCAT, L_CONTIGUOUS, L_BMM, L_SOFTMAX, L_SILU, L_GELU, L_ALLREDUCE, L_ALLGATHER, L_ARGMAX };
+enum { L_COPY_ROWS, L_DUP, L_RMS_NORM, L_MUL, L_ADD, L_SCALE, L_MATVEC, L_ROPE, L_CONCAT, L_CONTIGUOUS, L_BMM, L_SOFTMAX, L_SILU, L_GELU, L_ALLREDUCE, L_ALLGATHER, L_ARGMAX, L_SAMPLE };
 int cc_lazy_record(cc_device* dev, int kind, const cc_view* a, const cc_view* b, cc_buf* out, float f, int64_t i0, int64_t i1, int64_t i2,
                    const int64_t* rows, int n_rows);
 #define LAZY(dev) ((dev)->lz != nullptr && !(dev)->exact)
@@ -289,6 +289,32 @@ extern "C" CC_API int cc_argmax_to_slot(cc_device* dev, const cc_view* x, int32_
     if (rc) return rc;
     if (LAZY(dev)) return cc_lazy_record(dev, L_ARGMAX, x, nullptr, nullptr, 0, slot, hist_index, 0, nullptr, 0);
     return cc_launch_argmax(dev, (const float*)x->buf->plane[0], view_len(x), dev->slots + slot, dev->history, nullptr, hist_index);
+}
+// Temperature + top-p sampling into a slot (sampler.rs:27-107; sample_dev.cuh).  coin = 24 bits of splitmix64(seed ^
+// splitmix64(coin_index)) / 2^24, so one seed reproduces one run in every mode.  temperature 0 is cc_argmax_to_slot (same op, same bits).
+// The logits are not modified.
+extern "C" CC_API int cc_sample_to_slot(cc_device* dev, const cc_view* x, float temperature, float topp, uint64_t seed, int64_t coin_index,
+                                        int32_t slot, int64_t hist_index) {
+    CHECK_VIEW(dev, x, "sample_to_slot");
+    REQUIRE_F32(dev, x, "sample_to_slot");
+    CC_REQUIRE(dev, view_contiguous(x) && view_len(x) > 0, "sample_to_slot: tensor must be contiguous and non-empty");
+    CC_REQUIRE(dev, view_len(x) <= INT32_MAX, "sample_to_slot: %lld logits are too many", (long long)view_len(x));
+    CC_REQUIRE(dev, slot >= 0 && slot < CC_N_SLOTS && hist_index < CC_HISTORY_CAP, "sample_to_slot: slot %d / history index %lld out of range", slot, (long long)hist_index);
+    CC_REQUIRE(dev, temperature >= 0.0f, "sample_to_slot: temperature %g is not a number >= 0", (double)temperature);
+    CC_REQUIRE(dev, topp == topp, "sample_to_slot: topp is NaN");
+    if (temperature == 0.0f) return cc_argmax_to_slot(dev, x, slot, hist_index);        // sampler.rs:28-30
+    int rc = cc_ensure_slots(dev);
+    if (rc) return rc;
+    if (LAZY(dev)) {
+        uint32_t pb; memcpy(&pb, &topp, 4);
+        const int64_t extra[2] = {(int64_t)seed, (int64_t)pb};
+        return cc_lazy_record(dev, L_SAMPLE, x, nullptr, nullptr, temperature, slot, hist_index, coin_index, extra, 2);
+    }
+    rc = cc_ensure_sample_scratch(dev, view_len(x));
+    if (rc) return rc;
+    SampleDyn a;
+    a.seed = seed; a.coin_index = coin_index; a.hist_index = hist_index; a.temperature = temperature; a.topp = topp;
+    return cc_launch_sample(dev, (const float*)x->buf->plane[0], view_len(x), &a, nullptr, dev->slots + slot, dev->history);
 }
 // copy_rows_from with ONE row whose index is the content of a device slot
 extern "C" CC_API int cc_copy_rows_from_slot(cc_device* dev, const cc_view* dst, const cc_view* src, int32_t slot) {

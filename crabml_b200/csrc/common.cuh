@@ -128,6 +128,8 @@ struct cc_device {
     // of sampled ids, both in device memory
     int64_t* slots = nullptr;         // [CC_N_SLOTS]
     int64_t* history = nullptr;       // [CC_HISTORY_CAP]
+    void* sample_scratch = nullptr;   // temperature / top-p sampler (sample_dev.cuh): probabilities and the sort's key arrays
+    size_t sample_scratch_bytes = 0;
     unsigned* err_host = nullptr;     // host-mapped word a kernel raises when one of its bounded spins times out (mega.cu, comm.cu)
     unsigned* err_dev = nullptr;      // device copy polled by the other spinners of the same GPU
 
@@ -179,6 +181,14 @@ int cc_fail(cc_device* dev, int code, const char* fmt, ...);
                            cudaGetErrorString(_e), __FILE__, __LINE__);                     \
     } while (0)
 
+// counter-based generator of the synthetic weights (repack.cu) and of the sampler's coin (sample_dev.cuh)
+__host__ __device__ inline uint64_t cc_splitmix64(uint64_t x) {
+    x += 0x9E3779B97F4A7C15ull;
+    x = (x ^ (x >> 30)) * 0xBF58476D1CE4E5B9ull;
+    x = (x ^ (x >> 27)) * 0x94D049BB133111EBull;
+    return x ^ (x >> 31);
+}
+
 // ---- type facts ------------------------------------------------------------------------------
 int cc_block_elems(int t);
 size_t cc_block_bytes(int t);          // GGUF block size
@@ -228,6 +238,10 @@ int cc_launch_binary(cc_device* dev, float* x, int64_t n, const float* y, int64_
 int cc_launch_scale(cc_device* dev, float* x, int64_t n, float s);
 int cc_launch_argmax(cc_device* dev, const float* x, int64_t n, int64_t* slot, int64_t* hist, const int64_t* hist_index_dev, int64_t hist_index);
 int cc_ensure_slots(cc_device* dev);
+// ---- sample.cu: temperature + top-p sampling into a slot (sample_dev.cuh) ----
+struct SampleDyn;
+int cc_ensure_sample_scratch(cc_device* dev, int64_t n);
+int cc_launch_sample(cc_device* dev, const float* x, int64_t n, const SampleDyn* args, const SampleDyn* args_dev, int64_t* slot, int64_t* hist);
 int cc_launch_strided_copy(cc_device* dev, const void* src, int src_dtype, const int64_t* sshape,
                            const int64_t* sstrides, void* dst, int dst_dtype, const int64_t* dstrides,
                            int64_t dst_offset, int ndim);
@@ -266,7 +280,7 @@ struct AttnArgs {            // fused decode attention (fused.cu)
 };
 struct DeqPlanes { const uint8_t* p[CC_MAX_PLANES]; int64_t cols; };
 // megakernel phase descriptor (mega.cu); built by lazy.cu
-enum { MK_NORMQ = 0, MK_MATVEC = 1, MK_ATTN = 2, MK_ROWS = 3, MK_REDUCE = 4, MK_GATHER = 5, MK_ARGMAX = 6 };
+enum { MK_NORMQ = 0, MK_MATVEC = 1, MK_ATTN = 2, MK_ROWS = 3, MK_REDUCE = 4, MK_GATHER = 5, MK_ARGMAX = 6, MK_SAMPLE = 7 };
 struct MkPhase {
     int type, wtype, write_back, next_matvec;
     int xgpu, red_n, next_matvec2, spare; float* red_dst; const float* red_res;   // cross-GPU barrier after this phase ; REDUCE/GATHER phase operands   // next_matvec / next_matvec2: index of the next MATVEC phase and of the one after it (look-ahead prefetch), -1 if none
@@ -279,6 +293,7 @@ struct MkPhase {
     DeqPlanes planes; int src_dtype, dst_dtype, n_rows, pad; long long cols; void* dst;   // ROWS
     const long long* rows_dev;          // ROWS: row indices in device memory (a token slot) instead of the dyn block ; ARGMAX: x = input, n = length,
     long long* slot_dev; long long* hist_dev;   //   slot_dev / hist_dev = where the index goes (hist index at dyn_off, < 0: none)
+                                        // SAMPLE: as ARGMAX, with a SampleDyn at dyn_off and the sampler scratch at dst
 };
 size_t cc_mega_smem_for_phase(const MkPhase& ph);      // working area, without the norm-weight staging area on top of it
 const CommDev* cc_comm_dev(cc_device* dev);
@@ -289,7 +304,7 @@ int cc_launch_all_reduce(cc_device* dev, float* x, int64_t n, const float* resid
 int cc_launch_all_gather(cc_device* dev, const float* src, int64_t n, float* dst);
 extern "C" CC_API int cc_test_mega_barrier_floor(cc_device* dev, int n, float* us_per_phase);
 int cc_launch_mega(cc_device* dev, const MkPhase* phases_dev, int n_phases, const uint8_t* dyn_dev, unsigned* bar_dev, size_t smem_work, size_t smem_wstage,
-                   unsigned long long* prof, const CommDev* comm, bool generic);
+                   unsigned long long* prof, const CommDev* comm, bool generic, bool sample);
 // mega_ring.cu: the same phase table run by the kernel whose weights arrive through a TMA-fed shared-memory ring
 int cc_mega_flags();
 bool cc_mega_ring_enabled();
@@ -298,7 +313,7 @@ int cc_mega_ring_at_ch(const MkPhase& ph);
 size_t cc_mega_ring_smem_for_phase(const MkPhase& ph);
 bool cc_mega_ring_fits(size_t smem_work, size_t smem_wstage, int slot_bytes, bool generic);
 int cc_launch_mega_ring(cc_device* dev, const MkPhase* phases_dev, int n_phases, const uint8_t* dyn_dev, unsigned* bar_dev, size_t smem_work, size_t smem_wstage,
-                        unsigned long long* prof, const CommDev* comm, bool generic, int slot_bytes, int at_ch, int flags);
+                        unsigned long long* prof, const CommDev* comm, bool generic, bool sample, int slot_bytes, int at_ch, int flags);
 int cc_check_async_error(cc_device* dev);     // after a stream synchronize: did a persistent kernel give up on a barrier?
 int cc_launch_normq(cc_device* dev, float* x, float* orig, const float* norm_w, float eps, int64_t n, void* act_scratch, bool write_back);
 int cc_launch_attn_decode(cc_device* dev, const AttnArgs& a);

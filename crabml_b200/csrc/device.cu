@@ -123,6 +123,7 @@ extern "C" CC_API void cc_device_destroy(cc_device* dev) {
     if (dev->err_dev) cudaFree(dev->err_dev);
     if (dev->slots) cudaFree(dev->slots);
     if (dev->history) cudaFree(dev->history);
+    if (dev->sample_scratch) cudaFree(dev->sample_scratch);
     if (dev->dev_idx) cudaFree(dev->dev_idx);
     cudaFree(dev->exp_lut);
     cudaFree(dev->gelu_lut);

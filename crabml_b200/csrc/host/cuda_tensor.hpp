@@ -151,6 +151,10 @@ public:
         cc_view v = view();
         check(dev_, cc_argmax_to_slot(dev_, &v, slot, hist_index));
     }
+    void sample_to_slot(float temperature, float topp, uint64_t seed, int64_t coin_index, int slot, int64_t hist_index) const {
+        cc_view v = view();
+        check(dev_, cc_sample_to_slot(dev_, &v, temperature, topp, seed, coin_index, slot, hist_index));
+    }
     void export_async(float* dst, size_t n) const {
         cc_view v = view();
         check(dev_, cc_tensor_export_f32_async(dev_, &v, dst, n));

@@ -10,6 +10,7 @@
 
 #include "../../../include/crabml_runner.h"
 #include "cuda_tensor.hpp"
+#include "generate_loop.hpp"
 
 using crabml::CudaTensor;
 using crabml::TensorStrider;
@@ -40,7 +41,7 @@ struct ccr_runner {
     CudaTensor forward_qwen2(const std::vector<int64_t>& tokens, int64_t pos, int slot);
     CudaTensor forward_gemma(const std::vector<int64_t>& tokens, int64_t pos, int slot);
     CudaTensor logits_tensor(CudaTensor x, int64_t n_batch);
-    void greedy_step(const int64_t* token, int64_t pos, int64_t hist_index, float* logits_async);
+    void decode_step(const int64_t* token, int64_t pos, int64_t hist_index, float* logits_async, const ccr_step_sampler& pick);
     CudaTensor forward_multi_query_attention(CudaTensor q, CudaTensor k, CudaTensor v, int l, int64_t n_batch);
     CudaTensor forward_ffn(CudaTensor x, int l, bool gelu = false);
     void forward(const std::vector<int64_t>& tokens, int64_t pos, float* logits_out);
@@ -68,11 +69,11 @@ void ccr_runner::forward(const std::vector<int64_t>& tokens, int64_t pos, float*
 }
 
 // One decode step whose sampled token never visits the host: forward (token from the host, or -- token == nullptr -- from device slot 0),
-// greedy argmax (sampler.rs:109-116) into slot 0 and the device-side history; optionally the logits are exported WITHOUT waiting.
-void ccr_runner::greedy_step(const int64_t* token, int64_t pos, int64_t hist_index, float* logits_async) {
+// the sampler (greedy: argmax, sampler.rs:109-116) into slot 0 and the device-side history; optionally the logits are exported WITHOUT waiting.
+void ccr_runner::decode_step(const int64_t* token, int64_t pos, int64_t hist_index, float* logits_async, const ccr_step_sampler& pick) {
     CudaTensor x = token ? forward_arch({*token}, pos) : forward_arch({0}, pos, 0);
     CudaTensor lg = logits_tensor(std::move(x), 1);
-    lg.argmax_to_slot(0, hist_index);
+    pick(lg, hist_index);
     if (logits_async) lg.export_async(logits_async, (size_t)conf.vocab_size);     // flushes (asynchronously) as well
     else CudaTensor::check(dev, cc_device_flush(dev));
 }
@@ -320,6 +321,7 @@ extern "C" CC_API int ccr_runner_create(cc_device* dev, const ccr_llama_config* 
 }
 
 extern "C" CC_API void ccr_runner_destroy(ccr_runner* r) { delete r; }
+int ccr_runner_fail(ccr_runner* r, int code, const char* msg) { r->last_error = msg; return code; }
 extern "C" CC_API const char* ccr_runner_last_error(ccr_runner* r) { return r ? r->last_error.c_str() : ""; }
 extern "C" CC_API int64_t ccr_runner_kv_cache_len(ccr_runner* r) { return r ? r->kv_cache_len() : -1; }
 
@@ -337,6 +339,12 @@ extern "C" CC_API int ccr_runner_forward(ccr_runner* r, const int64_t* tokens, i
 // staging ring -- what a host-side sampler would consume.
 extern "C" CC_API int ccr_runner_generate_greedy_ex(ccr_runner* r, const int64_t* prompt, int32_t n_prompt, int32_t steps,
                                                     int64_t eos_token, int64_t* out_tokens, int32_t* n_out, float* logits_out) {
+    return ccr_runner_generate_loop(r, prompt, n_prompt, steps, eos_token, out_tokens, n_out, logits_out,
+                                    [](const CudaTensor& lg, int64_t i) { lg.argmax_to_slot(0, i); });
+}
+// the loop of both generate entry points (generate_loop.hpp); `pick` samples generated token i into slot 0 and history[i]
+int ccr_runner_generate_loop(ccr_runner* r, const int64_t* prompt, int32_t n_prompt, int32_t steps, int64_t eos_token, int64_t* out_tokens,
+                             int32_t* n_out, float* logits_out, const ccr_step_sampler& pick) {
     if (!r || !prompt || n_prompt < 1 || !out_tokens || !n_out || steps < 1) return CC_ERR_ARG;
     *n_out = 0;
     float* pinned = nullptr;
@@ -355,15 +363,15 @@ extern "C" CC_API int ccr_runner_generate_greedy_ex(ccr_runner* r, const int64_t
             pinned = r->pinned_logits;
         }
         for (int i = 0; i + 1 < n_prompt; i++) r->forward({prompt[i]}, pos++, nullptr);
-        r->greedy_step(&prompt[n_prompt - 1], pos++, 0, pinned);
+        r->decode_step(&prompt[n_prompt - 1], pos++, 0, pinned, pick);
         int64_t done = 1;
         if (eos_token < 0) {
-            for (; done < total; done++) r->greedy_step(nullptr, pos++, done, pinned ? pinned + (size_t)done * vocab : nullptr);
+            for (; done < total; done++) r->decode_step(nullptr, pos++, done, pinned ? pinned + (size_t)done * vocab : nullptr, pick);
             CudaTensor::check(r->dev, cc_read_history(r->dev, 0, done, out_tokens));
         } else {
             CudaTensor::check(r->dev, cc_read_history(r->dev, 0, 1, out_tokens));
             for (; done < total; done++) {
-                r->greedy_step(nullptr, pos++, done, pinned ? pinned + (size_t)done * vocab : nullptr);
+                r->decode_step(nullptr, pos++, done, pinned ? pinned + (size_t)done * vocab : nullptr, pick);
                 CudaTensor::check(r->dev, cc_read_history(r->dev, done, 1, out_tokens + done));
                 if (out_tokens[done] == eos_token) break;          // the reference returns before yielding EOS (llama2.rs:160-163)
             }

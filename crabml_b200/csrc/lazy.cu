@@ -19,9 +19,9 @@
 #include <chrono>
 #include <functional>
 
-#include "common.cuh"
+#include "sample_dev.cuh"
 
-enum LKind { L_COPY_ROWS, L_DUP, L_RMS_NORM, L_MUL, L_ADD, L_SCALE, L_MATVEC, L_ROPE, L_CONCAT, L_CONTIGUOUS, L_BMM, L_SOFTMAX, L_SILU, L_GELU, L_ALLREDUCE, L_ALLGATHER, L_ARGMAX };
+enum LKind { L_COPY_ROWS, L_DUP, L_RMS_NORM, L_MUL, L_ADD, L_SCALE, L_MATVEC, L_ROPE, L_CONCAT, L_CONTIGUOUS, L_BMM, L_SOFTMAX, L_SILU, L_GELU, L_ALLREDUCE, L_ALLGATHER, L_ARGMAX, L_SAMPLE };
 
 struct LView { cc_buf* buf = nullptr; int ndim = 0; int64_t shape[CC_MAX_DIMS] = {0, 0, 0, 0}, strides[CC_MAX_DIMS] = {0, 0, 0, 0}; };
 
@@ -140,6 +140,7 @@ struct Plan {
     bool mega_ring = false;          // weights through the shared-memory ring (mega_ring.cu)
     int ring_slot = 0, ring_at_ch = 64;
     bool mega_generic = false;       // some MATVEC phase is generic (K-quant weights): launch the instantiation that carries that code
+    bool mega_sample = false;        // the table ends with a SAMPLE phase: launch the instantiation that carries the sampler's call
     void S(uint64_t v) { sig.push_back(v); }
     void SP(const void* p) { sig.push_back((uint64_t)(uintptr_t)p); }
     size_t dyn_put(const void* p, size_t n) {
@@ -470,6 +471,30 @@ struct Fuser {
         return 1;
     }
 
+    // ---- pattern: temperature + top-p sampling (cc_sample_to_slot): seed, coin index, temperature, topp and the history index travel
+    // in dyn, so one graph serves every step and every setting -------------------------------------------------------------------------
+    size_t try_sample(size_t i) {
+        if (!is(i, L_SAMPLE)) return 0;
+        const LOp& op = q[i];
+        cc_device* d = dev;
+        const float* x = (const float*)op.a.buf->plane[0];
+        const int64_t n = vlen(op.a);
+        int64_t* slot = dev->slots + op.i0;
+        int64_t* hist = dev->history;
+        void* scratch = dev->sample_scratch;            // sized for this queue before fusing (cc_lazy_flush)
+        SampleDyn a;
+        a.seed = (unsigned long long)op.rows[0]; a.coin_index = op.i2; a.hist_index = op.i1; a.temperature = op.f;
+        const uint32_t pb = (uint32_t)op.rows[1]; memcpy(&a.topp, &pb, 4);
+        const size_t off = P.dyn_put(&a, sizeof(a));
+        P.S(0x2008); P.SP(x); P.S((uint64_t)n); P.SP(slot); P.S(off); P.SP(scratch);
+        P.steps.push_back([=](uint8_t* dyn_dev) { return cc_launch_sample(d, x, n, nullptr, (const SampleDyn*)(dyn_dev + off), slot, hist); });
+        { MkPhase ph = {}; ph.type = MK_SAMPLE; ph.x = (float*)x; ph.n = (int)n; ph.dyn_off = off; ph.slot_dev = (long long*)slot; ph.hist_dev = (long long*)hist;
+          ph.dst = scratch; P.phases.push_back(ph); }
+        P.mega_sample = true;
+        q[i].done = true;
+        return 1;
+    }
+
     // ---- pattern: K-quant matvecs (generic MATVEC phase of the megakernel) ----------------------------------------------------------------
     //   [[DUP] RMS_NORM MUL]  MATVEC{1..3, same K-quant type, same f32 row x, b = 1}  [SILU MUL | ADD]
     // In the CUDA-graph mode (lazy = 1) these ops keep running as their eager kernels, in order (fallback steps); for the megakernel
@@ -560,6 +585,7 @@ struct Fuser {
             cc_buf* xb = nullptr;
             if ((used = try_copy_rows(i))) { i += used; continue; }
             if ((used = try_argmax(i))) { i += used; continue; }
+            if ((used = try_sample(i))) { i += used; continue; }
             if ((used = try_generic(i))) { i += used; continue; }
             if ((used = try_normq(i, 0, &xb))) {
                 i += used;
@@ -612,6 +638,8 @@ int cc_lazy_flush(cc_device* dev) {
         int64_t bb = op.b.ndim == 1 ? 1 : op.b.shape[0];
         if (at != CC_F32 && (rc = cc_ensure_act_scratch(dev, cc_act_bytes(at, bb * op.a.shape[1])))) return rc;
     }
+    // the sampler's scratch is baked into captured graphs: it must have its final size before any capture
+    for (auto& op : lz->q) if (op.kind == L_SAMPLE && (rc = cc_ensure_sample_scratch(dev, vlen(op.a)))) return rc;
     auto t_f0 = std::chrono::steady_clock::now();
     Plan P;
     Fuser F{dev, lz, lz->q, P};
@@ -675,6 +703,13 @@ int cc_lazy_flush(cc_device* dev) {
                 }
                 if (work + wst + 4096 > 227 * 1024) use_mega = false;
             }
+            // the megakernel runs ONE SAMPLE phase, after its phase loop (mega.cu): a table with more than one, or with anything queued
+            // behind the sampler (several tokens submitted before one flush), runs in the CUDA-graph mode
+            if (use_mega && P.mega_sample) {
+                int n_sample = 0;
+                for (auto& ph : P.phases) n_sample += ph.type == MK_SAMPLE;
+                if (n_sample != 1 || P.phases.back().type != MK_SAMPLE) use_mega = false;
+            }
             if (use_mega) {       // phase table lives in device memory for the lifetime of the graph
                 int nxt = -1, nxt2 = -1;
                 for (int t = (int)P.phases.size() - 1; t >= 0; t--) {
@@ -719,8 +754,8 @@ int cc_lazy_flush(cc_device* dev) {
                 unsigned long long* prof = P.phases.size() < 4000 ? lz->prof_dev : nullptr;
                 if (!use_mega) rc = run_steps(lz->dyn_dev);
                 else if (P.mega_ring) rc = cc_launch_mega_ring(dev, ge.phases_dev, (int)P.phases.size(), lz->dyn_dev, lz->bar_dev, P.mega_smem, P.mega_wstage, prof, cc_comm_dev(dev),
-                                                               P.mega_generic, P.ring_slot, P.ring_at_ch, cc_mega_flags());
-                else rc = cc_launch_mega(dev, ge.phases_dev, (int)P.phases.size(), lz->dyn_dev, lz->bar_dev, P.mega_smem, P.mega_wstage, prof, cc_comm_dev(dev), P.mega_generic);
+                                                               P.mega_generic, P.mega_sample, P.ring_slot, P.ring_at_ch, cc_mega_flags());
+                else rc = cc_launch_mega(dev, ge.phases_dev, (int)P.phases.size(), lz->dyn_dev, lz->bar_dev, P.mega_smem, P.mega_wstage, prof, cc_comm_dev(dev), P.mega_generic, P.mega_sample);
                 e = cudaStreamEndCapture(dev->stream, &graph);
                 if (!rc && e != cudaSuccess) rc = cc_fail(dev, CC_ERR_CUDA, "lazy: end capture: %s", cudaGetErrorString(e));
             }

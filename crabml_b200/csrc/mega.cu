@@ -243,7 +243,9 @@ __device__ void phase_matvec(const MkPhase& ph, uint8_t* smem, float* s_w, bool 
 
 // GEN: the phase table contains generic (K-quant) MATVEC phases.  The streaming-only instantiation carries none of their code, so
 // its register allocation (the weight pipe lives in registers across phases) is not disturbed by them.
-template <bool GEN>
+// SMP: the table ends with its only SAMPLE phase, run after the phase loop.  Only these instantiations carry the call, so the greedy ones keep
+// their register allocation.
+template <bool GEN, bool SMP>
 __global__ void __launch_bounds__(MK_THREADS, MK_CTAS_PER_SM) mega_kernel(const MkPhase* __restrict__ phases, int n_phases, const uint8_t* dyn,
                                                                          unsigned* bar, const uint16_t* exp_lut, unsigned long long* prof, int flags, int wtop_off,
                                                                          unsigned* err_host, const CommDev comm) {
@@ -273,7 +275,8 @@ __global__ void __launch_bounds__(MK_THREADS, MK_CTAS_PER_SM) mega_kernel(const 
         int* dst = (int*)&s_phs[0];
         for (int i = threadIdx.x; i < (int)(sizeof(MkPhase) / 4); i += MK_THREADS) dst[i] = src[i];
     }
-    for (int p = 0; p < n_phases; p++) {
+    const int n_loop = SMP ? n_phases - 1 : n_phases;      // SMP: the last phase, the sampler, runs after the loop
+    for (int p = 0; p < n_loop; p++) {
         // developer profiling, 4 stamps per phase from CTA 0 / thread 0: start, activation ready (MATVEC), rows done, arrived + prefetch issued
         const bool stamp = prof && blockIdx.x == 0 && threadIdx.x == 0;
         if (stamp) { prof[p * MK_PROF_SLOTS] = globaltimer_ns(); prof[p * MK_PROF_SLOTS + 1] = 0; prof[p * MK_PROF_SLOTS + 4] = 0; prof[p * MK_PROF_SLOTS + 5] = 0; }
@@ -380,6 +383,12 @@ __global__ void __launch_bounds__(MK_THREADS, MK_CTAS_PER_SM) mega_kernel(const 
             }
         }
     }
+    // the SAMPLE phase (lazy.cu: the only one, and the last): called after the loop, where the weight pipe is dead, so the call saves
+    // nothing around itself (the barrier before it was the last iteration's)
+    if constexpr (SMP) {
+        __syncthreads();
+        if (!s_abort) phase_sample(s_phs[(n_phases - 1) & 1], dyn, work, exp_lut);
+    }
     if (comm.world > 0 && blockIdx.x == 0 && threadIdx.x == 0) *comm.seq = xseq;
     if (prof && blockIdx.x == 0 && threadIdx.x == 0) prof[n_phases * MK_PROF_SLOTS] = globaltimer_ns();
 }
@@ -393,6 +402,7 @@ size_t cc_mega_smem_for_phase(const MkPhase& ph) {
         return nbp * 40 + 256 + 2048 + (ph.x ? k * 4 : 0);
     }
     if (ph.type == MK_ATTN) return (size_t)(3 * ph.at.hd + ((ph.at.max_len + 8 + 3) & ~3) + AT_NBUF * AT_CH * ph.at.hd) * 4 + 64;
+    if (ph.type == MK_SAMPLE) return SMP_SMEM_BYTES;
     return 1024;
 }
 
@@ -411,7 +421,7 @@ extern "C" CC_API int cc_test_mega_barrier_floor(cc_device* dev, int n, float* u
     for (int rep = 0; rep < 4; rep++) {
         CC_CUDA(dev, cudaMemsetAsync(d_bar, 0, 4096, dev->stream));
         cudaEventRecord(e0, dev->stream);
-        int rc = cc_launch_mega(dev, d_tab, n, nullptr, d_bar, 1024, 0, nullptr, nullptr, false);
+        int rc = cc_launch_mega(dev, d_tab, n, nullptr, d_bar, 1024, 0, nullptr, nullptr, false, false);
         if (rc) return rc;
         cudaEventRecord(e1, dev->stream);
         CC_CUDA(dev, cudaEventSynchronize(e1));
@@ -436,13 +446,13 @@ int cc_mega_flags() {
 bool cc_mega_ring_enabled() { return (cc_mega_flags() & MK_F_RING) != 0; }
 
 int cc_launch_mega(cc_device* dev, const MkPhase* phases_dev, int n_phases, const uint8_t* dyn_dev, unsigned* bar_dev, size_t smem_work, size_t smem_wstage,
-                   unsigned long long* prof, const CommDev* comm, bool generic) {
+                   unsigned long long* prof, const CommDev* comm, bool generic, bool sample) {
     const int flags = cc_mega_flags();
     int max_ctas_per_sm = 0;
     const size_t wtop = (smem_work + 15) & ~(size_t)15;
     const size_t smem = wtop + smem_wstage;
     CC_REQUIRE(dev, smem <= 227 * 1024, "megakernel: a phase needs %zu bytes of shared memory", smem);
-    auto kern = generic ? mega_kernel<true> : mega_kernel<false>;
+    auto kern = generic ? (sample ? mega_kernel<true, true> : mega_kernel<true, false>) : (sample ? mega_kernel<false, true> : mega_kernel<false, false>);
     if (smem > 48 * 1024) CC_CUDA(dev, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     CC_CUDA(dev, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&max_ctas_per_sm, kern, MK_THREADS, smem));
     CC_REQUIRE(dev, max_ctas_per_sm >= 1, "megakernel does not fit on an SM");

@@ -10,6 +10,7 @@
 #include "dequant.cuh"
 #include "quantize_dev.cuh"
 #include "vecdot.cuh"
+#include "sample_dev.cuh"
 
 #ifndef MK_SYNC
 #error "define MK_SYNC() before including mega_phases.cuh"
@@ -626,6 +627,18 @@ static __device__ void phase_argmax(const MkPhase& ph, const uint8_t* dyn, float
         if (h >= 0 && h < CC_HISTORY_CAP) ph.hist_dev[h] = bi;
     }
     MK_SYNC();
+}
+
+// ---- SAMPLE phase: temperature + top-p sampling (sample_dev.cuh, the kernel of the other modes); CTA 0 only, in the working area ----------
+// __noinline__: the sampler's registers are its own; neither persistent kernel's allocation sees them
+static __device__ __noinline__ void phase_sample(const MkPhase& ph, const uint8_t* dyn, uint8_t* work, const uint16_t* exp_lut) {
+    if (blockIdx.x != 0) return;
+    const SampleDyn a = *(const SampleDyn*)(dyn + ph.dyn_off);
+    const long long id = cc_sample_block(ph.x, ph.n, a, false, cc_sample_scratch(ph.dst, ph.n), work, exp_lut);
+    if (threadIdx.x == 0) {
+        *ph.slot_dev = id;
+        if (a.hist_index >= 0 && a.hist_index < CC_HISTORY_CAP) ph.hist_dev[a.hist_index] = id;
+    }
 }
 
 // ---- REDUCE / GATHER phases: second half of an exchange (the first half is epilogue 3 of the MATVEC phase + the handshake

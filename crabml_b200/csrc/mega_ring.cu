@@ -514,7 +514,7 @@ __device__ void phase_matvec_ring(const MkPhase& ph, uint8_t* smem, const uint16
     }
 }
 
-template <bool GEN>
+template <bool GEN, bool SMP>      // SMP: the table ends with its only SAMPLE phase (see mega.cu)
 __global__ void __launch_bounds__(MR_THREADS, 1) mega_ring_kernel(const MkPhase* __restrict__ phases, int n_phases, const uint8_t* dyn, unsigned* bar,
                                                                   const uint16_t* exp_lut, unsigned long long* prof, int flags, int wtop_off, unsigned* err_host,
                                                                   const CommDev comm, const MrRing R) {
@@ -556,7 +556,8 @@ __global__ void __launch_bounds__(MR_THREADS, 1) mega_ring_kernel(const MkPhase*
     if (threadIdx.x == MK_BAR_THREAD) gen = ld_acquire_u32(&bar[32]);
     unsigned xseq = comm.world > 0 ? *comm.seq : 0u;
     for (int i = threadIdx.x; i < MR_DESC_WORDS; i += MK_THREADS) ((int*)&s_phs[0])[i] = ((const int*)phases)[i];
-    for (int p = 0; p < n_phases; p++) {
+    const int n_loop = SMP ? n_phases - 1 : n_phases;      // SMP: the last phase, the sampler, runs after the loop
+    for (int p = 0; p < n_loop; p++) {
         const bool stamp = prof && blockIdx.x == 0 && threadIdx.x == 0;
         if (stamp) { prof[p * MK_PROF_SLOTS] = globaltimer_ns(); prof[p * MK_PROF_SLOTS + 1] = 0; prof[p * MK_PROF_SLOTS + 4] = 0; prof[p * MK_PROF_SLOTS + 5] = 0; }
         MK_SYNC();                           // descriptor p is in shared memory (stored one phase ago)
@@ -604,6 +605,10 @@ __global__ void __launch_bounds__(MR_THREADS, 1) mega_ring_kernel(const MkPhase*
             if (s_abort) break;              // a barrier timed out: bail out, the host reports it
         }
     }
+    if constexpr (SMP) {                     // the SAMPLE phase after the loop, as in mega.cu
+        MK_SYNC();
+        if (!s_abort) phase_sample(s_phs[(n_phases - 1) & 1], dyn, work, exp_lut);
+    }
     if (comm.world > 0 && blockIdx.x == 0 && threadIdx.x == 0) *comm.seq = xseq;
     if (prof && blockIdx.x == 0 && threadIdx.x == 0) prof[n_phases * MK_PROF_SLOTS] = globaltimer_ns();
     // a launch that gave up: the producer stops at its next look at s_abort; bulk copies it has already issued must land before
@@ -641,6 +646,7 @@ size_t cc_mega_ring_smem_for_phase(const MkPhase& ph) {
         return nbp * 40 + 256 + 2048;
     }
     if (ph.type == MK_ATTN) return (size_t)(3 * ph.at.hd + ((ph.at.max_len + 8 + 3) & ~3)) * 4 + (size_t)AT_NBUF * cc_mega_ring_at_ch(ph) * ph.at.hd * (ph.at.kv_f16 ? 2 : 4) + 64;
+    if (ph.type == MK_SAMPLE) return SMP_SMEM_BYTES;
     return 1024;
 }
 // slots the ring would get beside a working area of `smem_work` (+ `smem_wstage`) bytes; lazy.cu falls back to the register-pipe kernel
@@ -649,7 +655,7 @@ size_t cc_mega_ring_smem_for_phase(const MkPhase& ph) {
 static size_t mr_ring_off(size_t smem_work, size_t smem_wstage) { return ((((smem_work + 15) & ~(size_t)15) + smem_wstage) + 127) & ~(size_t)127; }
 int cc_mega_ring_slots(size_t smem_work, size_t smem_wstage, int slot_bytes, bool generic) {
     cudaFuncAttributes fa;
-    if (cudaFuncGetAttributes(&fa, generic ? mega_ring_kernel<true> : mega_ring_kernel<false>) != cudaSuccess) { cudaGetLastError(); return 0; }
+    if (cudaFuncGetAttributes(&fa, generic ? mega_ring_kernel<true, false> : mega_ring_kernel<false, false>) != cudaSuccess) { cudaGetLastError(); return 0; }
     const size_t cap = 227 * 1024 - fa.sharedSizeBytes, off = mr_ring_off(smem_work, smem_wstage);
     if (slot_bytes <= 0 || off >= cap) return 0;
     const size_t n = (cap - off) / (size_t)slot_bytes;
@@ -658,8 +664,8 @@ int cc_mega_ring_slots(size_t smem_work, size_t smem_wstage, int slot_bytes, boo
 bool cc_mega_ring_fits(size_t smem_work, size_t smem_wstage, int slot_bytes, bool generic) { return cc_mega_ring_slots(smem_work, smem_wstage, slot_bytes, generic) >= MR_MIN_SLOTS; }
 
 int cc_launch_mega_ring(cc_device* dev, const MkPhase* phases_dev, int n_phases, const uint8_t* dyn_dev, unsigned* bar_dev, size_t smem_work, size_t smem_wstage,
-                        unsigned long long* prof, const CommDev* comm, bool generic, int slot_bytes, int at_ch, int flags) {
-    auto kern = generic ? mega_ring_kernel<true> : mega_ring_kernel<false>;
+                        unsigned long long* prof, const CommDev* comm, bool generic, bool sample, int slot_bytes, int at_ch, int flags) {
+    auto kern = generic ? (sample ? mega_ring_kernel<true, true> : mega_ring_kernel<true, false>) : (sample ? mega_ring_kernel<false, true> : mega_ring_kernel<false, false>);
     cudaFuncAttributes fa;
     CC_CUDA(dev, cudaFuncGetAttributes(&fa, kern));
     const size_t wtop = (smem_work + 15) & ~(size_t)15;

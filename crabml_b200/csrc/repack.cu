@@ -149,12 +149,6 @@ int cc_launch_dequant_rows(cc_device* dev, const cc_buf* src, const int64_t* row
 // written in GGUF block layout, f16 scale fields overwritten with values uniform in [0.75,1.25)*scale.
 // oracle/synth.py holds the identical CPU generator (checked bit for bit in tests/test_gpu_synth.py).
 // ---------------------------------------------------------------------------------------------------
-__host__ __device__ inline uint64_t splitmix64(uint64_t x) {
-    x += 0x9E3779B97F4A7C15ull;
-    x = (x ^ (x >> 30)) * 0xBF58476D1CE4E5B9ull;
-    x = (x ^ (x >> 27)) * 0x94D049BB133111EBull;
-    return x ^ (x >> 31);
-}
 
 struct SynthSpec { int n_f16; int off[2]; int is_min[2]; int d_f32_off; };
 
@@ -176,13 +170,13 @@ __global__ void synth_kernel(uint8_t* out, int64_t nblocks, int bb, SynthSpec sp
     int64_t total = nblocks * bb;
     int64_t base = w * 8;
     if (base >= total) return;
-    uint64_t r = splitmix64(key ^ (uint64_t)w);
+    uint64_t r = cc_splitmix64(key ^ (uint64_t)w);
     for (int j = 0; j < 8 && base + j < total; j++) out[base + j] = (uint8_t)(r >> (8 * j));
 }
 __global__ void synth_scales_kernel(uint8_t* out, int64_t nblocks, int bb, SynthSpec sp, uint64_t key, float scale) {
     int64_t b = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (b >= nblocks) return;
-    uint64_t r = splitmix64(key ^ 0xD1B54A32D192ED03ull ^ (uint64_t)b);
+    uint64_t r = cc_splitmix64(key ^ 0xD1B54A32D192ED03ull ^ (uint64_t)b);
     for (int f = 0; f < sp.n_f16; f++) {
         // uniform in [0.75, 1.25) * scale: plain f32 mul/add only, so oracle/synth.py reproduces it bit for bit
         float u = (float)((r >> (16 * f)) & 0xFFFF) * (1.0f / 65536.0f);
@@ -203,7 +197,7 @@ __global__ void synth_scales_kernel(uint8_t* out, int64_t nblocks, int bb, Synth
 int cc_launch_synth(cc_device* dev, uint8_t* gguf_dev, int t, int64_t nblocks, uint64_t seed, uint64_t tid, float scale) {
     int bb = (int)cc_block_bytes(t);
     SynthSpec sp = synth_spec(t);
-    uint64_t key = splitmix64(seed ^ splitmix64(tid));
+    uint64_t key = cc_splitmix64(seed ^ cc_splitmix64(tid));
     int64_t words = (nblocks * bb + 7) / 8;
     synth_kernel<<<(unsigned)((words + 255) / 256), 256, 0, dev->stream>>>(gguf_dev, nblocks, bb, sp, key, scale);
     CC_LAUNCH_CHECK(dev);

@@ -107,6 +107,26 @@ class LlamaRunner:
                                                                   logits.ctypes.data_as(C.c_void_p)))
         return [int(out[i]) for i in range(n.value)], logits[:n.value]
 
+    def _generate_ex(self, prompt, steps, temperature, topp, seed, eos, logits):
+        p = (C.c_int64 * len(prompt))(*[int(t) for t in prompt])
+        out = (C.c_int64 * max(1, steps))()
+        n = C.c_int32(0)
+        self._check(self.device.lib.ccr_runner_generate_ex(self.handle, p, len(prompt), steps, eos, float(temperature), float(topp),
+                                                           int(seed) & (2**64 - 1), out, C.byref(n),
+                                                           None if logits is None else logits.ctypes.data_as(C.c_void_p)))
+        return [int(out[i]) for i in range(n.value)]
+
+    def generate(self, prompt, steps, temperature, topp, seed, eos=-1):
+        """ccr_runner_generate_ex: the greedy loop with Llama2Sampler (sampler.rs:27-107) on the device; the coin of generated
+        token i is coin index i of `seed`.  temperature 0 is generate_greedy."""
+        return self._generate_ex(prompt, steps, temperature, topp, seed, eos, None)
+
+    def generate_logits(self, prompt, steps, temperature, topp, seed, eos=-1):
+        """generate, also returning the logits of every generated position (as generate_greedy_logits): (ids, logits[n, vocab])."""
+        logits = np.zeros((max(1, steps), self.conf.vocab_size), np.float32)
+        ids = self._generate_ex(prompt, steps, temperature, topp, seed, eos, logits)
+        return ids, logits[:len(ids)]
+
     def close(self):
         if self.handle:
             self.device.lib.ccr_runner_destroy(self.handle)

@@ -328,6 +328,14 @@ class CudaTensor:
         self.device.check(self.device.lib.cc_batch_matmul(self.device.handle, C.byref(self._view()), C.byref(b._view()), C.byref(h)))
         return self._new(h, [self.shape()[0], self.shape()[1], b.shape()[2]])
 
+    # -- sampling on the device (crabml_cuda.h; not part of the reference's trait) ------------------------------------
+    def sample_to_slot(self, temperature, topp, seed, coin_index, slot=0, hist_index=-1):
+        """Llama2Sampler::sample (sampler.rs:27-107) of these logits into device slot `slot` (and history[hist_index] when >= 0);
+        temperature 0 is the argmax.  Read the id back with the device's history (cc_read_history)."""
+        self.device.check(self.device.lib.cc_sample_to_slot(self.device.handle, C.byref(self._view()), float(temperature), float(topp),
+                                                            int(seed) & (2**64 - 1), int(coin_index), int(slot), int(hist_index)))
+        return self
+
     # -- test hooks -----------------------------------------------------------------------------------------------------
     def quantize_activation(self, act_type, nbytes):
         out = np.empty(nbytes, np.uint8)

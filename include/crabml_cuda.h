@@ -154,6 +154,13 @@ CC_API int cc_dump_debug_tensor(cc_device* dev, const char* name, float* dst, si
  * be pinned: cc_host_alloc) -- it is complete after the next synchronising call. */
 CC_API int cc_argmax_to_slot(cc_device* dev, const cc_view* x, int32_t slot, int64_t hist_index);
 CC_API int cc_copy_rows_from_slot(cc_device* dev, const cc_view* dst, const cc_view* src, int32_t slot);
+/* Llama2Sampler::sample (sampler.rs:27-107) on the device, into a slot like cc_argmax_to_slot: softmax of x / temperature, then the
+ * reference's top-p walk over the probabilities sorted ASCENDING (quirk B21: topp < 1 keeps the low-probability tail).  The coin is
+ * (splitmix64(seed ^ splitmix64(coin_index)) >> 40) * 2^-24, so one seed reproduces one run.  temperature == 0 is cc_argmax_to_slot.
+ * Where the reference panics (no probability reaches the cutoff) the argmax is taken.  x is not modified.  A NaN or negative
+ * temperature, a NaN topp, and a non-f32 or non-contiguous x are CC_ERR_TENSOR. */
+CC_API int cc_sample_to_slot(cc_device* dev, const cc_view* x, float temperature, float topp, uint64_t seed, int64_t coin_index,
+                             int32_t slot, int64_t hist_index);
 CC_API int cc_slot_set(cc_device* dev, int32_t slot, int64_t value);
 CC_API int cc_read_history(cc_device* dev, int64_t first, int64_t count, int64_t* out);
 CC_API int cc_tensor_export_f32_async(cc_device* dev, const cc_view* src, float* dst, size_t n);

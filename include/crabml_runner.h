@@ -65,6 +65,12 @@ CC_API int ccr_runner_generate_greedy(ccr_runner* r, const int64_t* prompt, int3
 CC_API int ccr_runner_generate_greedy_ex(ccr_runner* r, const int64_t* prompt, int32_t n_prompt, int32_t steps,
                                          int64_t eos_token, int64_t* out_tokens, int32_t* n_out, float* logits_out);
 
+/* the same loop with Llama2Sampler (sampler.rs:27-107: temperature, top-p) in place of the argmax, on the device
+ * (cc_sample_to_slot); the coin of generated token i is coin_index i of `seed`.  temperature == 0 is
+ * ccr_runner_generate_greedy_ex, bit for bit.  A NaN or negative temperature or a NaN topp is CC_ERR_TENSOR. */
+CC_API int ccr_runner_generate_ex(ccr_runner* r, const int64_t* prompt, int32_t n_prompt, int32_t steps, int64_t eos_token,
+                                  float temperature, float topp, uint64_t seed, int64_t* out_tokens, int32_t* n_out, float* logits_out);
+
 #ifdef __cplusplus
 }
 #endif
