@@ -282,8 +282,8 @@ struct DeqPlanes { const uint8_t* p[CC_MAX_PLANES]; int64_t cols; };
 // megakernel phase descriptor (mega.cu); built by lazy.cu
 enum { MK_NORMQ = 0, MK_MATVEC = 1, MK_ATTN = 2, MK_ROWS = 3, MK_REDUCE = 4, MK_GATHER = 5, MK_ARGMAX = 6, MK_SAMPLE = 7 };
 struct MkPhase {
-    int type, wtype, write_back, next_matvec;
-    int xgpu, red_n, next_matvec2, spare; float* red_dst; const float* red_res;   // cross-GPU barrier after this phase ; REDUCE/GATHER phase operands   // next_matvec / next_matvec2: index of the next MATVEC phase and of the one after it (look-ahead prefetch), -1 if none
+    int type, wtype, write_back, next_matvec;  // next_matvec: index of the next MATVEC phase (mega.cu stages its norm weights early), -1 if none
+    int xgpu, red_n, spare1, spare; float* red_dst; const float* red_res;   // cross-GPU barrier after this phase ; REDUCE/GATHER phase operands
     // NORMQ (and the output quantisation of ATTN)
     float* x; float* orig; const float* norm_w; float eps; int n; ActQ8_0 act;
     int act_type, spare2;               // MATVEC: CC_Q8_0 (streaming phases) or CC_Q8_K (generic phases: K-quant weights)
@@ -304,10 +304,9 @@ int cc_launch_all_reduce(cc_device* dev, float* x, int64_t n, const float* resid
 int cc_launch_all_gather(cc_device* dev, const float* src, int64_t n, float* dst);
 extern "C" CC_API int cc_test_mega_barrier_floor(cc_device* dev, int n, float* us_per_phase);
 int cc_launch_mega(cc_device* dev, const MkPhase* phases_dev, int n_phases, const uint8_t* dyn_dev, unsigned* bar_dev, size_t smem_work, size_t smem_wstage,
-                   unsigned long long* prof, const CommDev* comm, bool generic, bool sample);
+                   unsigned long long* prof, bool sample);
 // mega_ring.cu: the same phase table run by the kernel whose weights arrive through a TMA-fed shared-memory ring
 int cc_mega_flags();
-bool cc_mega_ring_enabled();
 bool cc_mega_ring_phase_ok(const MkPhase& ph);
 int cc_mega_ring_at_ch(const MkPhase& ph);
 size_t cc_mega_ring_smem_for_phase(const MkPhase& ph);

@@ -359,7 +359,7 @@ struct Fuser {
             else P.steps.push_back([=](uint8_t*) { return cc_launch_all_gather(d, part, mrows, xdst); });
             MkPhase ph = {}; ph.type = xchg == 1 ? MK_REDUCE : MK_GATHER; ph.red_n = (int)mrows; ph.red_dst = xdst; ph.red_res = xres; P.phases.push_back(ph);
             if (!cc_comm_dev(dev) || cc_comm_is_nccl(dev)) P.mega_ok = false;      // NCCL baseline: graph of kernels + NCCL nodes (lazy mode 1)
-            if ((((mrows + dev->sm_count - 1) / dev->sm_count + 3) & ~(int64_t)3) > 512) P.mega_ok = false;   // one CTA's row block must fit the exchange stage (mega.cu MK_XSTAGE_ROWS)
+            if ((((mrows + dev->sm_count - 1) / dev->sm_count + 3) & ~(int64_t)3) > 512) P.mega_ok = false;   // one CTA's row block must fit the exchange stage (mega_phases.cuh MK_XSTAGE_ROWS)
         }
         for (size_t t = i; t < i + used; t++) q[t].done = true;
         return used;
@@ -557,7 +557,7 @@ struct Fuser {
     }
 
     // megakernel only: phases[at] = NORMQ (not write-back) directly followed by its single MATVEC consumer -> one MATVEC
-    // phase with a fused prologue (saves a grid barrier per merge; see mega.cu phase_matvec)
+    // phase with a fused prologue (saves a grid barrier per merge; see mega_ring.cu phase_matvec_ring)
     void merge_prologue(size_t at) {
         // [at] NORMQ, [at + 1] MATVEC, optionally [at + 2] the REDUCE / GATHER half of the matvec's exchange (sharded path)
         const bool tail = at + 3 == P.phases.size() && (P.phases[at + 2].type == MK_REDUCE || P.phases[at + 2].type == MK_GATHER);
@@ -691,18 +691,6 @@ int cc_lazy_flush(cc_device* dev) {
             cudaGraph_t graph = nullptr;
             GraphEntry ge;
             bool use_mega = dev->mega && P.mega_ok && !P.phases.empty();
-            // a phase whose working area cannot fit beside anything: CUDA-graph mode.  The register kernel's attention area (three 64-row
-            // chunk buffers + the score row) decides this for both persistent kernels: at head_dim 128, max_len 32 105 and up, and 28 009
-            // and up beside a Llama-2-7B norm + qkv phase (its 16 KB of norm weights are staged too).  Past 50 808 positions the fuser
-            // leaves attention to the per-op kernels (try_attention).
-            if (use_mega) {
-                size_t work = 0, wst = 0;
-                for (auto& ph : P.phases) {
-                    work = std::max(work, cc_mega_smem_for_phase(ph));
-                    if (ph.type == MK_MATVEC && ph.x && ph.norm_w) wst = std::max(wst, (size_t)ph.n * 4);
-                }
-                if (work + wst + 4096 > 227 * 1024) use_mega = false;
-            }
             // the megakernel runs ONE SAMPLE phase, after its phase loop (mega.cu): a table with more than one, or with anything queued
             // behind the sampler (several tokens submitted before one flush), runs in the CUDA-graph mode
             if (use_mega && P.mega_sample) {
@@ -710,28 +698,17 @@ int cc_lazy_flush(cc_device* dev) {
                 for (auto& ph : P.phases) n_sample += ph.type == MK_SAMPLE;
                 if (n_sample != 1 || P.phases.back().type != MK_SAMPLE) use_mega = false;
             }
-            if (use_mega) {       // phase table lives in device memory for the lifetime of the graph
-                int nxt = -1, nxt2 = -1;
-                for (int t = (int)P.phases.size() - 1; t >= 0; t--) {
-                    P.phases[t].next_matvec = nxt; P.phases[t].next_matvec2 = nxt2;
-                    if (P.phases[t].type == MK_MATVEC) { nxt2 = nxt; nxt = t; }
-                }
-                // weights through the shared-memory ring (mega_ring.cu) when every streaming MATVEC phase can be fed by bulk copies
-                bool ring = cc_mega_ring_enabled(), any_stream = false;
+            // A table with a streaming (Q8_0 / Q4_0) MATVEC phase runs mega_ring.cu when every such phase can be fed by bulk copies and the
+            // ring gets enough slots beside the working area; any other table runs mega.cu when its working area fits.  Otherwise: the
+            // CUDA-graph mode.  At head_dim 128 the attention phase's working area (the score row + its chunk buffers) decides this at
+            // long contexts; past 50 808 positions the fuser leaves attention to the per-op kernels (try_attention).
+            if (use_mega) {
+                bool stream = false, ring_ok = true;
                 for (auto& ph : P.phases) {
-                    if (ph.type == MK_MATVEC && ph.act_type != CC_Q8_K) any_stream = true;
-                    if (!cc_mega_ring_phase_ok(ph)) ring = false;
+                    if (ph.type == MK_MATVEC && ph.act_type != CC_Q8_K) stream = true;
+                    if (!cc_mega_ring_phase_ok(ph)) ring_ok = false;
                 }
-                P.mega_ring = ring && any_stream;
-                if (P.mega_ring) {              // is there room for a useful ring beside the working area?  else: the register-pipe kernel
-                    size_t work = 0, wst = 0; int slot = 0;
-                    for (auto& ph : P.phases) {
-                        work = std::max(work, cc_mega_ring_smem_for_phase(ph));
-                        if (ph.type == MK_MATVEC && ph.act_type == CC_Q8_K && ph.x && ph.norm_w) wst = std::max(wst, (size_t)ph.n * 4);
-                        if (ph.type == MK_MATVEC && ph.act_type != CC_Q8_K) slot = std::max(slot, ph.wtype == CC_Q8_0 ? 4352 : 2304);
-                    }
-                    if (!cc_mega_ring_fits(work, wst, slot, P.mega_generic)) P.mega_ring = false;
-                }
+                P.mega_ring = stream;
                 for (auto& ph : P.phases) {
                     if (P.mega_ring) {
                         P.mega_smem = std::max(P.mega_smem, cc_mega_ring_smem_for_phase(ph));
@@ -742,6 +719,15 @@ int cc_lazy_flush(cc_device* dev) {
                         P.mega_smem = std::max(P.mega_smem, cc_mega_smem_for_phase(ph));
                         if (ph.type == MK_MATVEC && ph.x && ph.norm_w) P.mega_wstage = std::max(P.mega_wstage, (size_t)ph.n * 4);
                     }
+                }
+                if (P.mega_ring) use_mega = ring_ok && cc_mega_ring_fits(P.mega_smem, P.mega_wstage, P.ring_slot, P.mega_generic);
+                else use_mega = P.mega_smem + P.mega_wstage + 4096 <= 227 * 1024;
+            }
+            if (use_mega) {       // phase table lives in device memory for the lifetime of the graph
+                int nxt = -1;
+                for (int t = (int)P.phases.size() - 1; t >= 0; t--) {
+                    P.phases[t].next_matvec = nxt;
+                    if (P.phases[t].type == MK_MATVEC) nxt = t;
                 }
                 if (cudaMalloc(&ge.phases_dev, P.phases.size() * sizeof(MkPhase)) != cudaSuccess ||
                     cudaMemcpy(ge.phases_dev, P.phases.data(), P.phases.size() * sizeof(MkPhase), cudaMemcpyHostToDevice) != cudaSuccess)
@@ -755,7 +741,7 @@ int cc_lazy_flush(cc_device* dev) {
                 if (!use_mega) rc = run_steps(lz->dyn_dev);
                 else if (P.mega_ring) rc = cc_launch_mega_ring(dev, ge.phases_dev, (int)P.phases.size(), lz->dyn_dev, lz->bar_dev, P.mega_smem, P.mega_wstage, prof, cc_comm_dev(dev),
                                                                P.mega_generic, P.mega_sample, P.ring_slot, P.ring_at_ch, cc_mega_flags());
-                else rc = cc_launch_mega(dev, ge.phases_dev, (int)P.phases.size(), lz->dyn_dev, lz->bar_dev, P.mega_smem, P.mega_wstage, prof, cc_comm_dev(dev), P.mega_generic, P.mega_sample);
+                else rc = cc_launch_mega(dev, ge.phases_dev, (int)P.phases.size(), lz->dyn_dev, lz->bar_dev, P.mega_smem, P.mega_wstage, prof, P.mega_sample);
                 e = cudaStreamEndCapture(dev->stream, &graph);
                 if (!rc && e != cudaSuccess) rc = cc_fail(dev, CC_ERR_CUDA, "lazy: end capture: %s", cudaGetErrorString(e));
             }

@@ -1,5 +1,5 @@
-// mega_phases.cuh -- device code shared by the two persistent decode kernels (mega.cu: weights through registers,
-// mega_ring.cu: weights through a TMA-fed shared-memory ring): grid barrier, phase bodies other than the streaming MATVEC.
+// mega_phases.cuh -- device code shared by the two persistent decode kernels (mega.cu: tables without a Q8_0 / Q4_0 phase,
+// mega_ring.cu: Q8_0 / Q4_0 weights through a TMA-fed shared-memory ring): grid barrier, phase bodies other than the streaming MATVEC.
 // The including file defines MK_SYNC() -- the barrier of the 512 compute threads of a CTA (mega.cu: the whole CTA; mega_ring.cu:
 // named barrier 1, the producer warp stays out of it) -- before including this header.
 #pragma once
@@ -33,7 +33,7 @@ __device__ __forceinline__ void st_release_u32(unsigned* p, unsigned v) { asm vo
 // Split grid barrier (tools/barrier_floor.py times it against a two-level acq_rel-atomic version and relaxed polling + fence):
 //   arrive : bar.sync, then ONE thread does a fire-and-forget red.release.gpu.add on a flat monotonic counter
 //            (the release publishes the CTA's phase output; that thread never issues prefetch loads);
-//   ...      the other warps may already issue the next phase's weight prefetch;
+//   ...      the other warps may already request the next phase's norm weights (mega.cu);
 //   wait   : CTA 0 watches the counter reach (gen+1) * nblocks and publishes the generation word; everyone else spins on
 //            the generation with ld.acquire; then bar.sync.
 // Layout (u32 words on separate 128-byte lines): [0] arrival counter, [32] generation.  Both are monotonic ACROSS launches (u32
@@ -163,54 +163,10 @@ static __device__ void phase_normq(const MkPhase& ph, float* s_red) {
     for (int b = gw + 4 * tw; b < nb; b += tw) do_block(b, ldcg_f(x + b * 32 + lane));
 }
 
-// ---- MATVEC phase: the body of matvec_stream_kernel (see matvec_stream.cu for the design notes) -------------------------
+// ---- streaming MATVEC phase (mega_ring.cu): the body of matvec_stream_kernel (see matvec_stream.cu for the design notes) ----------
 __device__ __forceinline__ int mk_dp16(const int4& w, const int4& a) {
     return __dp4a(w.x, a.x, __dp4a(w.y, a.y, __dp4a(w.z, a.z, __dp4a(w.w, a.w, 0))));
 }
-typedef KSeg MkSeg;                                                  // (Q4_0 leaves b unused)
-static_assert(MK_SEG == 4, "KSeg holds 4 groups");
-struct MkRowPtr { const uint8_t* q; const uint16_t* d; };
-
-template <int TYPE>
-__device__ __forceinline__ void mk_seg_load(MkSeg& S, const MkRowPtr& p, int seg, int nb, int GR, int last_half_off, int lane, bool valid) {
-    constexpr int GB = TYPE == CC_Q8_0 ? 1024 : 512;
-    const uint8_t* q = p.q + (size_t)seg * (MK_SEG * GB);
-    const uint16_t* d = p.d + seg * (MK_SEG * 32);
-#pragma unroll
-    for (int g = 0; g < MK_SEG; g++) {
-        const int gi = seg * MK_SEG + g;
-        const bool on = valid && (gi * 32 + lane < nb);
-        if constexpr (TYPE == CC_Q8_0) {
-            const int hoff = gi == GR - 1 ? last_half_off : 512;
-            if (on) { S.a[g] = ld_stream_16(q + g * GB); S.b[g] = ld_stream_16(q + g * GB + hoff); S.s[g] = d[g * 32]; }
-            else { S.a[g] = make_int4(0, 0, 0, 0); S.b[g] = S.a[g]; S.s[g] = 0; }
-        } else {
-            if (on) { S.a[g] = ld_stream_16(q + g * GB); S.s[g] = d[g * 32]; }
-            else { S.a[g] = make_int4(0, 0, 0, 0); S.s[g] = 0; }
-        }
-    }
-}
-template <int TYPE>
-__device__ __forceinline__ float mk_seg_dot(const MkSeg& S, int seg, const int4* aq_l, const float* ad_l, const int* as_l) {
-    float acc = 0.0f;
-    const int4* aq = aq_l + seg * (MK_SEG * 64);
-    const float* ad = ad_l + seg * (MK_SEG * 32);
-#pragma unroll
-    for (int g = 0; g < MK_SEG; g++) {
-        if constexpr (TYPE == CC_Q8_0) {
-            int sumi = mk_dp16(S.a[g], aq[g * 64]) + mk_dp16(S.b[g], aq[g * 64 + 1]);
-            acc += (float)sumi * h2f_bits(S.s[g]) * ad[g * 32];
-        } else {
-            const int4 w = S.a[g];
-            int4 lo = make_int4(w.x & 0x0F0F0F0F, w.y & 0x0F0F0F0F, w.z & 0x0F0F0F0F, w.w & 0x0F0F0F0F);
-            int4 hi = make_int4((w.x >> 4) & 0x0F0F0F0F, (w.y >> 4) & 0x0F0F0F0F, (w.z >> 4) & 0x0F0F0F0F, (w.w >> 4) & 0x0F0F0F0F);
-            int sumi = mk_dp16(lo, aq[g * 64]) + mk_dp16(hi, aq[g * 64 + 1]) - 8 * as_l[(seg * MK_SEG + g) * 32];
-            acc += (float)sumi * h2f_bits(S.s[g]) * ad[g * 32];
-        }
-    }
-    return acc;
-}
-
 __device__ __forceinline__ void mbar_init(unsigned mbar, unsigned count) { asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(mbar), "r"(count) : "memory"); }
 __device__ __forceinline__ void mbar_wait(unsigned mbar, unsigned parity) {
     asm volatile(
@@ -218,87 +174,33 @@ __device__ __forceinline__ void mbar_wait(unsigned mbar, unsigned parity) {
         "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
         "@!p bra MK_WAIT_%=;\n}\n" ::"r"(mbar), "r"(parity) : "memory");
 }
-// look-ahead arguments of a coming MATVEC phase, fetched one word per thread at phase start (64 threads per slot)
-struct MkNext { StreamArgs mv; int wtype; int norm_n; const float* norm_w; };
-static_assert(sizeof(StreamArgs) % 4 == 0 && sizeof(StreamArgs) / 4 + 4 <= 64, "MkNext fetch layout: 64 threads per look-ahead slot");
-struct MkPipe { MkSeg buf0, buf1; };      // register stages of the weight stream, live across phases and barriers
-
 // (Tried and removed in round 2: an L2 look-ahead of each warp's coming rows -- cp.async.bulk.prefetch.L2 as
 // well as per-lane prefetch.global.L2 -- made the token SLOWER: a bulk prefetch request occupies its issuing thread for
 // a long time, line prefetches cost issue slots at the phase boundary, and the phase bodies already stream at HBM speed.)
 
-// geometry of one MATVEC phase for this warp
-struct MkGeo {
-    int nb, GR, NSEG, U, last_half_off, gw, TW, rpc;
-    bool pair;
-};
-__device__ __forceinline__ MkGeo mk_geo(const StreamArgs& A) {
-    MkGeo g;
-    const int warp = threadIdx.x >> 5;
-    g.nb = A.k >> 5; g.GR = (g.nb + 31) >> 5; g.NSEG = (g.GR + MK_SEG - 1) / MK_SEG;
-    // warp-major numbering: when rows do not divide by the warp count, every SM gets the same mix of k- and (k+1)-row warps
-    // (CTA-major numbering left the last SMs with half the work of the first ones)
-    g.gw = warp * gridDim.x + blockIdx.x; g.TW = gridDim.x * MK_WARPS;
-    g.pair = A.epilogue == 2;
-    const StreamMats& M = A.mats;
-    const int m_cat = g.pair ? M.m[0] : M.m[0] + (M.n > 1 ? M.m[1] : 0) + (M.n > 2 ? M.m[2] : 0);
-    int n_rows = g.gw < m_cat ? (m_cat - g.gw + g.TW - 1) / g.TW : 0;
-    g.rpc = 0;
-    if (A.epilogue == 3) {
-        // exchange phases: every CTA owns ONE contiguous block of rows (rpc rows, a multiple of 4), warp w takes the rows w, w + 16, ...
-        // of the block -- so the CTA's partial results are one contiguous run of floats and go to each peer as a single coalesced store
-        g.rpc = (((m_cat + (int)gridDim.x - 1) / (int)gridDim.x) + 3) & ~3;
-        const int first = (int)blockIdx.x * g.rpc;
-        const int cnt = min(g.rpc, max(0, m_cat - first));
-        g.gw = first + warp; g.TW = MK_WARPS;
-        n_rows = warp < cnt ? (cnt - warp + MK_WARPS - 1) / MK_WARPS : 0;
-    }
-    g.U = (g.pair ? 2 * n_rows : n_rows) * g.NSEG;
-    g.last_half_off = 16 * (g.nb - 32 * (g.GR - 1));
-    return g;
-}
-template <int TYPE>
-__device__ __forceinline__ MkRowPtr mk_vrow_ptr(const StreamMats& M, const MkGeo& g, int i, int lane) {
-    constexpr int BB = TYPE == CC_Q8_0 ? 32 : 16;
-    int mat = 0, r;
-    if (g.pair) { mat = i & 1; r = g.gw + (i >> 1) * g.TW; }
-    else {
-        r = g.gw + i * g.TW;
-        if (M.n > 1 && r >= M.m[0]) { r -= M.m[0]; mat = 1; if (M.n > 2 && r >= M.m[1]) { r -= M.m[1]; mat = 2; } }
-    }
-    const uint8_t* q0 = mat == 0 ? M.qs[0] : mat == 1 ? M.qs[1] : M.qs[2];
-    const uint16_t* d0 = mat == 0 ? M.d[0] : mat == 1 ? M.d[1] : M.d[2];
-    MkRowPtr p;
-    p.q = q0 + (size_t)r * g.nb * BB + lane * 16;
-    p.d = d0 + (size_t)r * CC_D_STRIDE(g.nb) + lane;
-    return p;
-}
-
 // ---- generic MATVEC phase: K-quant weights (Q2_K .. Q6_K, Q8_K) against the Q8_K-quantised activation ---------------------------
-// Same shape as phase_matvec -- fused prologue ([rms_norm * w] + activation quantisation, recomputed by every CTA), rows dealt
-// warp-major, the same epilogues -- but the row dot is the type's T::row_dot of vecdot.cuh (what the eager matvec_kernel runs, hence
-// the same bits) and the weights are not pipelined through registers across phase boundaries.
+// Same shape as the streaming phase of mega_ring.cu -- fused prologue ([rms_norm * w] + activation quantisation, recomputed by every
+// CTA), the same epilogues -- but the row dot is the type's T::row_dot of vecdot.cuh (what the eager matvec_kernel runs, hence the
+// same bits) and the weights are loaded by the computing warp itself.
 // shared memory: qs [k] | d [k/256] | bsums [k/16] (TKBase) | reduction scratch | f32 x
 __device__ __forceinline__ int mk_generic_sx_offset(int k) { return ((TKBase::smem_bytes(k) + 15) & ~15) + 256; }
-// __noinline__ (ring kernel): the K-quant row dots are register-hungry; as a called function they get their own allocation instead of pushing spills into
-// the streaming phases of the same kernel (every phase of the Q4_0 body was slower in the instantiation that carries
-// the generic code inline).
-// MK_GENERIC_NOINLINE (mega_ring.cu): as a called function with registers of its own.  In mega.cu the phase stays inline and borrows the
-// weight pipe's registers: there the pipe would have to be saved around every call.
+// __noinline__ in the ring kernel (MK_GENERIC_NOINLINE, mega_ring.cu): the K-quant row dots are register-hungry; as a called function they
+// get their own allocation instead of pushing spills into the streaming phases of the same kernel (every phase of the Q4_0 body was slower
+// in the instantiation that carries the generic code inline).  mega.cu has no streaming phase: there the phase stays inline, and the two
+// weight segments in flight live in the caller's KSeg pair (MK_GENERIC_SEGS), one pair for all six inlined instantiations -- a pair of
+// their own each costs mega_kernel a 480-byte stack frame and 848 / 1320 bytes of spills instead of 104 and 208 / 292.
 #ifndef MK_GENERIC_NOINLINE
 #define MK_GENERIC_NOINLINE 0
 #endif
 #if MK_GENERIC_NOINLINE
 #define MK_GENERIC_ATTR __noinline__
-#define MK_GENERIC_PIPE_PARAM
-#define MK_GENERIC_PIPE_ARG
+#define MK_GENERIC_SEGS
 #else
 #define MK_GENERIC_ATTR
-#define MK_GENERIC_PIPE_PARAM MkPipe& P,
-#define MK_GENERIC_PIPE_ARG pipe,
+#define MK_GENERIC_SEGS , KSeg& S0, KSeg& S1
 #endif
 template <class T>
-static __device__ MK_GENERIC_ATTR void phase_matvec_generic(const MkPhase& ph, uint8_t* smem, float* s_w, bool w_staged, bool x_staged, const uint16_t* exp_lut, MK_GENERIC_PIPE_PARAM unsigned long long* stamp1) {
+static __device__ MK_GENERIC_ATTR void phase_matvec_generic(const MkPhase& ph, uint8_t* smem, float* s_w, bool w_staged, bool x_staged, const uint16_t* exp_lut, unsigned long long* stamp1 MK_GENERIC_SEGS) {
     const StreamArgs& A = ph.mv;
     const StreamMats& M = A.mats;
     const int k = A.k;
@@ -340,7 +242,8 @@ static __device__ MK_GENERIC_ATTR void phase_matvec_generic(const MkPhase& ph, u
     }
     MK_SYNC();
     if (stamp1) *stamp1 = globaltimer_ns();
-    // rows: the same warp-major dealing and epilogues as phase_matvec
+    // rows dealt warp-major: when rows do not divide by the warp count, every SM gets the same mix of k- and (k+1)-row warps
+    // (CTA-major numbering left the last SMs with half the work of the first ones)
     const int gw = warp * gridDim.x + blockIdx.x, TW = gridDim.x * MK_WARPS;
     const bool pair = A.epilogue == 2;
     const int m_cat = pair ? M.m[0] : M.m[0] + (M.n > 1 ? M.m[1] : 0) + (M.n > 2 ? M.m[2] : 0);
@@ -396,9 +299,6 @@ static __device__ MK_GENERIC_ATTR void phase_matvec_generic(const MkPhase& ph, u
         const int U = n_vrows * NSEG;
 #if MK_GENERIC_NOINLINE
         KSeg S0, S1;
-#else
-        KSeg& S0 = P.buf0;                                                   // the weight pipe's registers (no streaming look-ahead is pending: caller)
-        KSeg& S1 = P.buf1;
 #endif
         int x0[4] = {0, 0, 0, 0}, x1[4] = {0, 0, 0, 0};
         int l_i = 0, l_seg = 0;
@@ -666,11 +566,9 @@ static __device__ void phase_reduce(const MkPhase& ph, const CommDev& comm, unsi
 
 
 #define MK_PROF_SLOTS 8      // developer profiling: u64 stamps per phase (CTA 0 / thread 0): 0 start, 1 activation ready, 2 rows done, 3 arrived, 4 x staged, 5 rms known
-// look-ahead arguments of the next two MATVEC phases, fetched one word per thread at phase start
 
-// flags: 1 look-ahead weight prefetch | 4 norm weights staged before the barrier | 8 every CTA polls the arrival counter |
-//        32 per-warp early look-ahead | 64 x of the next fused prologue requested right after the barrier
-#define MK_F_LOOK 1
+// flags: 4 norm weights staged before the barrier | 8 every CTA polls the arrival counter | 64 x of the next fused prologue requested
+//        right after the barrier (4 and 64: mega.cu)
 #define MK_F_WSTAGE 4
 #define MK_F_POLLCNT 8
 #define MK_F_SYSFENCE 256      // exchange phases: a system-scope fence in EVERY CTA before its arrival (not needed, see grid_barrier_arrive;
@@ -679,6 +577,3 @@ static __device__ void phase_reduce(const MkPhase& ph, const CommDev& comm, unsi
 #define MK_F_XEARLY 64         // the f32 row of the next fused prologue is requested (cp.async) right after the barrier opens
 #define MK_F_KVPF 2048         // ring kernel: the producer warps prefetch the attention phase's cached K / V rows into L2 one phase ahead
 #define MK_F_RPAIR 1024        // ring kernel: consumer warps take two units per round (shared activation loads; the slots are held twice as long)
-#define MK_F_RING 512          // weights through the TMA-fed shared-memory ring of mega_ring.cu (when every streaming phase qualifies)
-#define MK_F_EARLY 32          // a warp requests its first segments of the next MATVEC phase as soon as IT has finished its rows
-#define MK_TYPE_CALL(T, CALL_Q8, CALL_Q4) do { if ((T) == CC_Q8_0) { CALL_Q8; } else { CALL_Q4; } } while (0)

@@ -1,15 +1,15 @@
 // mega_ring.cu -- the persistent decode kernel with the weight stream decoupled from the compute warps.
 //
-// Why: in mega.cu every warp alternates "issue the loads of a segment" and "consume a segment"; at a phase
-// boundary (slowest warp -> grid barrier -> activation prologue) no warp issues loads, so only the 2 look-ahead segments per
-// warp cover the bubble and HBM idles for the rest.  Weights are immutable, so nothing forces the weight stream to follow the phase order of the compute:
+// Why: when every warp alternates "issue the loads of a segment" and "consume a segment" (weights through registers, as in
+// matvec_stream.cu), no warp issues loads at a phase boundary (slowest warp -> grid barrier -> activation prologue), so at most the
+// segments a warp requested ahead cover the bubble and HBM idles for the rest.  Weights are immutable, so nothing forces the weight stream to follow the phase order of the compute:
 //   * warps 16-19 of every CTA are PRODUCERS: their threads walk the phase table on their own, ahead of the compute warps, and
 //     issue cp.async.bulk (TMA) copies of row segments (4 groups of 32 blocks: 4096 B of Q8_0 quants + 256 B of f16 scales) into a
 //     ring of shared-memory slots -- as many as fit beside the per-phase working area (~37-47 slots = 160-200 KB per SM, 24-30 MB
 //     per GPU in flight or landed).  It never waits for a barrier or an activation: whenever a slot is free the next segment of
 //     this CTA's rows -- of this phase or any later one -- is already being fetched.
 //   * warps 0-15 are CONSUMERS: same row dealing (row r -> CTA r % gridDim.x, rows of a CTA -> its warps round-robin), same per-lane
-//     block order, same arithmetic as mega.cu / matvec_stream.cu (bit-identical results), but a segment is read from the ring with
+//     block order, same arithmetic as matvec_stream.cu (bit-identical results), but a segment is read from the ring with
 //     LDS.128 after waiting on the slot's "full" mbarrier, and the slot is handed back through its "empty" mbarrier.  No weight
 //     registers live across phases -> no register pipe, no look-ahead bookkeeping, 96 registers are enough.
 //   * the activation prologue works from registers (x row: <= 4 float4 per thread straight from L2) instead of a shared-memory
@@ -43,11 +43,6 @@ __device__ __forceinline__ bool mr_try_wait(unsigned bar, unsigned parity) {
     asm volatile("{\n.reg .pred p;\nmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\nselp.u32 %0, 1, 0, p;\n}\n" : "=r"(ok) : "r"(bar), "r"(parity) : "memory");
     return ok != 0;
 }
-__device__ __forceinline__ bool mr_test_wait(unsigned bar, unsigned parity) {
-    unsigned ok;
-    asm volatile("{\n.reg .pred p;\nmbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\nselp.u32 %0, 1, 0, p;\n}\n" : "=r"(ok) : "r"(bar), "r"(parity) : "memory");
-    return ok != 0;
-}
 // Slot hand-back: the consumer stores (entry number + 1) into the slot's "done" word (release), the producer polls it (acquire) for
 // exactly the previous tenant's number -- an mbarrier parity could not tell one lap from two.  `dep` ties the store behind the
 // arithmetic that consumed the slot's data.
@@ -71,7 +66,7 @@ __device__ __forceinline__ MrGeo mr_geo(const StreamArgs& A) {
     g.pair = A.epilogue == 2;
     const StreamMats& M = A.mats;
     g.m_cat = g.pair ? M.m[0] : M.m[0] + (M.n > 1 ? M.m[1] : 0) + (M.n > 2 ? M.m[2] : 0);
-    if (A.epilogue == 3) {             // exchange phases: one contiguous block of rows per CTA (mega.cu mk_geo)
+    if (A.epilogue == 3) {             // exchange phases: one contiguous block of rows per CTA, so its partial rows go to each peer as one run
         const int rpc = (((g.m_cat + (int)gridDim.x - 1) / (int)gridDim.x) + 3) & ~3;
         g.first = (int)blockIdx.x * rpc; g.stride = 1;
         g.n_units = min(rpc, max(0, g.m_cat - g.first));
@@ -216,26 +211,6 @@ __device__ __forceinline__ void mr_wait_full(const MrCons& RC, unsigned slot, un
     }
 }
 
-template <int TYPE>
-__device__ __forceinline__ void mr_seg_lds(MkSeg& S, const uint8_t* sp, int seg, int nb, int GR, int last_half_off, int lane) {
-    constexpr int GB = TYPE == CC_Q8_0 ? 1024 : 512;
-    const uint8_t* q = sp + lane * 16;
-    const uint16_t* d = (const uint16_t*)(sp + MK_SEG * GB) + lane;
-#pragma unroll
-    for (int g = 0; g < MK_SEG; g++) {
-        const int gi = seg * MK_SEG + g;
-        const bool on = gi * 32 + lane < nb;
-        if constexpr (TYPE == CC_Q8_0) {
-            const int hoff = gi == GR - 1 ? last_half_off : 512;
-            if (on) { S.a[g] = *(const int4*)(q + g * GB); S.b[g] = *(const int4*)(q + g * GB + hoff); S.s[g] = d[g * 32]; }
-            else { S.a[g] = make_int4(0, 0, 0, 0); S.b[g] = S.a[g]; S.s[g] = 0; }
-        } else {
-            if (on) { S.a[g] = *(const int4*)(q + g * GB); S.s[g] = d[g * 32]; }
-            else { S.a[g] = make_int4(0, 0, 0, 0); S.s[g] = 0; }
-        }
-    }
-}
-
 // Activation quants in shared memory, per group of 32 blocks: the 16-byte first halves of all 32 blocks, then the second halves (the layout of
 // the Q8_0 weight plane) -- lane l reads block 32 g + l with two conflict-free LDS.128 (block-major, 32 bytes apart, is a 2-way bank conflict:
 // 64 instead of 32 shared-memory wavefronts per segment, and the ring's throughput is bounded by shared-memory bandwidth)
@@ -250,7 +225,7 @@ __device__ __forceinline__ int mr_act_int4(int i) {           // i = 16-byte ind
 
 // One segment (4 groups) of TWO rows against the same activation segment: the activation quants and scales are read once for both rows
 // (shared-memory wavefronts per 4352-byte entry: 34 TMA write + 34 weight read + 16 activation, against 64 + for one row at a time).
-// Per row the arithmetic is mk_seg_dot's, term by term (bit-identical to matvec_stream.cu).
+// Per row the arithmetic is matvec_stream.cu's, term by term (bit-identical).
 template <int TYPE>
 __device__ __forceinline__ void mr_dot2(const uint8_t* spA, const uint8_t* spB, int seg, int nb, int GR, int last_half_off, int lane,
                                         const int4* aq_l, const float* ad_l, const int* as_l, float& partA, float& partB) {
@@ -427,7 +402,7 @@ __device__ void phase_matvec_ring(const MkPhase& ph, uint8_t* smem, const uint16
     const int4* aq_l = (const int4*)s_q + lane;
     const float* ad_l = s_d + lane;
     const int* as_l = s_s + lane;
-    // Epilogues that need a value from memory (the residual, or the exp LUT entry of silu) are finished one round later (mega.cu); lane 0 only
+    // Epilogues that need a value from memory (the residual, or the exp LUT entry of silu) are finished one round later, so the warp never stalls an L2 round trip; lane 0 only
     float pend_a[2] = {0.0f, 0.0f}, pend_b[2] = {0.0f, 0.0f}, pend_res[2] = {0.0f, 0.0f};
     unsigned short pend_lut[2] = {0, 0};
     int pend_row[2] = {-1, -1};
@@ -505,7 +480,7 @@ __device__ void phase_matvec_ring(const MkPhase& ph, uint8_t* smem, const uint16
     RC.ent_base += (unsigned)(g.n_units * g.E);
     if (A.epilogue == 3) {
         // the CTA's block of partial rows -> slot[rank] of every GPU's exchange window: warp p serves peer p with coalesced 16-byte
-        // NVLink stores (mega.cu)
+        // NVLink stores instead of one 4-byte store per row and peer
         MK_SYNC();
         if (warp < comm.world) {
             const size_t off = ((size_t)((xseq + 1u) & 1u) * CC_COMM_MAX_RANKS + comm.rank) * CC_COMM_MAX_ELEMS + g.first;
@@ -571,12 +546,12 @@ __global__ void __launch_bounds__(MR_THREADS, 1) mega_ring_kernel(const MkPhase*
         case MK_MATVEC:
             if (GEN && s_ph.act_type == CC_Q8_K) {
                 switch (s_ph.wtype) {
-                case CC_Q2_K: phase_matvec_generic<TQ2_K>(s_ph, work, s_w, false, false, exp_lut, MK_GENERIC_PIPE_ARG st1); break;
-                case CC_Q3_K: phase_matvec_generic<TQ3_K>(s_ph, work, s_w, false, false, exp_lut, MK_GENERIC_PIPE_ARG st1); break;
-                case CC_Q4_K: phase_matvec_generic<TQ45_K<false>>(s_ph, work, s_w, false, false, exp_lut, MK_GENERIC_PIPE_ARG st1); break;
-                case CC_Q5_K: phase_matvec_generic<TQ45_K<true>>(s_ph, work, s_w, false, false, exp_lut, MK_GENERIC_PIPE_ARG st1); break;
-                case CC_Q6_K: phase_matvec_generic<TQ6_K>(s_ph, work, s_w, false, false, exp_lut, MK_GENERIC_PIPE_ARG st1); break;
-                default: phase_matvec_generic<TQ8_K>(s_ph, work, s_w, false, false, exp_lut, MK_GENERIC_PIPE_ARG st1); break;
+                case CC_Q2_K: phase_matvec_generic<TQ2_K>(s_ph, work, s_w, false, false, exp_lut, st1); break;
+                case CC_Q3_K: phase_matvec_generic<TQ3_K>(s_ph, work, s_w, false, false, exp_lut, st1); break;
+                case CC_Q4_K: phase_matvec_generic<TQ45_K<false>>(s_ph, work, s_w, false, false, exp_lut, st1); break;
+                case CC_Q5_K: phase_matvec_generic<TQ45_K<true>>(s_ph, work, s_w, false, false, exp_lut, st1); break;
+                case CC_Q6_K: phase_matvec_generic<TQ6_K>(s_ph, work, s_w, false, false, exp_lut, st1); break;
+                default: phase_matvec_generic<TQ8_K>(s_ph, work, s_w, false, false, exp_lut, st1); break;
                 }
                 break;
             }
@@ -649,8 +624,8 @@ size_t cc_mega_ring_smem_for_phase(const MkPhase& ph) {
     if (ph.type == MK_SAMPLE) return SMP_SMEM_BYTES;
     return 1024;
 }
-// slots the ring would get beside a working area of `smem_work` (+ `smem_wstage`) bytes; lazy.cu falls back to the register-pipe kernel
-// (mega.cu) below MR_MIN_SLOTS -- e.g. a 32 K-token context, whose attention phase needs 128 KB for the score row alone
+// slots the ring would get beside a working area of `smem_work` (+ `smem_wstage`) bytes; lazy.cu runs the table in the CUDA-graph mode
+// below MR_MIN_SLOTS -- e.g. a 32 K-token context, whose attention phase needs 128 KB for the score row alone
 #define MR_MIN_SLOTS 12
 static size_t mr_ring_off(size_t smem_work, size_t smem_wstage) { return ((((smem_work + 15) & ~(size_t)15) + smem_wstage) + 127) & ~(size_t)127; }
 int cc_mega_ring_slots(size_t smem_work, size_t smem_wstage, int slot_bytes, bool generic) {

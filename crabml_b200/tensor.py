@@ -139,7 +139,7 @@ class CudaTensorDevice:
                 "host_us_record": a[4] / 1e3, "host_us_fuse": a[5] / 1e3, "host_us_submit": a[6] / 1e3, "ops": a[7]}
 
     def mega_variant(self) -> int:
-        """0 none yet, 1 mega_kernel (register pipe), 2 mega_ring_kernel (TMA-fed shared-memory ring)."""
+        """0 none yet, 1 mega_kernel (tables without a Q8_0 / Q4_0 matvec), 2 mega_ring_kernel (TMA-fed shared-memory ring)."""
         return int(self.lib.cc_lazy_mega_variant(self.handle))
 
     def dump_debug_tensor(self, name):                              # cpu_device.rs:96-98

@@ -71,7 +71,7 @@ typedef struct cc_device_options {
     int32_t device_ordinal;        /* CUDA device index */
     int32_t debug_named_tensors;   /* with_name() snapshots tensors to host (cpu_tensor.rs:232-241) */
     int32_t lazy;                  /* 0 = eager: one launch per trait call; 1 = record + fuse + CUDA-graph replay;
-                                      2 = as 1, and a fused token runs as ONE persistent kernel (mega.cu) */
+                                      2 = as 1, and a fused token runs as ONE persistent kernel (mega_ring.cu, mega.cu) */
     int32_t exact_order;           /* 1 = verification mode: every reduction in the reference's scalar order,
                                       bit-identical to the scalar CPU path (slow; see csrc/exact.cu) */
     uint64_t pool_bytes;           /* activation pool size hint, 0 = default */
@@ -92,8 +92,8 @@ CC_API int cc_lazy_stats(cc_device* dev, uint64_t* out8);
 CC_API int cc_test_mega_barrier_floor(cc_device* dev, int n, float* us_per_phase);
 /* developer profiling (CRABML_MEGA_PROF=1): phase start timestamps of the last megakernel run */
 CC_API int cc_lazy_mega_profile(cc_device* dev, unsigned long long* ts, int* types, int cap, int* n_out);
-/* which persistent kernel ran the last megakernel flush: 0 none yet, 1 mega_kernel (weights through registers, mega.cu),
- * 2 mega_ring_kernel (weights through the TMA-fed shared-memory ring, mega_ring.cu) */
+/* which persistent kernel ran the last megakernel flush: 0 none yet, 1 mega_kernel (tables without a Q8_0 / Q4_0 matvec, mega.cu),
+ * 2 mega_ring_kernel (Q8_0 / Q4_0 weights through the TMA-fed shared-memory ring, mega_ring.cu) */
 CC_API int cc_lazy_mega_variant(cc_device* dev);
 /* counters: kernels launched by this library since creation (bench.py "gpu_launches") */
 CC_API uint64_t cc_device_launch_count(cc_device* dev);

@@ -1,6 +1,6 @@
-"""Worker of tests/test_gpu_sampling.py::test_fast_modes_sample_bit_identical_ids: sampled generation (temperature / top-p on the
-device) with the execution mode and megakernel flag word of its environment (CRABML_MEGA_FLAGS is read once per process); saves the
-ids, the exported logits and the persistent kernel that ran.  The prompt is one token, so every flush of the run contains the sampler."""
+"""Worker of tests/test_gpu_sampling.py::test_fast_modes_sample_bit_identical_ids_on_ring_and_k_quant_kernels: sampled generation
+(temperature / top-p on the device) in one execution mode; saves the ids, the exported logits and the persistent kernel that ran.
+The prompt is one token, so every flush of the run contains the sampler."""
 import sys
 
 import numpy as np
@@ -32,11 +32,14 @@ def main():
         conf, w, _ = R.load_gguf(gguf, dev)
         return conf, w, 128
 
-    def l7b(dev):          # one Llama-2-7B-shaped layer on bench.py's synthetic Q8_0 weights
-        conf = R.LlamaConfig(32, 32, 1, 4096, 11008, 4096, 32000, 1e-5, 128)
-        return conf, R.synthetic_weights(dev, conf, oc.Q8_0, oc.Q8_0, seed=7), 80
+    def l7b(wt, ct):       # one Llama-2-7B-shaped layer on bench.py's synthetic weights
+        def build(dev):
+            conf = R.LlamaConfig(32, 32, 1, 4096, 11008, 4096, 32000, 1e-5, 128)
+            return conf, R.synthetic_weights(dev, conf, wt, ct, seed=7), 80
+        return build
     res["tiny_ids"], res["tiny_logits"], res["tiny_variant"] = run(lazy, tiny, 96, 0.8, 0.9, 1234)
-    res["l7b_ids"], res["l7b_logits"], res["l7b_variant"] = run(lazy, l7b, 66, 1.0, 0.9, 99)
+    res["l7b_ids"], res["l7b_logits"], res["l7b_variant"] = run(lazy, l7b(oc.Q8_0, oc.Q8_0), 66, 1.0, 0.9, 99)
+    res["l7bk_ids"], res["l7bk_logits"], res["l7bk_variant"] = run(lazy, l7b(oc.Q4_K, oc.Q6_K), 66, 1.0, 0.9, 99)
     np.savez(out, **res)
 
 

@@ -15,8 +15,9 @@ side of every chunk and buffer boundary, and at contexts where the fuser switche
    CTA wrote into the cache and which must now come back through a bulk copy.
 2. Random data at long KV lengths: every mode equals the eager kernels bit for bit, exact_order mode equals the CPU oracle bit for
    bit, and the megakernel is within a derived bound of an f64 softmax attention with the true exp.
-3. The context-length switches of lazy mode 2 (ring kernel -> register kernel -> CUDA graph of fused kernels), found by probing,
-   and contexts past what the single-pass fused kernel can hold."""
+3. The context-length switches of lazy mode 2, found by probing: a flush with a Q8_0 matvec goes from the ring kernel to the CUDA
+   graph of fused kernels, attention alone from the register kernel to the graph; and contexts past what the single-pass fused
+   kernel can hold."""
 import numpy as np
 import pytest
 
@@ -340,10 +341,12 @@ def test_random_attention_step_modes_oracle_and_f64(kv_len, f16, hd, n_heads, n_
 
 
 # ---- part 4: the context-length switches -------------------------------------------------------------------------------------------
-# Two flush shapes, both with head_dim 128: the ring kernel's flush of part 1 with 8 heads, and the same attention with 32 query heads
+# Three flush shapes, all with head_dim 128: the ring kernel's flush of part 1 with 8 heads; the same attention with 32 query heads
 # after the qkv phase of a Llama-2-7B layer (rms_norm * w of a 4096 row, three Q8_0 4096 x 4096 matvecs: its norm weights are staged in
-# shared memory beside the working area, as in the real layer).  The decision depends on head_dim and max_len, not on n_kv.
-SWITCH_SHAPES = {"small": (128, 8, 2, None), "7b": (128, 32, 8, 4096)}
+# shared memory beside the working area, as in the real layer); and the 8-head attention alone, which runs the register kernel.  The
+# decision depends on head_dim and max_len, not on n_kv.  (head_dim, n_heads, n_kv, other phase: None = the ring matvec, 0 = none,
+# else the qkv phase of that dim; the persistent kernel below the switch)
+SWITCH_SHAPES = {"small": (128, 8, 2, None, 2), "7b": (128, 32, 8, 4096, 2), "attn": (128, 8, 2, 0, 1)}
 
 
 def qkv_phase(dev, dim):
@@ -362,13 +365,13 @@ def switch_step(shape, lazy, f16, max_len, kv_len, R=None):
     """fresh device; one step of the shape's flush at this max_len -> (variant, attention output, outputs of the other phase)"""
     from crabml_b200 import CudaTensor
     from tests.gpu_common import make_device
-    hd, n_heads, n_kv, dim = SWITCH_SHAPES[shape]
+    hd, n_heads, n_kv, dim, _ = SWITCH_SHAPES[shape]
     dt = oc.F16 if f16 else oc.F32
     R = R or Retrieval(hd, n_heads, n_kv, kv_len)
     dev = make_device(lazy=lazy)
     try:
         kc, vc = fill(CudaTensor, dev, CudaTensor.alloc([n_kv, max_len, hd], dt, dev), CudaTensor.alloc([n_kv, max_len, hd], dt, dev), R.K, R.V)
-        ys = qkv_phase(dev, dim) if dim else [ring_matvec(dev)]
+        ys = qkv_phase(dev, dim) if dim else [] if dim == 0 else [ring_matvec(dev)]
         out = attention(CudaTensor, dev, kc, vc, R.q1, R.k1, R.v1, n_heads, n_kv, hd).export()
         return dev.mega_variant(), out, [y.export() for y in ys]
     finally:
@@ -390,32 +393,30 @@ _SWITCHES = {}
 
 
 def switches(shape):
-    """-> (first max_len that leaves the ring kernel, first max_len that leaves the persistent kernels)"""
+    """-> first max_len that leaves the persistent kernel for the CUDA graph"""
     if shape not in _SWITCHES:
         lo, hi = 256, 50808
-        assert switch_step(shape, 2, False, lo, 1)[0] == 2 and switch_step(shape, 2, False, hi, 1)[0] == 0
-        graph = first_max_len(shape, lambda v: v == 0, lo, hi)
-        ring_end = first_max_len(shape, lambda v: v != 2, lo, graph)
-        _SWITCHES[shape] = (ring_end, graph)
+        assert switch_step(shape, 2, False, lo, 1)[0] == SWITCH_SHAPES[shape][4] and switch_step(shape, 2, False, hi, 1)[0] == 0
+        _SWITCHES[shape] = first_max_len(shape, lambda v: v == 0, lo, hi)
     return _SWITCHES[shape]
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("shape", list(SWITCH_SHAPES))
 def test_each_side_of_the_context_length_switches(shape, capsys):
-    """Probe (one step per candidate, a fresh device each) the max_len at which lazy mode 2 leaves the ring kernel and the persistent
-    kernels; then on each side of each switch fill the cache to max_len - 1 and require the analytic answer and the eager bits, for
-    both cache types."""
-    ring_end, graph = switches(shape)
+    """Probe (one step per candidate, a fresh device each) the max_len at which lazy mode 2 leaves its persistent kernel for the CUDA
+    graph; then on each side of the switch fill the cache to max_len - 1 and require the analytic answer and the eager bits, for both
+    cache types."""
+    graph = switches(shape)
+    hd, n_heads, n_kv, _, kernel = SWITCH_SHAPES[shape]
     with capsys.disabled():
-        print(f"\n{shape}: lazy=2 runs the ring kernel up to max_len {ring_end - 1}, the register kernel on [{ring_end}, {graph - 1}], "
+        print(f"\n{shape}: lazy=2 runs the {'ring' if kernel == 2 else 'register'} kernel up to max_len {graph - 1}, "
               f"the CUDA graph of fused kernels from {graph}")
-    hd, n_heads, n_kv, _ = SWITCH_SHAPES[shape]
-    for max_len in sorted({ring_end - 1, ring_end, graph - 1, graph}):
+    for max_len in (graph - 1, graph):
         for f16 in (False, True):
             R = Retrieval(hd, n_heads, n_kv, max_len - 1)
             variant, out, ys = switch_step(shape, 2, f16, max_len, max_len - 1, R)
-            assert variant == (2 if max_len < ring_end else 1 if max_len < graph else 0), (max_len, variant)
+            assert variant == (kernel if max_len < graph else 0), (max_len, variant)
             R.check(out, 1, f16, f"{shape} lazy=2 max_len {max_len} variant {variant}")
             _, out0, ys0 = switch_step(shape, 0, f16, max_len, max_len - 1, R)
             np.testing.assert_array_equal(out.view(np.uint32), out0.view(np.uint32))

@@ -18,7 +18,8 @@ from crabml_b200 import CudaTensorDevice, CudaError, TensorError
 from crabml_b200 import capi, runner as R
 dev = CudaTensorDevice(0, lazy=2)
 conf = R.LlamaConfig(8, 8, 2, 1024, 2048, 64, 512, 1e-5, 128)
-w = R.synthetic_weights(dev, conf, capi.Q8_0, capi.Q8_0, seed=3)
+wt = getattr(capi, sys.argv[1]) if len(sys.argv) > 1 else capi.Q8_0
+w = R.synthetic_weights(dev, conf, wt, wt, seed=3)
 r = R.LlamaRunner(dev, conf, w, 16)
 t0 = time.time()
 try:
@@ -31,15 +32,16 @@ print("CLEAN-EXIT")
 """ % ROOT
 
 
-@pytest.mark.parametrize("flags", [0x4D, 0x64D], ids=["register-pipe kernel", "ring kernel"])
-def test_deserting_cta_is_a_timeout_error_not_a_hang(flags):
+# Q4_K weights run mega_kernel (mega.cu), Q8_0 weights the ring kernel (mega_ring.cu)
+@pytest.mark.parametrize("wt", ["Q4_K", "Q8_0"], ids=["register-pipe kernel", "ring kernel"])
+def test_deserting_cta_is_a_timeout_error_not_a_hang(wt):
     """test hook MK_F_TESTSTALL (0x80): the last CTA leaves before the third grid barrier, i.e. the grid behaves as if one CTA had
     never become resident (another tenant on the GPU).  Every other CTA must give up after the spin bound, the kernel must drain
     (ring kernel: the producer warps stop, bulk copies in flight land before the CTA's shared memory goes away), and the host must
     see CC_ERR_CUDA 'megakernel barrier timeout' -- within seconds."""
-    env = dict(os.environ, CRABML_MEGA_FLAGS=str(flags | 0x80))
+    env = dict(os.environ, CRABML_MEGA_FLAGS=str(0x44C | 0x80))          # the default flag word + the hook
     t0 = time.time()
-    p = subprocess.run([sys.executable, "-c", CHILD], env=env, capture_output=True, text=True, timeout=120)
+    p = subprocess.run([sys.executable, "-c", CHILD, wt], env=env, capture_output=True, text=True, timeout=120)
     out = p.stdout + p.stderr
     assert "ERROR:" in out and "barrier timeout" in out, out
     assert "CLEAN-EXIT" in out, out

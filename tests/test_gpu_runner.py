@@ -155,7 +155,9 @@ def test_lazy_mode_matches_eager_ops_through_python_mirror(fixture_path):
 @pytest.mark.parametrize("wt,ct", [(oc.Q8_0, oc.Q8_0), (oc.Q4_0, oc.Q6_K), (oc.Q4_K, oc.Q6_K)])
 def test_lazy_7b_shaped_layer(wt, ct):
     """Every execution mode on the same model.  The K-quant rows do not take the streaming kernel: they check that the fuser
-    hands the f32 normalised row (not only the Q8_0 scratch) to matvecs that fall back to their eager kernels."""
+    hands the f32 normalised row (not only the Q8_0 scratch) to matvecs that fall back to their eager kernels.  Lazy mode 2 runs
+    both persistent kernels here: the ring kernel (mega_ring.cu) for the tables with Q8_0 / Q4_0 phases, mega_kernel (mega.cu)
+    for the all-K-quant one."""
     from crabml_b200 import runner as R
     conf = R.LlamaConfig(32, 32, 2, 4096, 11008, 4096, 32000, 1e-5, 128)
     res = {}
@@ -168,6 +170,8 @@ def test_lazy_7b_shaped_layer(wt, ct):
             if lazy:
                 st = dev.lazy_stats()
                 assert st["uncached"] == 0 and st["graph_replays"] >= 2, st
+            if lazy == 2:
+                assert dev.mega_variant() == (1 if wt == oc.Q4_K else 2), dev.mega_variant()
             r.close()
         finally:
             dev.close()
@@ -177,31 +181,6 @@ def test_lazy_7b_shaped_layer(wt, ct):
     assert np.isfinite(res[0]).all() and np.abs(res[0]).max() > 1e-3
     for mode in (1, 2):
         np.testing.assert_array_equal(res[mode].view(np.uint32), res[0].view(np.uint32), err_msg=f"lazy={mode} vs eager")
-
-
-@pytest.mark.parametrize("wt,ct", [(oc.Q8_0, oc.Q8_0), (oc.Q4_0, oc.Q6_K)])
-def test_both_persistent_kernels_bit_identical_on_7b_shapes(tmp_path, wt, ct):
-    """The two persistent kernels -- weights through registers (mega.cu: what sharded runs and shapes the ring cannot feed use) and
-    weights through the TMA-fed shared-memory ring (mega_ring.cu: the default) -- against the eager kernels on the same 7B-shaped
-    model, each in its own process (the flag word that selects the kernel is read once per process)."""
-    import subprocess
-    import sys
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    got = {}
-    for name, lazy, flags in (("eager", 0, None), ("registers", 2, "0x4d"), ("ring", 2, None)):
-        env = dict(os.environ)
-        env.pop("CRABML_MEGA_FLAGS", None)
-        if flags:
-            env["CRABML_MEGA_FLAGS"] = flags
-        out = str(tmp_path / f"{name}.npz")
-        subprocess.run([sys.executable, os.path.join(root, "tests", "mega_variant_worker.py"), str(lazy), str(wt), str(ct), out],
-                       check=True, cwd=root, env=env, timeout=600)
-        got[name] = np.load(out)
-    assert int(got["registers"]["variant"]) == 1 and int(got["ring"]["variant"]) == 2
-    ref = got["eager"]["logits"]
-    assert np.isfinite(ref).all() and np.abs(ref).max() > 1e-3
-    for name in ("registers", "ring"):
-        np.testing.assert_array_equal(got[name]["logits"].view(np.uint32), ref.view(np.uint32), err_msg=f"{name} vs eager")
 
 
 @pytest.mark.parametrize("fname", ["tinyllamas-stories-15m-q8_0.gguf", "tinyllamas-stories-15m-q4_0.gguf"])

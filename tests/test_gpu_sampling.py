@@ -144,26 +144,25 @@ def test_lazy_megakernel_runs_one_sample_per_token_and_hands_the_rest_to_the_gra
     assert eager == want
 
 
-def test_fast_modes_sample_bit_identical_ids(tmp_path, fixture_path):
-    """eager, CUDA graph, ring megakernel and register megakernel: same ids and logits over 96 tinyllamas steps and 66 steps of a
-    Llama-2-7B-shaped layer, each in its own process; lazy mode 2 stays in its persistent kernel while sampling."""
+def test_fast_modes_sample_bit_identical_ids_on_ring_and_k_quant_kernels(tmp_path, fixture_path):
+    """eager, CUDA graph and megakernel: same ids and logits over 96 tinyllamas steps and 66 steps of a Llama-2-7B-shaped layer in
+    Q8_0 (the ring megakernel) and in Q4_K + Q6_K (the register megakernel, mega.cu), each mode in its own process; lazy mode 2
+    stays in its persistent kernel while sampling."""
     gguf = fixture_path("tinyllamas-stories-15m-q8_0.gguf")
     got = {}
-    for name, lazy, flags in (("eager", 0, None), ("graph", 1, None), ("registers", 2, "0x4d"), ("ring", 2, None)):
+    for name, lazy in (("eager", 0), ("graph", 1), ("mega", 2)):
         env = dict(os.environ)
         env.pop("CRABML_MEGA_FLAGS", None)
-        if flags:
-            env["CRABML_MEGA_FLAGS"] = flags
         out = str(tmp_path / f"{name}.npz")
         subprocess.run([sys.executable, os.path.join(ROOT, "tests", "sampling_mode_worker.py"), str(lazy), gguf, out], check=True, cwd=ROOT,
                        env=env, timeout=900)
         got[name] = np.load(out)
-    assert int(got["registers"]["tiny_variant"]) == 1 and int(got["registers"]["l7b_variant"]) == 1
-    assert int(got["ring"]["l7b_variant"]) == 2 and int(got["ring"]["tiny_variant"]) in (1, 2)
-    for key in ("tiny", "l7b"):
+    assert int(got["mega"]["l7b_variant"]) == 2 and int(got["mega"]["tiny_variant"]) in (1, 2)
+    assert int(got["mega"]["l7bk_variant"]) == 1
+    for key in ("tiny", "l7b", "l7bk"):
         ref_ids, ref_lg = got["eager"][f"{key}_ids"], got["eager"][f"{key}_logits"]
         assert ref_ids.size >= 64 and len(set(ref_ids.tolist())) > 8, ref_ids
-        for name in ("graph", "registers", "ring"):
+        for name in ("graph", "mega"):
             np.testing.assert_array_equal(got[name][f"{key}_ids"], ref_ids, err_msg=f"{key}: {name} vs eager")
             np.testing.assert_array_equal(got[name][f"{key}_logits"].view(np.uint32), ref_lg.view(np.uint32), err_msg=f"{key}: {name} vs eager")
 

@@ -58,7 +58,7 @@ for i in range(n):
     cw, pk = int(ts[i * SL + 6]), int(ts[i * SL + 7])          # ring kernel: warp 0 wait cycles ; (row-loop cycles << 20) | entries
     sub[k].append((act, (s2 - max(s0, s1)) / 1e3, (s3 - s2) / 1e3, (raw[i + 1, 0] - s3) / 1e3, xs, rm, qz, cw, pk >> 20, pk & 0xFFF, (pk >> 12) & 0xFF))
 print(f"flags {os.environ.get('CRABML_MEGA_FLAGS', 'default')}: phases {n}, token total {(t[-1] - t[0]) / 1e3:.1f} us (phase time includes the barrier that ends it)")
-print("  CTA 0 per phase: activation ready | rows of warp 0 done | arrive + look-ahead issue | barrier wait || prologue: x staged | rms | quantise")
+print("  CTA 0 per phase: activation ready | rows of warp 0 done | arrive (+ next norm weights requested) | barrier wait || prologue: x staged | rms | quantise")
 for k, v in sorted(agg.items(), key=lambda kv: -sum(kv[1])):
     m = np.mean(np.array(sub[k]), axis=0)
     ringinfo = f" || ring w0: {m[9]:4.1f} entries, {m[8] / max(m[9], 1):6.0f} cyc/entry, waiting {100 * m[7] / max(m[8], 1):3.0f} %, {m[10]:4.1f} entries landed at start" if m[9] > 0 else ""

@@ -55,7 +55,7 @@ if rank == 0:
         s0, s1, s2, s3 = raw[i, :4]
         sub[k].append(((s1 - s0) / 1e3 if s1 > 0 else 0.0, (s2 - max(s0, s1)) / 1e3, (s3 - s2) / 1e3, (raw[i + 1, 0] - s3) / 1e3))
     print(f"world {world} flags {os.environ.get('CRABML_MEGA_FLAGS', 'default')}: {ms / 40 * 1e3:.1f} us per token (events); phases {n}, token total {(t[-1] - t[0]) / 1e3:.1f} us")
-    print("  activation ready | rows done | arrive + look-ahead | barrier wait (incl. the cross-GPU handshake on exchange phases)")
+    print("  activation ready | rows done | arrive | barrier wait (incl. the cross-GPU handshake on exchange phases)")
     for k, v in sorted(agg.items(), key=lambda kv: -sum(kv[1])):
         m = np.mean(np.array(sub[k]), axis=0)
         print(f"  {k:18s} n={len(v):3d}  sum {sum(v):8.1f} us  avg {np.mean(v):6.2f}   | {m[0]:5.2f} | {m[1]:5.2f} | {m[2]:5.2f} | {m[3]:5.2f}")
