@@ -305,14 +305,14 @@ int cc_launch_all_gather(cc_device* dev, const float* src, int64_t n, float* dst
 extern "C" CC_API int cc_test_mega_barrier_floor(cc_device* dev, int n, float* us_per_phase);
 int cc_launch_mega(cc_device* dev, const MkPhase* phases_dev, int n_phases, const uint8_t* dyn_dev, unsigned* bar_dev, size_t smem_work, size_t smem_wstage,
                    unsigned long long* prof, bool sample);
+bool cc_mega_test_stall();
 // mega_ring.cu: the same phase table run by the kernel whose weights arrive through a TMA-fed shared-memory ring
-int cc_mega_flags();
 bool cc_mega_ring_phase_ok(const MkPhase& ph);
 int cc_mega_ring_at_ch(const MkPhase& ph);
 size_t cc_mega_ring_smem_for_phase(const MkPhase& ph);
 bool cc_mega_ring_fits(size_t smem_work, size_t smem_wstage, int slot_bytes, bool generic);
 int cc_launch_mega_ring(cc_device* dev, const MkPhase* phases_dev, int n_phases, const uint8_t* dyn_dev, unsigned* bar_dev, size_t smem_work, size_t smem_wstage,
-                        unsigned long long* prof, const CommDev* comm, bool generic, bool sample, int slot_bytes, int at_ch, int flags);
+                        unsigned long long* prof, const CommDev* comm, bool generic, bool sample, int slot_bytes, int at_ch);
 int cc_check_async_error(cc_device* dev);     // after a stream synchronize: did a persistent kernel give up on a barrier?
 int cc_launch_normq(cc_device* dev, float* x, float* orig, const float* norm_w, float eps, int64_t n, void* act_scratch, bool write_back);
 int cc_launch_attn_decode(cc_device* dev, const AttnArgs& a);

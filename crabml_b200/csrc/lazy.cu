@@ -740,7 +740,7 @@ int cc_lazy_flush(cc_device* dev) {
                 unsigned long long* prof = P.phases.size() < 4000 ? lz->prof_dev : nullptr;
                 if (!use_mega) rc = run_steps(lz->dyn_dev);
                 else if (P.mega_ring) rc = cc_launch_mega_ring(dev, ge.phases_dev, (int)P.phases.size(), lz->dyn_dev, lz->bar_dev, P.mega_smem, P.mega_wstage, prof, cc_comm_dev(dev),
-                                                               P.mega_generic, P.mega_sample, P.ring_slot, P.ring_at_ch, cc_mega_flags());
+                                                               P.mega_generic, P.mega_sample, P.ring_slot, P.ring_at_ch);
                 else rc = cc_launch_mega(dev, ge.phases_dev, (int)P.phases.size(), lz->dyn_dev, lz->bar_dev, P.mega_smem, P.mega_wstage, prof, P.mega_sample);
                 e = cudaStreamEndCapture(dev->stream, &graph);
                 if (!rc && e != cudaSuccess) rc = cc_fail(dev, CC_ERR_CUDA, "lazy: end capture: %s", cudaGetErrorString(e));

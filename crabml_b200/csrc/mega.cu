@@ -18,14 +18,14 @@
 #define MK_SYNC() __syncthreads()
 #include "mega_phases.cuh"
 
-// norm weights of the next MATVEC phase's fused prologue, fetched one word per thread at phase start (MK_F_WSTAGE)
+// norm weights of the next MATVEC phase's fused prologue, fetched one word per thread at phase start
 struct MkNextNorm { const float* norm_w; int norm_n; };
 
 // SMP: the table ends with its only SAMPLE phase, run after the phase loop.  Only these instantiations carry the call, so the greedy ones keep
 // their register allocation.
 template <bool SMP>
 __global__ void __launch_bounds__(MK_THREADS, MK_CTAS_PER_SM) mega_kernel(const MkPhase* __restrict__ phases, int n_phases, const uint8_t* dyn,
-                                                                         unsigned* bar, const uint16_t* exp_lut, unsigned long long* prof, int flags, int wtop_off,
+                                                                         unsigned* bar, const uint16_t* exp_lut, unsigned long long* prof, bool test_stall, int wtop_off,
                                                                          unsigned* err_host) {
     extern __shared__ __align__(16) uint8_t smem[];
     __shared__ float s_red[MK_WARPS];
@@ -64,7 +64,7 @@ __global__ void __launch_bounds__(MK_THREADS, MK_CTAS_PER_SM) mega_kernel(const 
         // (in-order issue) before it could issue the phase's own loads.
         static_assert(sizeof(MkPhase) / 4 <= MK_THREADS, "descriptor does not fit one word per thread");
         const int nx = s_ph.next_matvec;
-        const bool look = (flags & MK_F_WSTAGE) && nx > p && nx < n_phases;
+        const bool look = nx > p && nx < n_phases;
         int desc_w = 0, next_w = 0;
         if (p + 1 < n_phases && threadIdx.x < sizeof(MkPhase) / 4) desc_w = ((const int*)(phases + p + 1))[threadIdx.x];
         if (look && threadIdx.x < 3) {
@@ -96,7 +96,7 @@ __global__ void __launch_bounds__(MK_THREADS, MK_CTAS_PER_SM) mega_kernel(const 
         if (look && threadIdx.x < 3) ((int*)&s_next)[threadIdx.x] = next_w;
         const bool more = p + 1 < n_phases;
         // test hook (tests/test_gpu_robustness.py): one CTA deserts before the third barrier, as if it had never become resident
-        if ((flags & MK_F_TESTSTALL) && p == 2 && blockIdx.x == gridDim.x - 1) return;
+        if (test_stall && p == 2 && blockIdx.x == gridDim.x - 1) return;
         if (more) grid_barrier_arrive(bar, gridDim.x, gen);       // its bar.sync also publishes s_next (written just above)
         // immutable norm weights of the next fused prologue, requested before waiting at the barrier: one L2 trip less after it
         if (look && s_next.norm_n > 0) {
@@ -109,13 +109,13 @@ __global__ void __launch_bounds__(MK_THREADS, MK_CTAS_PER_SM) mega_kernel(const 
         }
         if (stamp) prof[p * MK_PROF_SLOTS + 3] = globaltimer_ns();
         if (more) {
-            grid_barrier_wait(bar, gridDim.x, gen, nocomm, 0u, (flags & MK_F_POLLCNT) != 0, &s_abort, err_host);
+            grid_barrier_wait(bar, gridDim.x, gen, nocomm, 0u, &s_abort, err_host);
             gen++;
             if (s_abort) break;              // a barrier timed out (a CTA never became resident): bail out, host reports
             // the barrier is open: the row the next fused prologue normalises is complete -- request it before anything else (descriptor
             // bookkeeping, geometry) so that its L2 round trip overlaps them
             const MkPhase& nph = s_phs[(p + 1) & 1];
-            if ((flags & MK_F_XEARLY) && nph.type == MK_MATVEC && nph.x) {
+            if (nph.type == MK_MATVEC && nph.x) {
                 const unsigned sx = (unsigned)__cvta_generic_to_shared(work + mk_generic_sx_offset(nph.mv.k));      // = s_x of the phase's prologue
                 const float* xg = nph.x;
                 for (int i = threadIdx.x; i < (nph.mv.k >> 2); i += MK_THREADS)
@@ -174,16 +174,14 @@ bool cc_mega_generic_supported(int type, int64_t k) {
     return (type == CC_Q2_K || type == CC_Q3_K || type == CC_Q4_K || type == CC_Q5_K || type == CC_Q6_K || type == CC_Q8_K) && k % 256 == 0 && k <= 32768;
 }
 
-// developer A/B switches: CRABML_MEGA_FLAGS replaces the default flag word (see MK_F_* and the L2 budget byte)
-#define MK_DEFAULT_FLAGS (MK_F_WSTAGE | MK_F_POLLCNT | MK_F_XEARLY | MK_F_RPAIR)      // 0x44C; pairs: the fastest of the measured flag words
-int cc_mega_flags() {
-    static const int f = getenv("CRABML_MEGA_FLAGS") ? (int)strtol(getenv("CRABML_MEGA_FLAGS"), nullptr, 0) : MK_DEFAULT_FLAGS;
-    return f;
+// test hook of both persistent kernels: bit 0x80 (MK_F_TESTSTALL) of CRABML_MEGA_FLAGS; the word's other bits have no effect
+bool cc_mega_test_stall() {
+    static const bool on = getenv("CRABML_MEGA_FLAGS") && (strtol(getenv("CRABML_MEGA_FLAGS"), nullptr, 0) & MK_F_TESTSTALL);
+    return on;
 }
 
 int cc_launch_mega(cc_device* dev, const MkPhase* phases_dev, int n_phases, const uint8_t* dyn_dev, unsigned* bar_dev, size_t smem_work, size_t smem_wstage,
                    unsigned long long* prof, bool sample) {
-    const int flags = cc_mega_flags();
     int max_ctas_per_sm = 0;
     const size_t wtop = (smem_work + 15) & ~(size_t)15;
     const size_t smem = wtop + smem_wstage;
@@ -207,7 +205,7 @@ int cc_launch_mega(cc_device* dev, const MkPhase* phases_dev, int n_phases, cons
     attr[0].val.cooperative = getenv("CRABML_MEGA_COOP") ? 1 : 0;
     cfg.attrs = attr; cfg.numAttrs = 1;
     const uint16_t* lut = dev->exp_lut;
-    CC_CUDA(dev, cudaLaunchKernelEx(&cfg, kern, phases_dev, n_phases, dyn_dev, bar_dev, lut, prof, flags, (int)wtop, dev->err_host));
+    CC_CUDA(dev, cudaLaunchKernelEx(&cfg, kern, phases_dev, n_phases, dyn_dev, bar_dev, lut, prof, cc_mega_test_stall(), (int)wtop, dev->err_host));
     CC_LAUNCH_CHECK(dev);
     return CC_OK;
 }

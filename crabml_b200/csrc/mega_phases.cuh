@@ -34,8 +34,9 @@ __device__ __forceinline__ void st_release_u32(unsigned* p, unsigned v) { asm vo
 //   arrive : bar.sync, then ONE thread does a fire-and-forget red.release.gpu.add on a flat monotonic counter
 //            (the release publishes the CTA's phase output; that thread never issues prefetch loads);
 //   ...      the other warps may already request the next phase's norm weights (mega.cu);
-//   wait   : CTA 0 watches the counter reach (gen+1) * nblocks and publishes the generation word; everyone else spins on
-//            the generation with ld.acquire; then bar.sync.
+//   wait   : every CTA watches the counter reach (gen+1) * nblocks with ld.acquire (one L2 round trip less than counter -> CTA 0
+//            -> generation word); CTA 0 also publishes the generation word, which the next launch starts from and which the other
+//            CTAs wait for at an exchange barrier; then bar.sync.
 // Layout (u32 words on separate 128-byte lines): [0] arrival counter, [32] generation.  Both are monotonic ACROSS launches (u32
 // wrap-around included: only equality is tested): a launch starts from the generation the previous one left, so a graph
 // replay needs no reset node in front of the kernel.
@@ -48,31 +49,25 @@ struct MkSpin {
     CcSpin sp;
     __device__ __forceinline__ bool expired(unsigned* bar, unsigned* err_host, unsigned code) { return sp.expired(&bar[MK_BAR_ERR], err_host, code); }
 };
-// xgpu: this CTA stored partial rows into the peers' exchange slots.  Those stores are ordered before the peers' reads by the chain
-// (CTA i) red.release.gpu -> (CTA 0) ld.acquire.gpu ... fence.sys + st.release.sys -> (peer) ld.acquire.sys: release/acquire patterns of
-// different scopes compose (PTX memory model: causality order is transitive over morally strong synchronisation), so a system-scope
-// fence in EVERY CTA is not required (default: off; the 2-GPU parity test runs this way); sysfence = true adds it (it waits for this
-// CTA's NVLink stores to be acknowledged).
-__device__ __forceinline__ void grid_barrier_arrive(unsigned* bar, unsigned nblocks, unsigned gen, bool xgpu = false, bool sysfence = false) {
+// Exchange phases: the partial rows a CTA stored into the peers' exchange slots are ordered before the peers' reads by the chain
+// (CTA i) red.release.gpu -> (CTA 0) ld.acquire.gpu ... st.release.sys -> (peer) ld.acquire.sys (grid_barrier_wait): release/acquire
+// patterns of different scopes compose (PTX memory model: causality order is transitive over morally strong synchronisation), so no
+// CTA needs a system-scope fence of its own before it arrives.
+__device__ __forceinline__ void grid_barrier_arrive(unsigned* bar, unsigned nblocks, unsigned gen) {
     MK_SYNC();
-    if (threadIdx.x == MK_BAR_THREAD) {
-        if (xgpu && sysfence) __threadfence_system();
-        red_add_release(&bar[0], 1u);
-    }
+    if (threadIdx.x == MK_BAR_THREAD) red_add_release(&bar[0], 1u);
 }
 // xseq != 0: the barrier doubles as the handshake of exchange number xseq with the other GPUs (protocol: comm.cu).  CTA 0's
 // barrier thread, once every local CTA has arrived (all partial rows are stored in the peers' slots), publishes xseq in each
-// peer's flag word, waits for every peer's xseq in its own flag words, and only then opens the local barrier.
-// poll_counter: (local barriers only) every CTA watches the arrival counter itself -- one L2 round trip less than
-// counter -> CTA 0 -> generation word; CTA 0 still publishes the generation (the next launch starts from it).
-__device__ __forceinline__ void grid_barrier_wait(unsigned* bar, unsigned nblocks, unsigned gen, const CommDev& comm, unsigned xseq, bool poll_counter,
+// peer's flag word, waits for every peer's xseq in its own flag words, and only then opens the local barrier (the generation word).
+__device__ __forceinline__ void grid_barrier_wait(unsigned* bar, unsigned nblocks, unsigned gen, const CommDev& comm, unsigned xseq,
                                                   int* s_abort, unsigned* err_host) {
     const int lane = threadIdx.x & 31;
     if ((threadIdx.x >> 5) == MK_WARPS - 1) {              // the warp of MK_BAR_THREAD (its lane 31)
         const unsigned target = (gen + 1u) * nblocks;
         bool ok = true;
         if (blockIdx.x == 0) {
-            if (lane == 31) { MkSpin sp; while ((int)(ld_acquire_u32(&bar[0]) - target) < 0) if (sp.expired(bar, err_host, 1u)) { ok = false; break; } }   // (poll mode: the others may already be arriving at the next barrier)
+            if (lane == 31) { MkSpin sp; while ((int)(ld_acquire_u32(&bar[0]) - target) < 0) if (sp.expired(bar, err_host, 1u)) { ok = false; break; } }   // (the others may already be arriving at the next barrier)
             if (xseq) {                                     // kernel-uniform: the whole warp takes this branch together
                 __syncwarp();                               // every local CTA has arrived: all partial rows are in the peers' slots
                 if (lane < comm.world) {                    // one lane per peer: publish and poll in parallel, not rank after rank
@@ -88,8 +83,8 @@ __device__ __forceinline__ void grid_barrier_wait(unsigned* bar, unsigned nblock
             if (lane == 31) st_release_u32(&bar[32], gen + 1u);
         } else if (lane == 31) {
             MkSpin sp;
-            if (poll_counter && !xseq) { while ((int)(ld_acquire_u32(&bar[0]) - target) < 0) if (sp.expired(bar, err_host, 1u)) { ok = false; break; } }   // fast CTAs may already have arrived at the NEXT barrier
-            else { while (ld_acquire_u32(&bar[32]) != gen + 1u) if (sp.expired(bar, err_host, 1u)) { ok = false; break; } }
+            if (!xseq) { while ((int)(ld_acquire_u32(&bar[0]) - target) < 0) if (sp.expired(bar, err_host, 1u)) { ok = false; break; } }   // fast CTAs may already have arrived at the NEXT barrier
+            else { while (ld_acquire_u32(&bar[32]) != gen + 1u) if (sp.expired(bar, err_host, 1u)) { ok = false; break; } }   // exchange: opened by CTA 0 after the handshake
         }
         if (!ok) *s_abort = 1;
     }
@@ -188,7 +183,8 @@ __device__ __forceinline__ int mk_generic_sx_offset(int k) { return ((TKBase::sm
 // get their own allocation instead of pushing spills into the streaming phases of the same kernel (every phase of the Q4_0 body was slower
 // in the instantiation that carries the generic code inline).  mega.cu has no streaming phase: there the phase stays inline, and the two
 // weight segments in flight live in the caller's KSeg pair (MK_GENERIC_SEGS), one pair for all six inlined instantiations -- a pair of
-// their own each costs mega_kernel a 480-byte stack frame and 848 / 1320 bytes of spills instead of 104 and 208 / 292.
+// their own each costs mega_kernel a 480-byte stack frame and 848 / 1312-1328 bytes of spills instead of 112 and 208 / 284 (both layouts compiled from the same
+// sources, nvcc 12.9 -Xptxas -v).
 #ifndef MK_GENERIC_NOINLINE
 #define MK_GENERIC_NOINLINE 0
 #endif
@@ -567,13 +563,4 @@ static __device__ void phase_reduce(const MkPhase& ph, const CommDev& comm, unsi
 
 #define MK_PROF_SLOTS 8      // developer profiling: u64 stamps per phase (CTA 0 / thread 0): 0 start, 1 activation ready, 2 rows done, 3 arrived, 4 x staged, 5 rms known
 
-// flags: 4 norm weights staged before the barrier | 8 every CTA polls the arrival counter | 64 x of the next fused prologue requested
-//        right after the barrier (4 and 64: mega.cu)
-#define MK_F_WSTAGE 4
-#define MK_F_POLLCNT 8
-#define MK_F_SYSFENCE 256      // exchange phases: a system-scope fence in EVERY CTA before its arrival (not needed, see grid_barrier_arrive;
-                               // measured faster at N = 2)
-#define MK_F_TESTSTALL 128     // test hook: the last CTA leaves before barrier 2 -> every other CTA must time out, not hang
-#define MK_F_XEARLY 64         // the f32 row of the next fused prologue is requested (cp.async) right after the barrier opens
-#define MK_F_KVPF 2048         // ring kernel: the producer warps prefetch the attention phase's cached K / V rows into L2 one phase ahead
-#define MK_F_RPAIR 1024        // ring kernel: consumer warps take two units per round (shared activation loads; the slots are held twice as long)
+#define MK_F_TESTSTALL 128     // test hook: the last CTA leaves before barrier 2 -> every other CTA must time out, not hang (cc_mega_test_stall)

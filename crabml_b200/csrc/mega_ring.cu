@@ -97,7 +97,7 @@ __device__ __forceinline__ int mr_locate(const StreamMats& M, const MrGeo& g, in
 // cycles, so the number of polling warps bounds the refill rate, and at 8 the 80-register cap starts to cost.  Sleeping after a failed probe,
 // SIMT-wide parameter computation, in-order probe loops and fence-free hand-back words changed nothing.)
 __device__ void mr_producer(const MkPhase* __restrict__ phases, int n_phases, const MrRing R, unsigned full0, unsigned done0, unsigned ring0,
-                            MkPhase* s_pd, volatile unsigned* s_seq, volatile int* s_abort, int* s_prod_done, unsigned long long* prof_tail, const bool pairs, const bool kvpf, const uint8_t* __restrict__ dyn) {
+                            MkPhase* s_pd, volatile unsigned* s_seq, volatile int* s_abort, int* s_prod_done, unsigned long long* prof_tail) {
     const int lane = threadIdx.x & 31;
     const int pt = (int)threadIdx.x - MK_THREADS;          // producer thread 0 .. 32 * MR_PRODUCER_WARPS - 1: owns the entries pt, pt + 128, ... of every phase
     unsigned long long p_trips = 0, p_cyc = 0, p_iss = 0;       // developer profiling (CTA 0 / lane 0)
@@ -110,24 +110,6 @@ __device__ void mr_producer(const MkPhase* __restrict__ phases, int n_phases, co
 #pragma unroll
         for (int j = 0; j < MR_DESC_PER_LANE; j++) { const int i = lane + 32 * j; nw[j] = (p + 1 < n_phases && i < MR_DESC_WORDS) ? ((const int*)(phases + p + 1))[i] : 0; }
         const MkPhase& ph = s_pd[p & 1];
-        if (kvpf && ph.type == MK_ATTN) {
-            // The attention phase streams a head's K and V rows through 48 KB of shared memory: bytes in flight over latency bounds the rate
-            // (the attention phase grows with every cached position and layer).  The producers reach this table entry while the compute warps are still in
-            // the qkv phase: they ask L2 for the cached rows [0, kv_len) of every kv head now, so that the phase's bulk copies hit L2.
-            // (rows written by earlier launches: stable; the current token's row never goes through the cache on its way to the phase)
-            const AttnArgs& a = ph.at;
-            const long long kv_len = ((const long long*)(dyn + ph.dyn_off))[1];
-            const unsigned ELT = a.kv_f16 ? 2u : 4u, PIECE = 4096u;
-            const size_t head_bytes = (size_t)kv_len * (size_t)a.hd * ELT;
-            const long long per_head = (long long)((head_bytes + PIECE - 1) / PIECE), per_cache = per_head * a.n_kv;
-            for (long long r = (long long)blockIdx.x * (32 * MR_PRODUCER_WARPS) + pt; r < 2 * per_cache; r += (long long)gridDim.x * (32 * MR_PRODUCER_WARPS)) {
-                const long long rr = r >= per_cache ? r - per_cache : r, gk = rr / per_head, piece = rr - gk * per_head;
-                const uint8_t* base = (const uint8_t*)(r >= per_cache ? a.vcache : a.kcache) + (size_t)gk * (size_t)a.seq_stride * ELT + (size_t)piece * PIECE;
-                const size_t left = head_bytes - (size_t)piece * PIECE;
-                const unsigned bytes = (unsigned)(left < PIECE ? left : PIECE) & ~15u;
-                if (bytes) asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(base), "r"(bytes) : "memory");
-            }
-        }
         if (ph.type == MK_MATVEC && ph.act_type != CC_Q8_K) {
             const StreamArgs& A = ph.mv;
             const StreamMats& M = A.mats;
@@ -149,8 +131,7 @@ __device__ void mr_producer(const MkPhase* __restrict__ phases, int n_phases, co
                     // takes a pair always works on two ADJACENT entries and hands them back at once (16 warps x 2 entries < the ring); an odd last unit
                     // follows on its own
                     int u, vs;
-                    if (!pairs) { u = j / g.E; vs = j - u * g.E; }
-                    else if (j < Npair) { const int P = j / twoE, w = j - P * twoE; u = 2 * P + (w & 1); vs = w >> 1; }
+                    if (j < Npair) { const int P = j / twoE, w = j - P * twoE; u = 2 * P + (w & 1); vs = w >> 1; }
                     else { u = g.n_units - 1; vs = j - Npair; }
                     const int v = vs / g.NSEG, sg = vs - v * g.NSEG;
                     int mat;
@@ -186,7 +167,7 @@ __device__ void mr_producer(const MkPhase* __restrict__ phases, int n_phases, co
 }
 
 // ---- consumer side of a streaming MATVEC phase ------------------------------------------------------------------------------------------
-struct MrCons { bool pairs; unsigned full0, done0; const uint8_t* ring; int slot_bytes, nslots; unsigned ent_base; int* s_unit; volatile unsigned* s_seq; volatile int* s_dead; unsigned* err_dev; unsigned* err_host; };
+struct MrCons { unsigned full0, done0; const uint8_t* ring; int slot_bytes, nslots; unsigned ent_base; int* s_unit; volatile unsigned* s_seq; volatile int* s_dead; unsigned* err_dev; unsigned* err_host; };
 
 // Bounded wait for a slot to fill.  A wait that does not end within 2 s (it takes microseconds) raises the error words (code 4, reported by
 // cc_check_async_error) and marks the ring dead for the whole CTA: every later wait returns at once, the launch drains with garbage
@@ -416,22 +397,26 @@ __device__ void phase_matvec_ring(const MkPhase& ph, uint8_t* smem, const uint16
             pend_row[t] = -1;
         }
     };
-    long long c_wait = 0, c_all = 0; int c_n = 0, c_fill = 0;  // developer profiling (CTA 0 / warp 0): cycles waiting for slots, cycles in the row loop, entries, ring fill
+    long long c_wait = 0, c_all = 0; int c_n = 0;  // developer profiling (CTA 0 / warp 0): cycles waiting for slots, cycles in the row loop, entries
     if (stamp1) c_all = clock64();
     const unsigned NS = (unsigned)RC.nslots;
     // Pairs of units are dealt dynamically in ring order (the CTA's pair counter): no warp idles while another still has rows left, and the
     // two rows of a pair share every activation load.  Which warp computes a row does not change its bits.
     const int npairs = g.n_units >> 1, twoE = 2 * g.E;
+    // A CTA with at most one unit claims it alone at entry 0 under either arithmetic below.  The single-unit arm is kept for it on
+    // purpose: compiled for pairs only, ptxas allocates this kernel worse (64 -> 72-byte frame, 128 / 208 -> 140-180 / 240-274 bytes of
+    // spills) and a sampled Llama-2-7B Q8_0 token got 1 % slower (NVIDIA H100 80GB HBM3, 700 W).
+    const bool pairs = g.n_units > 1;
     for (;;) {
         int P = 0;
         if (lane == 0) P = atomicAdd(RC.s_unit, 1);
         P = __shfl_sync(0xffffffffu, P, 0);
-        // pairs off: one unit per round, entries in plain (unit, virtual row, segment) order -- a slot is held for one row's arithmetic only
-        const bool two = RC.pairs && P < npairs;
-        if (RC.pairs ? (!two && !(P == npairs && (g.n_units & 1))) : P >= g.n_units) break;
-        const int u0 = !RC.pairs ? P : two ? 2 * P : g.n_units - 1;
+        // claim P: units 2P and 2P + 1, or an odd last unit alone
+        const bool two = pairs && P < npairs;
+        if (pairs ? (!two && !(P == npairs && (g.n_units & 1))) : P >= g.n_units) break;
+        const int u0 = !pairs ? P : two ? 2 * P : g.n_units - 1;
         const unsigned step = two ? 2u : 1u;
-        unsigned eA = RC.ent_base + (unsigned)(!RC.pairs ? P * g.E : two ? P * twoE : npairs * twoE);
+        unsigned eA = RC.ent_base + (unsigned)(!pairs ? P * g.E : two ? P * twoE : npairs * twoE);
         unsigned slotA = eA % NS, parA = (eA / NS) & 1u;
         float first[2] = {0.0f, 0.0f};
         for (int v = 0; v < g.V; v++) {
@@ -476,7 +461,7 @@ __device__ void phase_matvec_ring(const MkPhase& ph, uint8_t* smem, const uint16
         }
     }
     flush_pending();
-    if (stamp1) { stamp1[5] = (unsigned long long)c_wait; stamp1[6] = ((unsigned long long)(clock64() - c_all) << 20) | ((unsigned long long)c_fill << 12) | (unsigned long long)c_n; }
+    if (stamp1) { stamp1[5] = (unsigned long long)c_wait; stamp1[6] = ((unsigned long long)(clock64() - c_all) << 20) | (unsigned long long)c_n; }
     RC.ent_base += (unsigned)(g.n_units * g.E);
     if (A.epilogue == 3) {
         // the CTA's block of partial rows -> slot[rank] of every GPU's exchange window: warp p serves peer p with coalesced 16-byte
@@ -491,7 +476,7 @@ __device__ void phase_matvec_ring(const MkPhase& ph, uint8_t* smem, const uint16
 
 template <bool GEN, bool SMP>      // SMP: the table ends with its only SAMPLE phase (see mega.cu)
 __global__ void __launch_bounds__(MR_THREADS, 1) mega_ring_kernel(const MkPhase* __restrict__ phases, int n_phases, const uint8_t* dyn, unsigned* bar,
-                                                                  const uint16_t* exp_lut, unsigned long long* prof, int flags, int wtop_off, unsigned* err_host,
+                                                                  const uint16_t* exp_lut, unsigned long long* prof, bool test_stall, int wtop_off, unsigned* err_host,
                                                                   const CommDev comm, const MrRing R) {
     extern __shared__ __align__(128) uint8_t smem[];
     __shared__ float s_red[MK_WARPS];
@@ -519,12 +504,12 @@ __global__ void __launch_bounds__(MR_THREADS, 1) mega_ring_kernel(const MkPhase*
     __syncthreads();                         // the only barrier all 640 threads share
     if (threadIdx.x >= MK_THREADS) {
         mr_producer(phases, n_phases, R, full0, done0, (unsigned)__cvta_generic_to_shared(smem + R.ring_off), s_pd[(threadIdx.x - MK_THREADS) >> 5], s_seq, &s_abort, &s_prod_done,
-                    prof ? prof + (size_t)n_phases * MK_PROF_SLOTS : nullptr, (flags & MK_F_RPAIR) != 0, (flags & MK_F_KVPF) != 0, dyn);
+                    prof ? prof + (size_t)n_phases * MK_PROF_SLOTS : nullptr);
         return;
     }
     MrCons RC;
     RC.full0 = full0; RC.done0 = done0; RC.ring = smem + R.ring_off; RC.slot_bytes = R.slot_bytes; RC.nslots = R.nslots; RC.ent_base = 0u;
-    RC.pairs = (flags & MK_F_RPAIR) != 0; RC.s_unit = &s_unit; RC.s_seq = s_seq; RC.s_dead = &s_ring_dead; RC.err_dev = &bar[MK_BAR_ERR]; RC.err_host = err_host;
+    RC.s_unit = &s_unit; RC.s_seq = s_seq; RC.s_dead = &s_ring_dead; RC.err_dev = &bar[MK_BAR_ERR]; RC.err_host = err_host;
     uint8_t* work = smem;
     float* s_w = (float*)(smem + wtop_off);  // generic phases: staging of the norm weights
     unsigned gen = 0;
@@ -571,11 +556,11 @@ __global__ void __launch_bounds__(MR_THREADS, 1) mega_ring_kernel(const MkPhase*
         if (p + 1 < n_phases && threadIdx.x < sizeof(MkPhase) / 4) ((int*)&s_phs[(p + 1) & 1])[threadIdx.x] = desc_w;
         const bool more = p + 1 < n_phases;
         const bool xg = s_ph.xgpu != 0;
-        if ((flags & MK_F_TESTSTALL) && p == 2 && blockIdx.x == gridDim.x - 1) { if (threadIdx.x == 0) s_abort = 1; break; }     // test hook: this CTA deserts
-        if (more) grid_barrier_arrive(bar, gridDim.x, gen, xg, (flags & MK_F_SYSFENCE) != 0);
+        if (test_stall && p == 2 && blockIdx.x == gridDim.x - 1) { if (threadIdx.x == 0) s_abort = 1; break; }     // test hook: this CTA deserts
+        if (more) grid_barrier_arrive(bar, gridDim.x, gen);
         if (stamp) prof[p * MK_PROF_SLOTS + 3] = globaltimer_ns();
         if (more) {
-            grid_barrier_wait(bar, gridDim.x, gen, comm, xg ? xseq + 1u : 0u, (flags & MK_F_POLLCNT) != 0, &s_abort, err_host);
+            grid_barrier_wait(bar, gridDim.x, gen, comm, xg ? xseq + 1u : 0u, &s_abort, err_host);
             gen++; if (xg) xseq++;
             if (s_abort) break;              // a barrier timed out: bail out, the host reports it
         }
@@ -609,9 +594,7 @@ bool cc_mega_ring_phase_ok(const MkPhase& ph) {
         if (((uintptr_t)ph.mv.mats.qs[t] | (uintptr_t)ph.mv.mats.d[t]) & 15u) return false;
     return true;
 }
-int cc_mega_ring_at_ch(const MkPhase& ph) {       // 48 KB of cache rows in flight per head either way (CRABML_RING_ATCH: developer A/B)
-    static const int env = getenv("CRABML_RING_ATCH") ? atoi(getenv("CRABML_RING_ATCH")) : 0;
-    if (env >= 8 && env <= 64) return env;
+int cc_mega_ring_at_ch(const MkPhase& ph) {       // 48 KB of cache rows in flight per head either way
     return ph.at.kv_f16 ? 64 : 32;
 }
 size_t cc_mega_ring_smem_for_phase(const MkPhase& ph) {
@@ -639,7 +622,7 @@ int cc_mega_ring_slots(size_t smem_work, size_t smem_wstage, int slot_bytes, boo
 bool cc_mega_ring_fits(size_t smem_work, size_t smem_wstage, int slot_bytes, bool generic) { return cc_mega_ring_slots(smem_work, smem_wstage, slot_bytes, generic) >= MR_MIN_SLOTS; }
 
 int cc_launch_mega_ring(cc_device* dev, const MkPhase* phases_dev, int n_phases, const uint8_t* dyn_dev, unsigned* bar_dev, size_t smem_work, size_t smem_wstage,
-                        unsigned long long* prof, const CommDev* comm, bool generic, bool sample, int slot_bytes, int at_ch, int flags) {
+                        unsigned long long* prof, const CommDev* comm, bool generic, bool sample, int slot_bytes, int at_ch) {
     auto kern = generic ? (sample ? mega_ring_kernel<true, true> : mega_ring_kernel<true, false>) : (sample ? mega_ring_kernel<false, true> : mega_ring_kernel<false, false>);
     cudaFuncAttributes fa;
     CC_CUDA(dev, cudaFuncGetAttributes(&fa, kern));
@@ -651,8 +634,7 @@ int cc_launch_mega_ring(cc_device* dev, const MkPhase* phases_dev, int n_phases,
     // Ring depth: a Q8_0 ring (4352-byte slots) is faster SHALLOW -- 24 slots = 104 KB per SM decode a Llama-2-7B token in 3.88 ms
     // against 4.04 ms with the ~40 that fit, and 20 / 16 / 12 slots are slower again (NVIDIA H100 80GB HBM3, 400 W).  The Q4_0 consumer is
     // ALU-bound and keeps every slot that fits: a 55 KB ring (24 of its slots) cost it 2-4 %, 46 KB 9 %.
-    int nslots = slot_bytes >= 4352 ? std::min(fit, MR_Q8_SLOTS) : fit;
-    if (const char* e = getenv("CRABML_RING_SLOTS")) { const int v = atoi(e); if (v >= 2 && v <= fit) nslots = v; }      // developer A/B
+    const int nslots = slot_bytes >= 4352 ? std::min(fit, MR_Q8_SLOTS) : fit;
     const size_t smem = ring_off + (size_t)nslots * slot_bytes;
     CC_CUDA(dev, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     int max_ctas_per_sm = 0;
@@ -671,7 +653,7 @@ int cc_launch_mega_ring(cc_device* dev, const MkPhase* phases_dev, int n_phases,
     attr[0].val.cooperative = getenv("CRABML_MEGA_COOP") ? 1 : 0;          // see cc_launch_mega
     cfg.attrs = attr; cfg.numAttrs = 1;
     const uint16_t* lut = dev->exp_lut;
-    CC_CUDA(dev, cudaLaunchKernelEx(&cfg, kern, phases_dev, n_phases, dyn_dev, bar_dev, lut, prof, flags, (int)wtop, dev->err_host, (const CommDev)cd, (const MrRing)R));
+    CC_CUDA(dev, cudaLaunchKernelEx(&cfg, kern, phases_dev, n_phases, dyn_dev, bar_dev, lut, prof, cc_mega_test_stall(), (int)wtop, dev->err_host, (const CommDev)cd, (const MrRing)R));
     CC_LAUNCH_CHECK(dev);
     return CC_OK;
 }

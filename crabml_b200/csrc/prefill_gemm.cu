@@ -303,10 +303,8 @@ void cc_prefill_release(cc_device* dev) {
 }
 
 bool cc_prefill_supported(int wtype, int64_t m, int64_t k, int64_t b) {
-    static const int min_b = getenv("CRABML_PREFILL_MIN_B") ? atoi(getenv("CRABML_PREFILL_MIN_B")) : 32;
-    if (getenv("CRABML_PREFILL_OFF")) return false;
     const int at = cc_partner_type(wtype);
-    return b >= min_b && k % PG_BLOCK_K == 0 && k >= PG_BLOCK_K && m >= 1 && (at == CC_Q8_0 || at == CC_Q8_K);
+    return b >= 32 && k % PG_BLOCK_K == 0 && k >= PG_BLOCK_K && m >= 1 && (at == CC_Q8_0 || at == CC_Q8_K);
 }
 
 template <int BLOCK_N>

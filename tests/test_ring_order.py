@@ -29,15 +29,13 @@ def geo(m, n_mats, k, epilogue, cta, grid=GRID):
     return dict(nb=nb, nseg=nseg, V=v, E=v * nseg, n_units=n_units, first=first, stride=stride)
 
 
-def producer_order(g, pairs):
+def producer_order(g):
     """mr_producer: entry index j -> (unit, virtual row, segment)."""
-    n, e, two_e = g["n_units"] * g["E"], g["E"], 2 * g["E"]
+    n, two_e = g["n_units"] * g["E"], 2 * g["E"]
     npair = (g["n_units"] >> 1) * two_e
     out = []
     for j in range(n):
-        if not pairs:
-            u, vs = divmod(j, e)
-        elif j < npair:
+        if j < npair:
             p, w = divmod(j, two_e)
             u, vs = 2 * p + (w & 1), w >> 1
         else:
@@ -47,9 +45,10 @@ def producer_order(g, pairs):
     return out
 
 
-def consumer_walk(g, pairs):
+def consumer_walk(g):
     """phase_matvec_ring: for every claim P the list of (entry index, unit, virtual row, segment) it consumes, in order."""
     e, two_e, npairs = g["E"], 2 * g["E"], g["n_units"] >> 1
+    pairs = g["n_units"] > 1                                          # a lone unit: the single-unit arm (same claim either way)
     claims = []
     for p in itertools.count():
         two = pairs and p < npairs
@@ -80,22 +79,21 @@ SHAPES = [  # (rows per matrix, matrices, k, epilogue)
 ]
 
 
-@pytest.mark.parametrize("pairs", [True, False])
 @pytest.mark.parametrize("m,n_mats,k,epilogue", SHAPES)
-def test_producer_and_consumers_agree_on_the_ring_order(m, n_mats, k, epilogue, pairs):
+def test_producer_and_consumers_agree_on_the_ring_order(m, n_mats, k, epilogue):
     covered_rows = set()
     for cta in (0, 1, 37, 146, 147):
         g = geo(m, n_mats, k, epilogue, cta)
-        order = producer_order(g, pairs)
+        order = producer_order(g)
         # every (unit, virtual row, segment) of the CTA exactly once
         want = {(u, v, s) for u in range(g["n_units"]) for v in range(g["V"]) for s in range(g["nseg"])}
         assert len(order) == len(want) and set(order) == want
         seen = []
-        for walk in consumer_walk(g, pairs):
+        for walk in consumer_walk(g):
             for idx, (e, u, v, s) in enumerate(walk):
                 assert order[e] == (u, v, s), (cta, e, order[e], (u, v, s))
                 seen.append(e)
-            if pairs and len(walk) == 2 * g["E"]:                       # a pair round: its two entries of every step are adjacent in the ring
+            if len(walk) == 2 * g["E"]:                                       # a pair round: its two entries of every step are adjacent in the ring
                 for a, b in zip(walk[0::2], walk[1::2]):
                     assert b[0] == a[0] + 1
         assert sorted(seen) == list(range(len(order)))                # the consumers release every slot exactly once

@@ -56,12 +56,12 @@ for i in range(n):
     rm = (s5 - s4) / 1e3 if s5 > 0 and s4 > 0 else 0.0  # prologue: rms known
     qz = (s1 - s5) / 1e3 if s5 > 0 and s1 > 0 else 0.0  # prologue: quantised
     cw, pk = int(ts[i * SL + 6]), int(ts[i * SL + 7])          # ring kernel: warp 0 wait cycles ; (row-loop cycles << 20) | entries
-    sub[k].append((act, (s2 - max(s0, s1)) / 1e3, (s3 - s2) / 1e3, (raw[i + 1, 0] - s3) / 1e3, xs, rm, qz, cw, pk >> 20, pk & 0xFFF, (pk >> 12) & 0xFF))
-print(f"flags {os.environ.get('CRABML_MEGA_FLAGS', 'default')}: phases {n}, token total {(t[-1] - t[0]) / 1e3:.1f} us (phase time includes the barrier that ends it)")
+    sub[k].append((act, (s2 - max(s0, s1)) / 1e3, (s3 - s2) / 1e3, (raw[i + 1, 0] - s3) / 1e3, xs, rm, qz, cw, pk >> 20, pk & 0xFFF))
+print(f"phases {n}, token total {(t[-1] - t[0]) / 1e3:.1f} us (phase time includes the barrier that ends it)")
 print("  CTA 0 per phase: activation ready | rows of warp 0 done | arrive (+ next norm weights requested) | barrier wait || prologue: x staged | rms | quantise")
 for k, v in sorted(agg.items(), key=lambda kv: -sum(kv[1])):
     m = np.mean(np.array(sub[k]), axis=0)
-    ringinfo = f" || ring w0: {m[9]:4.1f} entries, {m[8] / max(m[9], 1):6.0f} cyc/entry, waiting {100 * m[7] / max(m[8], 1):3.0f} %, {m[10]:4.1f} entries landed at start" if m[9] > 0 else ""
+    ringinfo = f" || ring w0: {m[9]:4.1f} entries, {m[8] / max(m[9], 1):6.0f} cyc/entry, waiting {100 * m[7] / max(m[8], 1):3.0f} %" if m[9] > 0 else ""
     print(f"  {k:16s} n={len(v):3d}  sum {sum(v):8.1f} us  avg {np.mean(v):6.2f}  min {min(v):6.2f}  max {max(v):6.2f}   | {m[0]:5.2f} | {m[1]:5.2f} | {m[2]:5.2f} | {m[3]:5.2f} || {m[4]:5.2f} | {m[5]:5.2f} | {m[6]:5.2f}{ringinfo}")
 tail = [int(ts[n * SL + i]) for i in range(1, 4)]
 if tail[0]:

@@ -54,7 +54,7 @@ if rank == 0:
         agg[k].append(d[i])
         s0, s1, s2, s3 = raw[i, :4]
         sub[k].append(((s1 - s0) / 1e3 if s1 > 0 else 0.0, (s2 - max(s0, s1)) / 1e3, (s3 - s2) / 1e3, (raw[i + 1, 0] - s3) / 1e3))
-    print(f"world {world} flags {os.environ.get('CRABML_MEGA_FLAGS', 'default')}: {ms / 40 * 1e3:.1f} us per token (events); phases {n}, token total {(t[-1] - t[0]) / 1e3:.1f} us")
+    print(f"world {world}: {ms / 40 * 1e3:.1f} us per token (events); phases {n}, token total {(t[-1] - t[0]) / 1e3:.1f} us")
     print("  activation ready | rows done | arrive | barrier wait (incl. the cross-GPU handshake on exchange phases)")
     for k, v in sorted(agg.items(), key=lambda kv: -sum(kv[1])):
         m = np.mean(np.array(sub[k]), axis=0)
