@@ -283,10 +283,11 @@ struct DeqPlanes { const uint8_t* p[CC_MAX_PLANES]; int64_t cols; };
 enum { MK_NORMQ = 0, MK_MATVEC = 1, MK_ATTN = 2, MK_ROWS = 3, MK_REDUCE = 4, MK_GATHER = 5, MK_ARGMAX = 6, MK_SAMPLE = 7 };
 struct MkPhase {
     int type, wtype, write_back, next_matvec;  // next_matvec: index of the next MATVEC phase (mega.cu stages its norm weights early), -1 if none
-    int xgpu, red_n, spare1, spare; float* red_dst; const float* red_res;   // cross-GPU barrier after this phase ; REDUCE/GATHER phase operands
+    int xgpu, red_n; const float* next_norm_w; float* red_dst; const float* red_res;   // cross-GPU barrier after this phase ; norm weights of the next
+                                        // fused-norm MATVEC phase after this one (mega_ring.cu stages them one phase ahead), null if none ; REDUCE/GATHER phase operands
     // NORMQ (and the output quantisation of ATTN)
     float* x; float* orig; const float* norm_w; float eps; int n; ActQ8_0 act;
-    int act_type, spare2;               // MATVEC: CC_Q8_0 (streaming phases) or CC_Q8_K (generic phases: K-quant weights)
+    int act_type, next_norm_n;          // MATVEC: CC_Q8_0 (streaming phases) or CC_Q8_K (generic phases: K-quant weights) ; length of next_norm_w
     StreamArgs mv;                      // MATVEC
     AttnArgs at;                        // ATTN
     unsigned long long dyn_off, rope_off;   // ATTN {pos, kv_len} / ROWS row list ; RoPE table
@@ -294,6 +295,7 @@ struct MkPhase {
     const long long* rows_dev;          // ROWS: row indices in device memory (a token slot) instead of the dyn block ; ARGMAX: x = input, n = length,
     long long* slot_dev; long long* hist_dev;   //   slot_dev / hist_dev = where the index goes (hist index at dyn_off, < 0: none)
                                         // SAMPLE: as ARGMAX, with a SampleDyn at dyn_off and the sampler scratch at dst
+    int norm_ahead, pad2;               // fused norm: no op of the table writes norm_w (model weights), so it may be staged before earlier phases end
 };
 size_t cc_mega_smem_for_phase(const MkPhase& ph);      // working area, without the norm-weight staging area on top of it
 const CommDev* cc_comm_dev(cc_device* dev);

@@ -93,7 +93,7 @@ LazyState* cc_lazy_create(cc_device* dev) {
     for (int i = 0; i < LZ_DYN_SLOTS; i++)
         if (cudaMallocHost(&lz->dyn_host[i], lz->dyn_cap) != cudaSuccess || cudaEventCreateWithFlags(&lz->dyn_ev[i], cudaEventDisableTiming) != cudaSuccess) { delete lz; return nullptr; }
     if (cudaMalloc(&lz->dyn_dev, lz->dyn_cap) != cudaSuccess) { delete lz; return nullptr; }
-    if (getenv("CRABML_MEGA_PROF")) cudaMalloc(&lz->prof_dev, 8 * 8 * 4097);
+    if (getenv("CRABML_MEGA_PROF") && cudaMalloc(&lz->prof_dev, 9 * 8 * 4097) == cudaSuccess) cudaMemset(lz->prof_dev, 0, 9 * 8 * 4097);    // stamps a kernel never takes read 0
     if (cudaMalloc(&lz->bar_dev, 4096) != cudaSuccess || cudaMemset(lz->bar_dev, 0, 4096) != cudaSuccess) { delete lz; return nullptr; }
     return lz;
 }
@@ -175,6 +175,11 @@ struct Fuser {
         }
     }
     // no op at or after `from` touches buf, and nobody outside the queue holds it
+    // may an op of this flush write b?  (`a` is the destination of every in-place op; conservative for the others)
+    bool written(const cc_buf* b) const {
+        for (const LOp& op : q) if (op.a.buf == b || op.out == b) return true;
+        return false;
+    }
     bool dead_after(cc_buf* b, size_t from) const {
         auto lu = last_use.find(b);
         if (lu != last_use.end() && lu->second >= from) return false;
@@ -284,7 +289,8 @@ struct Fuser {
         const bool write_back = !dead_after(rn.a.buf, end);
         P.S(0x2001); P.SP(x); P.SP(og); P.SP(w); P.SP(act); P.S((uint64_t)n); uint32_t eb; memcpy(&eb, &eps, 4); P.S(eb); P.S(write_back);
         P.steps.push_back([=](uint8_t*) { return cc_launch_normq(d, x, og, w, eps, n, act, write_back); });
-        { MkPhase ph = {}; ph.type = MK_NORMQ; ph.write_back = write_back; ph.x = x; ph.orig = og; ph.norm_w = w; ph.eps = eps; ph.n = (int)n; ph.act = cc_act_q8_0(act, n); P.phases.push_back(ph); }
+        { MkPhase ph = {}; ph.type = MK_NORMQ; ph.write_back = write_back; ph.x = x; ph.orig = og; ph.norm_w = w; ph.eps = eps; ph.n = (int)n; ph.act = cc_act_q8_0(act, n);
+          ph.norm_ahead = !written(mu.b.buf); P.phases.push_back(ph); }
         *xbuf = rn.a.buf;
         size_t used = (j + 2) - i;
         for (size_t t = i; t < i + used; t++) q[t].done = true;
@@ -547,6 +553,7 @@ struct Fuser {
         MkPhase ph = {};
         ph.type = MK_MATVEC; ph.wtype = wt; ph.act_type = CC_Q8_K; ph.mv = A;
         ph.x = (float*)xb->plane[0]; ph.orig = orig ? (float*)orig->base : nullptr; ph.norm_w = norm_w; ph.eps = eps; ph.n = (int)k;
+        ph.norm_ahead = norm_w && !written(q[j - 1].b.buf);
         // eager steps for the CUDA-graph mode, op by op, without disqualifying the megakernel form
         covered_by_phase = true;
         for (size_t t = i; t < end; t++) fallback(t);
@@ -565,7 +572,7 @@ struct Fuser {
         MkPhase& nq = P.phases[at];
         MkPhase& mv = P.phases[at + 1];
         if (nq.type != MK_NORMQ || mv.type != MK_MATVEC || nq.write_back || nq.n != mv.mv.k) return;
-        mv.x = nq.x; mv.orig = nq.orig; mv.norm_w = nq.norm_w; mv.eps = nq.eps; mv.n = nq.n;
+        mv.x = nq.x; mv.orig = nq.orig; mv.norm_w = nq.norm_w; mv.eps = nq.eps; mv.n = nq.n; mv.norm_ahead = nq.norm_ahead;
         P.phases.erase(P.phases.begin() + at);
         // sharded path: the REDUCE phase that produced x folds into the same prologue (x itself is dead after this group:
         // !write_back), so an exchange costs no phase of its own
@@ -712,7 +719,7 @@ int cc_lazy_flush(cc_device* dev) {
                 for (auto& ph : P.phases) {
                     if (P.mega_ring) {
                         P.mega_smem = std::max(P.mega_smem, cc_mega_ring_smem_for_phase(ph));
-                        if (ph.type == MK_MATVEC && ph.act_type == CC_Q8_K && ph.x && ph.norm_w) P.mega_wstage = std::max(P.mega_wstage, (size_t)ph.n * 4);
+                        if (ph.type == MK_MATVEC && ph.x && ph.norm_w) P.mega_wstage = std::max(P.mega_wstage, (size_t)ph.n * 4);
                         if (ph.type == MK_MATVEC && ph.act_type != CC_Q8_K) P.ring_slot = std::max(P.ring_slot, ph.wtype == CC_Q8_0 ? 4352 : 2304);
                         if (ph.type == MK_ATTN) P.ring_at_ch = cc_mega_ring_at_ch(ph);
                     } else {
@@ -724,10 +731,14 @@ int cc_lazy_flush(cc_device* dev) {
                 else use_mega = P.mega_smem + P.mega_wstage + 4096 <= 227 * 1024;
             }
             if (use_mega) {       // phase table lives in device memory for the lifetime of the graph
-                int nxt = -1;
+                int nxt = -1, nxn = -1;
                 for (int t = (int)P.phases.size() - 1; t >= 0; t--) {
-                    P.phases[t].next_matvec = nxt;
-                    if (P.phases[t].type == MK_MATVEC) nxt = t;
+                    MkPhase& ph = P.phases[t];
+                    ph.next_matvec = nxt;
+                    ph.next_norm_w = nxn >= 0 && P.phases[nxn].norm_ahead ? P.phases[nxn].norm_w : nullptr;
+                    ph.next_norm_n = ph.next_norm_w ? P.phases[nxn].n : 0;
+                    if (ph.type == MK_MATVEC) nxt = t;
+                    if (ph.type == MK_MATVEC && ph.x && ph.norm_w) nxn = t;
                 }
                 if (cudaMalloc(&ge.phases_dev, P.phases.size() * sizeof(MkPhase)) != cudaSuccess ||
                     cudaMemcpy(ge.phases_dev, P.phases.data(), P.phases.size() * sizeof(MkPhase), cudaMemcpyHostToDevice) != cudaSuccess)
@@ -801,8 +812,8 @@ extern "C" CC_API int cc_lazy_mega_profile(cc_device* dev, unsigned long long* t
     if (!dev || !dev->lz || !dev->lz->prof_dev || !ts || !types || !n_out) return CC_ERR_ARG;
     cudaStreamSynchronize(dev->stream);
     int n = (int)dev->lz->prof_types.size();
-    if ((n + 1) * 8 > cap) return CC_ERR_ARG;          // 8 stamps per phase (mega.cu MK_PROF_SLOTS)
-    if (cudaMemcpy(ts, dev->lz->prof_dev, (size_t)(n + 1) * 8 * 8, cudaMemcpyDeviceToHost) != cudaSuccess) return CC_ERR_CUDA;
+    if ((n + 1) * 9 > cap) return CC_ERR_ARG;          // 9 stamps per phase (mega_phases.cuh MK_PROF_SLOTS)
+    if (cudaMemcpy(ts, dev->lz->prof_dev, (size_t)(n + 1) * 9 * 8, cudaMemcpyDeviceToHost) != cudaSuccess) return CC_ERR_CUDA;
     for (int i = 0; i < n; i++) types[i] = dev->lz->prof_types[i];
     *n_out = n;
     return CC_OK;

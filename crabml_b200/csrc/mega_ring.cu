@@ -12,8 +12,10 @@
 //     block order, same arithmetic as matvec_stream.cu (bit-identical results), but a segment is read from the ring with
 //     LDS.128 after waiting on the slot's "full" mbarrier, and the slot is handed back through its "empty" mbarrier.  No weight
 //     registers live across phases -> no register pipe, no look-ahead bookkeeping, 96 registers are enough.
-//   * the activation prologue works from registers (x row: <= 4 float4 per thread straight from L2) instead of a shared-memory
-//     staging copy: the working area shrinks from 78 KB to ~18 KB (matvec) and the ring takes the rest.
+//   * the inputs of a fused prologue arrive before it needs them: the norm weights go into a stage that lives across phases as soon
+//     as the previous fused-norm prologue is done (a phase ahead, while HBM is busy with weights anyway), and the input row is
+//     requested into the phase's working area with cp.async the moment the grid barrier opens -- one L2 trip for every width,
+//     ffn_down's 11008 included.  Only an exchange prologue (sharded path) sums its `world` partial rows from registers.
 // The 512 compute threads synchronise on named barrier 1 (MK_SYNC); the producer warp never joins it.
 // 20 warps: five per SM sub-partition, so its 16384 registers allow 96 per thread (what __launch_bounds__(640, 1) yields).
 #define MK_SYNC() asm volatile("bar.sync 1, 512;" ::: "memory")
@@ -35,9 +37,22 @@ struct MrRing {
 };
 
 __device__ __forceinline__ void mr_expect_tx(unsigned bar, unsigned bytes) { asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory"); }
-__device__ __forceinline__ void mr_bulk_g2s(unsigned dst, const void* src, unsigned bytes, unsigned bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
+// `pol`: an L2::evict_first policy -- every weight byte is read once per token, so its lines should be the first to leave L2, not the
+// rows a token reads again (norm weights, the exp LUT, the KV history)
+__device__ __forceinline__ void mr_bulk_g2s(unsigned dst, const void* src, unsigned bytes, unsigned bar, unsigned long long pol) {
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;" ::"r"(dst), "l"(src), "r"(bytes), "r"(bar), "l"(pol) : "memory");
 }
+// cp.async.cg of floats [0, n) to shared memory, thread t the 16-byte chunks t, t + 512, ... -- the chunks it later reads itself (the
+// prologue's mapping), so its own cp.async.wait_group makes them visible without a CTA barrier; one commit group per call
+__device__ __forceinline__ void mr_stage_f32(float* dst, const float* src, int n) {
+    const unsigned s = (unsigned)__cvta_generic_to_shared(dst);
+    for (int i = threadIdx.x; i < (n >> 2); i += MK_THREADS) asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(s + i * 16), "l"(src + i * 4) : "memory");
+    asm volatile("cp.async.commit_group;" ::: "memory");
+}
+// working area of a streaming MATVEC phase: quants [nbp * 32] | f32 scales [nbp] | block sums [nbp] | reduction scratch 256 B |
+// exchange stage 2 KB | f32 input row [k] (fused prologues without an exchange)
+__host__ __device__ __forceinline__ int mr_nbp(int k) { const int GR = ((k >> 5) + 31) >> 5; return (GR + MK_SEG - 1) / MK_SEG * MK_SEG * 32; }
+__host__ __device__ __forceinline__ int mr_x_off(int k) { return mr_nbp(k) * 40 + 256 + 2048; }
 __device__ __forceinline__ bool mr_try_wait(unsigned bar, unsigned parity) {
     unsigned ok;
     asm volatile("{\n.reg .pred p;\nmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\nselp.u32 %0, 1, 0, p;\n}\n" : "=r"(ok) : "r"(bar), "r"(parity) : "memory");
@@ -101,6 +116,8 @@ __device__ void mr_producer(const MkPhase* __restrict__ phases, int n_phases, co
     const int lane = threadIdx.x & 31;
     const int pt = (int)threadIdx.x - MK_THREADS;          // producer thread 0 .. 32 * MR_PRODUCER_WARPS - 1: owns the entries pt, pt + 128, ... of every phase
     unsigned long long p_trips = 0, p_cyc = 0, p_iss = 0;       // developer profiling (CTA 0 / lane 0)
+    unsigned long long pol;
+    asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
     for (int i = lane; i < MR_DESC_WORDS; i += 32) ((int*)&s_pd[0])[i] = ((const int*)phases)[i];
     __syncwarp();
     unsigned ent = 0;
@@ -146,8 +163,8 @@ __device__ void mr_producer(const MkPhase* __restrict__ phases, int n_phases, co
                     const unsigned fb = full0 + 8u * slot, dst = ring0 + slot * (unsigned)R.slot_bytes;
                     const unsigned dbytes = (nbe * 2u + 15u) & ~15u;        // the scale rows are padded to 16 bytes (CC_D_STRIDE): a short last segment copies its padding
                     mr_expect_tx(fb, nbe * BB + dbytes);
-                    mr_bulk_g2s(dst, q0, nbe * BB, fb);
-                    mr_bulk_g2s(dst + doff, d0, dbytes, fb);
+                    mr_bulk_g2s(dst, q0, nbe * BB, fb, pol);
+                    mr_bulk_g2s(dst + doff, d0, dbytes, fb, pol);
                     __threadfence_block();
                     s_seq[slot] = e + 1u;
                     j += 32 * MR_PRODUCER_WARPS; have = false; p_iss++;
@@ -251,9 +268,12 @@ __device__ __forceinline__ void mr_dot2(const uint8_t* spA, const uint8_t* spB, 
     partA = accA; partB = accB;
 }
 
-// shared memory of the phase: quants [nbp * 32] | f32 scales [nbp] | block sums [nbp] | reduction scratch 256 B | exchange stage 2 KB
+// smem: the phase's working area (mr_x_off); s_wn: the norm-weight stage, holding the weights `wst` once this thread's cp.async groups
+// are complete (requested here when they are not ph.norm_w); x_staged: the input row was requested into the working area as the
+// barrier opened
 template <int TYPE>
-__device__ void phase_matvec_ring(const MkPhase& ph, uint8_t* smem, const uint16_t* exp_lut, MrCons& RC, const CommDev& comm, unsigned xseq, unsigned long long* stamp1) {
+__device__ void phase_matvec_ring(const MkPhase& ph, uint8_t* smem, float* s_wn, const float*& wst, bool x_staged, const uint16_t* exp_lut, MrCons& RC,
+                                  const CommDev& comm, unsigned xseq, unsigned long long* stamp1) {
     const StreamArgs& A = ph.mv;
     const int k = A.k;
     const MrGeo g = mr_geo(A);
@@ -269,37 +289,42 @@ __device__ void phase_matvec_ring(const MkPhase& ph, uint8_t* smem, const uint16
     const StreamMats& M = A.mats;
     if (threadIdx.x == 0) *RC.s_unit = 0;          // ordered before the row loop by the MK_SYNC that ends the prologue
     if (ph.x) {
-        // Fused prologue: [exchange reduction] + [rms_norm * w] + Q8_0 quantisation of x by EVERY CTA, from registers: thread t owns the
-        // float4 chunks t, t + 512, ... (the canonical reduction order of common.cuh, and 8 consecutive threads = one 32-block)
+        // Fused prologue: [exchange reduction] + [rms_norm * w] + Q8_0 quantisation of x by EVERY CTA: thread t owns the float4 chunks
+        // t, t + 512, ... (the canonical reduction order of common.cuh, and 8 consecutive threads = one 32-block).  The norm weights were
+        // staged one fused-norm phase ago; the row itself lands in shared memory after one L2 trip, except in an exchange prologue, which
+        // sums `world` partial rows from registers.
         const int n4 = k >> 2;
         const int npass = nbp >> 6;                                    // 64 blocks per pass of 512 threads (nbp % 128 == 0)
         const float4 z4 = make_float4(0, 0, 0, 0);
+        const float4* s_w4 = (const float4*)s_wn;
+        const float4* s_x4 = (const float4*)(smem + mr_x_off(k));
         const float* xbase = ph.red_n ? comm.data[comm.rank] + (size_t)(xseq & 1u) * CC_COMM_MAX_RANKS * CC_COMM_MAX_ELEMS : ph.x;
         auto load_x = [&](int i) -> float4 {                            // chunk i of the input row
             if (i >= n4) return z4;
-            float4 a4 = __ldcg((const float4*)xbase + i);
-            if (ph.red_n) {                                             // sum over ranks in rank order (+ residual): comm.cu
-                for (int p = 1; p < comm.world; p++) {
-                    const float4 t4 = __ldcg((const float4*)(xbase + (size_t)p * CC_COMM_MAX_ELEMS) + i);
-                    a4.x += t4.x; a4.y += t4.y; a4.z += t4.z; a4.w += t4.w;
-                }
-                if (ph.red_res) { const float4 r4 = __ldcg((const float4*)ph.red_res + i); a4.x += r4.x; a4.y += r4.y; a4.z += r4.z; a4.w += r4.w; }
+            if (!ph.red_n) return s_x4[i];
+            float4 a4 = __ldcg((const float4*)xbase + i);               // sum over ranks in rank order (+ residual): comm.cu
+            for (int p = 1; p < comm.world; p++) {
+                const float4 t4 = __ldcg((const float4*)(xbase + (size_t)p * CC_COMM_MAX_ELEMS) + i);
+                a4.x += t4.x; a4.y += t4.y; a4.z += t4.z; a4.w += t4.w;
             }
+            if (ph.red_res) { const float4 r4 = __ldcg((const float4*)ph.red_res + i); a4.x += r4.x; a4.y += r4.y; a4.z += r4.z; a4.w += r4.w; }
             return a4;
         };
+        if (ph.norm_w && ph.norm_w != wst) { mr_stage_f32(s_wn, ph.norm_w, k); wst = ph.norm_w; }     // weights an earlier phase writes
+        if (!ph.red_n && !x_staged) mr_stage_f32((float*)s_x4, ph.x, k);
+        asm volatile("cp.async.wait_group 1;" ::: "memory");           // groups in flight, oldest first: [norm-weight stage] [x row]
+        if (stamp1) stamp1[7] = globaltimer_ns();
+        asm volatile("cp.async.wait_group 0;" ::: "memory");
+        if (stamp1) stamp1[3] = globaltimer_ns();
         float rms = 1.0f;
-        const bool in_regs = npass <= 4;
-        float4 xr[4], wr[4];
+        const bool in_regs = ph.red_n && npass <= 4;
+        float4 xr[4];
 #pragma unroll
-        for (int j = 0; j < 4; j++) { xr[j] = z4; wr[j] = z4; }
+        for (int j = 0; j < 4; j++) xr[j] = z4;
         if (in_regs) {
 #pragma unroll
-            for (int j = 0; j < 4; j++) {
-                const int i = j * MK_THREADS + (int)threadIdx.x;
-                if (j < npass) { xr[j] = load_x(i); if (ph.norm_w && i < n4) wr[j] = __ldg((const float4*)ph.norm_w + i); }
-            }
+            for (int j = 0; j < 4; j++) if (j < npass) xr[j] = load_x(j * MK_THREADS + (int)threadIdx.x);
         }
-        if (stamp1) stamp1[3] = globaltimer_ns();
         if (ph.norm_w) {
             float ss = 0.0f;
             if (in_regs) {
@@ -338,20 +363,19 @@ __device__ void phase_matvec_ring(const MkPhase& ph, uint8_t* smem, const uint16
             }
             if (sub == 0) s_d[i >> 3] = live ? __half2float(__float2half_rn(d)) : 0.0f;
         };
+        auto load_w = [&](int i) -> float4 { return ph.norm_w && i < n4 ? s_w4[i] : z4; };
         if (in_regs) {
 #pragma unroll
-            for (int j = 0; j < 4; j++) if (j < npass) quant_chunk(j * MK_THREADS + (int)threadIdx.x, xr[j], wr[j]);
+            for (int j = 0; j < 4; j++) if (j < npass) quant_chunk(j * MK_THREADS + (int)threadIdx.x, xr[j], load_w(j * MK_THREADS + (int)threadIdx.x));
+        } else if (!ph.red_n) {
+            for (int j = 0; j < npass; j++) { const int i = j * MK_THREADS + (int)threadIdx.x; quant_chunk(i, load_x(i), load_w(i)); }
         } else {
             for (int j0 = 0; j0 < npass; j0 += 4) {                      // four chunks requested before the first is quantised
-                float4 v[4], w4[4];
+                float4 v[4];
 #pragma unroll
-                for (int j = 0; j < 4; j++) {
-                    const int i = (j0 + j) * MK_THREADS + (int)threadIdx.x;
-                    v[j] = j0 + j < npass ? load_x(i) : z4;
-                    w4[j] = (ph.norm_w && j0 + j < npass && i < n4) ? __ldg((const float4*)ph.norm_w + i) : z4;
-                }
+                for (int j = 0; j < 4; j++) v[j] = j0 + j < npass ? load_x((j0 + j) * MK_THREADS + (int)threadIdx.x) : z4;
 #pragma unroll
-                for (int j = 0; j < 4; j++) if (j0 + j < npass) quant_chunk((j0 + j) * MK_THREADS + (int)threadIdx.x, v[j], w4[j]);
+                for (int j = 0; j < 4; j++) if (j0 + j < npass) quant_chunk((j0 + j) * MK_THREADS + (int)threadIdx.x, v[j], load_w((j0 + j) * MK_THREADS + (int)threadIdx.x));
             }
         }
     } else {   // stage the quantised activation (written by other CTAs in the previous phase: L2 loads)
@@ -380,6 +404,8 @@ __device__ void phase_matvec_ring(const MkPhase& ph, uint8_t* smem, const uint16
     }
     MK_SYNC();
     if (stamp1) *stamp1 = globaltimer_ns();
+    // every thread has read the stage: the next fused-norm phase's weights may go in now, a phase ahead of their use
+    if (ph.x && ph.norm_w) { wst = ph.next_norm_w; if (wst) mr_stage_f32(s_wn, wst, ph.next_norm_n); }
     const int4* aq_l = (const int4*)s_q + lane;
     const float* ad_l = s_d + lane;
     const int* as_l = s_s + lane;
@@ -511,7 +537,11 @@ __global__ void __launch_bounds__(MR_THREADS, 1) mega_ring_kernel(const MkPhase*
     RC.full0 = full0; RC.done0 = done0; RC.ring = smem + R.ring_off; RC.slot_bytes = R.slot_bytes; RC.nslots = R.nslots; RC.ent_base = 0u;
     RC.s_unit = &s_unit; RC.s_seq = s_seq; RC.s_dead = &s_ring_dead; RC.err_dev = &bar[MK_BAR_ERR]; RC.err_host = err_host;
     uint8_t* work = smem;
-    float* s_w = (float*)(smem + wtop_off);  // generic phases: staging of the norm weights
+    // norm-weight stage: the weights of the next fused-norm MATVEC phase, requested when the previous one's prologue is done (the
+    // first at kernel start) -- they are read once per token, so from HBM, and would otherwise cost a trip after the barrier
+    float* s_wn = (float*)(smem + wtop_off);
+    const float* wst = nullptr;              // the norm weights requested into s_wn
+    int xstaged = -1;                        // phase whose input row was requested into its working area as the barrier opened
     unsigned gen = 0;
     if (threadIdx.x == MK_BAR_THREAD) gen = ld_acquire_u32(&bar[32]);
     unsigned xseq = comm.world > 0 ? *comm.seq : 0u;
@@ -519,9 +549,10 @@ __global__ void __launch_bounds__(MR_THREADS, 1) mega_ring_kernel(const MkPhase*
     const int n_loop = SMP ? n_phases - 1 : n_phases;      // SMP: the last phase, the sampler, runs after the loop
     for (int p = 0; p < n_loop; p++) {
         const bool stamp = prof && blockIdx.x == 0 && threadIdx.x == 0;
-        if (stamp) { prof[p * MK_PROF_SLOTS] = globaltimer_ns(); prof[p * MK_PROF_SLOTS + 1] = 0; prof[p * MK_PROF_SLOTS + 4] = 0; prof[p * MK_PROF_SLOTS + 5] = 0; }
+        if (stamp) { prof[p * MK_PROF_SLOTS] = globaltimer_ns(); prof[p * MK_PROF_SLOTS + 1] = 0; prof[p * MK_PROF_SLOTS + 4] = 0; prof[p * MK_PROF_SLOTS + 5] = 0; prof[p * MK_PROF_SLOTS + 8] = 0; }
         MK_SYNC();                           // descriptor p is in shared memory (stored one phase ago)
         const MkPhase& s_ph = s_phs[p & 1];
+        if (p == 0 && !(s_ph.type == MK_MATVEC && s_ph.x && s_ph.norm_w)) { wst = s_ph.next_norm_w; if (wst) mr_stage_f32(s_wn, wst, s_ph.next_norm_n); }
         static_assert(sizeof(MkPhase) / 4 <= MK_THREADS, "descriptor does not fit one word per thread");
         int desc_w = 0;
         if (p + 1 < n_phases && threadIdx.x < sizeof(MkPhase) / 4) desc_w = ((const int*)(phases + p + 1))[threadIdx.x];
@@ -530,18 +561,19 @@ __global__ void __launch_bounds__(MR_THREADS, 1) mega_ring_kernel(const MkPhase*
         case MK_NORMQ: phase_normq(s_ph, s_red); break;
         case MK_MATVEC:
             if (GEN && s_ph.act_type == CC_Q8_K) {
-                switch (s_ph.wtype) {
-                case CC_Q2_K: phase_matvec_generic<TQ2_K>(s_ph, work, s_w, false, false, exp_lut, st1); break;
-                case CC_Q3_K: phase_matvec_generic<TQ3_K>(s_ph, work, s_w, false, false, exp_lut, st1); break;
-                case CC_Q4_K: phase_matvec_generic<TQ45_K<false>>(s_ph, work, s_w, false, false, exp_lut, st1); break;
-                case CC_Q5_K: phase_matvec_generic<TQ45_K<true>>(s_ph, work, s_w, false, false, exp_lut, st1); break;
-                case CC_Q6_K: phase_matvec_generic<TQ6_K>(s_ph, work, s_w, false, false, exp_lut, st1); break;
-                default: phase_matvec_generic<TQ8_K>(s_ph, work, s_w, false, false, exp_lut, st1); break;
+                switch (s_ph.wtype) {      // its cp.async.wait_group 0 also completes the norm-weight stage; without one it requests its weights
+                case CC_Q2_K: phase_matvec_generic<TQ2_K>(s_ph, work, s_wn, s_ph.norm_w == wst, false, exp_lut, st1); break;
+                case CC_Q3_K: phase_matvec_generic<TQ3_K>(s_ph, work, s_wn, s_ph.norm_w == wst, false, exp_lut, st1); break;
+                case CC_Q4_K: phase_matvec_generic<TQ45_K<false>>(s_ph, work, s_wn, s_ph.norm_w == wst, false, exp_lut, st1); break;
+                case CC_Q5_K: phase_matvec_generic<TQ45_K<true>>(s_ph, work, s_wn, s_ph.norm_w == wst, false, exp_lut, st1); break;
+                case CC_Q6_K: phase_matvec_generic<TQ6_K>(s_ph, work, s_wn, s_ph.norm_w == wst, false, exp_lut, st1); break;
+                default: phase_matvec_generic<TQ8_K>(s_ph, work, s_wn, s_ph.norm_w == wst, false, exp_lut, st1); break;
                 }
+                if (s_ph.x && s_ph.norm_w) { wst = s_ph.next_norm_w; if (wst) mr_stage_f32(s_wn, wst, s_ph.next_norm_n); }
                 break;
             }
-            if (s_ph.wtype == CC_Q8_0) phase_matvec_ring<CC_Q8_0>(s_ph, work, exp_lut, RC, comm, xseq, st1);
-            else phase_matvec_ring<CC_Q4_0>(s_ph, work, exp_lut, RC, comm, xseq, st1);
+            if (s_ph.wtype == CC_Q8_0) phase_matvec_ring<CC_Q8_0>(s_ph, work, s_wn, wst, xstaged == p, exp_lut, RC, comm, xseq, st1);
+            else phase_matvec_ring<CC_Q4_0>(s_ph, work, s_wn, wst, xstaged == p, exp_lut, RC, comm, xseq, st1);
             break;
         case MK_ATTN:
             if (s_ph.at.kv_f16) phase_attn<true>(s_ph, (float*)work, s_red, dyn, exp_lut, abar0, apar, R.at_ch);
@@ -563,8 +595,12 @@ __global__ void __launch_bounds__(MR_THREADS, 1) mega_ring_kernel(const MkPhase*
             grid_barrier_wait(bar, gridDim.x, gen, comm, xg ? xseq + 1u : 0u, &s_abort, err_host);
             gen++; if (xg) xseq++;
             if (s_abort) break;              // a barrier timed out: bail out, the host reports it
+            // the barrier is open: the row the next fused prologue quantises is complete -- request it before the descriptor bookkeeping
+            const MkPhase& nph = s_phs[(p + 1) & 1];
+            if (nph.type == MK_MATVEC && nph.act_type != CC_Q8_K && nph.x && !nph.red_n) { mr_stage_f32((float*)(work + mr_x_off(nph.mv.k)), nph.x, nph.mv.k); xstaged = p + 1; }
         }
     }
+    asm volatile("cp.async.wait_all;" ::: "memory");      // a launch that gave up may still have stage copies in flight
     if constexpr (SMP) {                     // the SAMPLE phase after the loop, as in mega.cu
         MK_SYNC();
         if (!s_abort) phase_sample(s_phs[(n_phases - 1) & 1], dyn, work, exp_lut);
@@ -599,15 +635,13 @@ int cc_mega_ring_at_ch(const MkPhase& ph) {       // 48 KB of cache rows in flig
 }
 size_t cc_mega_ring_smem_for_phase(const MkPhase& ph) {
     if (ph.type == MK_MATVEC && ph.act_type == CC_Q8_K) return cc_mega_smem_for_phase(ph);
-    if (ph.type == MK_MATVEC) {
-        const size_t k = (size_t)ph.mv.k, nb = k / 32, GR = (nb + 31) / 32, NSEG = (GR + MK_SEG - 1) / MK_SEG, nbp = NSEG * MK_SEG * 32;
-        return nbp * 40 + 256 + 2048;
-    }
+    if (ph.type == MK_MATVEC) return (size_t)mr_x_off(ph.mv.k) + (ph.x && !ph.red_n ? (size_t)ph.mv.k * 4 : 0);
     if (ph.type == MK_ATTN) return (size_t)(3 * ph.at.hd + ((ph.at.max_len + 8 + 3) & ~3)) * 4 + (size_t)AT_NBUF * cc_mega_ring_at_ch(ph) * ph.at.hd * (ph.at.kv_f16 ? 2 : 4) + 64;
     if (ph.type == MK_SAMPLE) return SMP_SMEM_BYTES;
     return 1024;
 }
-// slots the ring would get beside a working area of `smem_work` (+ `smem_wstage`) bytes; lazy.cu runs the table in the CUDA-graph mode
+// slots the ring would get beside a working area of `smem_work` bytes and the norm-weight stage of `smem_wstage` bytes (the largest
+// n * 4 of a fused-norm phase); lazy.cu runs the table in the CUDA-graph mode
 // below MR_MIN_SLOTS -- e.g. a 32 K-token context, whose attention phase needs 128 KB for the score row alone
 #define MR_MIN_SLOTS 12
 static size_t mr_ring_off(size_t smem_work, size_t smem_wstage) { return ((((smem_work + 15) & ~(size_t)15) + smem_wstage) + 127) & ~(size_t)127; }
@@ -632,7 +666,8 @@ int cc_launch_mega_ring(cc_device* dev, const MkPhase* phases_dev, int n_phases,
     CC_REQUIRE(dev, ring_off + 4 * (size_t)slot_bytes <= cap, "megakernel: the phases leave no room for the weight ring (%zu bytes of working area)", ring_off);
     const int fit = std::min((int)((cap - ring_off) / (size_t)slot_bytes), MR_MAX_SLOTS);
     // Ring depth: a Q8_0 ring (4352-byte slots) is faster SHALLOW -- 24 slots = 104 KB per SM decode a Llama-2-7B token in 3.88 ms
-    // against 4.04 ms with the ~40 that fit, and 20 / 16 / 12 slots are slower again (NVIDIA H100 80GB HBM3, 400 W).  The Q4_0 consumer is
+    // against 4.04 ms with the ~40 that fit, and 20 / 16 / 12 slots are slower again (NVIDIA H100 80GB HBM3, 400 W).  Retuned with the
+    // prologue inputs staged early: 16-24 slots within the spread, 28 and 32 are 4-6 % slower (same card, 700 W).  The Q4_0 consumer is
     // ALU-bound and keeps every slot that fits: a 55 KB ring (24 of its slots) cost it 2-4 %, 46 KB 9 %.
     const int nslots = slot_bytes >= 4352 ? std::min(fit, MR_Q8_SLOTS) : fit;
     const size_t smem = ring_off + (size_t)nslots * slot_bytes;
