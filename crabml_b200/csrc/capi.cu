@@ -384,6 +384,24 @@ extern "C" CC_API void cc_host_free(cc_device* dev, void* p) {
     cudaFreeHost(p);
 }
 
+// fast-order matmul_vec of b rows of x (eager calls, and the lazy fallback step in lazy.cu): x quantised to the weight's partner type,
+// then the streaming kernel (decode), the dense tensor-core GEMM (prefill_gemm.cu) or the warp-per-row kernel.  The activation scratch
+// only grows here when it is too small; lazy.cu sizes it before any capture.
+int cc_launch_matmul_vec(cc_device* dev, const cc_buf* w, const float* xf, float* out, int64_t m, int64_t k, int64_t b) {
+    const int wt = w->dtype, at = cc_partner_type(wt);
+    const bool stream = b == 1 && cc_stream_supported(wt, k);
+    const bool dense = !stream && cc_prefill_supported(wt, m, k, b);
+    int rc = CC_OK;
+    if (at != CC_F32 && !(dense && at == CC_Q8_0)) {         // (the dense path quantises Q8_0 partners itself, fused with the f16 conversion)
+        rc = cc_ensure_act_scratch(dev, cc_act_bytes(at, b * k));
+        if (!rc) rc = cc_launch_quantize(dev, xf, b * k, at, dev->act_scratch);     // matmul_vec.rs:37-40
+    }
+    if (rc) return rc;
+    if (stream) return cc_launch_matvec_stream_plain(dev, w, dev->act_scratch, out, m, k);     // decode hot path
+    if (dense) return cc_launch_prefill_matmul(dev, w, dev->act_scratch, at == CC_Q8_0 ? xf : nullptr, out, m, k, b);
+    return cc_launch_matvec(dev, w, dev->act_scratch, xf, out, m, k, b);
+}
+
 // ---- matmul_vec: cpu_tensor.rs:371-386 + primitives/matmul_vec.rs:9-78 -------------------------------------------------
 extern "C" CC_API int cc_matmul_vec(cc_device* dev, const cc_view* w, const cc_view* x, cc_buf** out) {
     CHECK_VIEW(dev, w, "matmul_vec");
@@ -406,15 +424,14 @@ extern "C" CC_API int cc_matmul_vec(cc_device* dev, const cc_view* w, const cc_v
     if (rc) return rc;
     if (LAZY(dev)) { *out = c; return cc_lazy_record(dev, L_MATVEC, w, x, c, 0, 0, 0, 0, nullptr, 0); }
     const float* xf = (const float*)x->buf->plane[0];
-    const bool dense = !dev->exact && !(b == 1 && cc_stream_supported(wt, k)) && cc_prefill_supported(wt, m, k, b);      // tensor-core path (prefill_gemm.cu)
-    if (at != CC_F32 && !(dense && at == CC_Q8_0)) {         // (the dense path quantises Q8_0 partners itself, fused with the f16 conversion)
-        rc = cc_ensure_act_scratch(dev, cc_act_bytes(at, b * k));
-        if (!rc) rc = cc_launch_quantize(dev, xf, b * k, at, dev->act_scratch);     // matmul_vec.rs:37-40
-    }
-    if (!rc && dev->exact) {
+    if (dev->exact) {
         // exact_order: reference-layout activation blocks + scalar-order dot on the GGUF-layout weights
+        if (at != CC_F32) {
+            rc = cc_ensure_act_scratch(dev, cc_act_bytes(at, b * k));
+            if (!rc) rc = cc_launch_quantize(dev, xf, b * k, at, dev->act_scratch);     // matmul_vec.rs:37-40
+        }
         const uint8_t* wraw = cc_is_quant(wt) ? w->buf->raw : w->buf->plane[0];
-        if (!wraw) rc = cc_fail(dev, CC_ERR_TENSOR, "matmul_vec(exact): weight has no GGUF-layout copy");
+        if (!rc && !wraw) rc = cc_fail(dev, CC_ERR_TENSOR, "matmul_vec(exact): weight has no GGUF-layout copy");
         void* blocks = nullptr; size_t cls = 0;
         if (!rc && (at == CC_Q8_0 || at == CC_Q8_1 || at == CC_Q8_K)) {
             rc = cc_pool_alloc(dev, (size_t)(b * k / cc_block_elems(at)) * cc_block_bytes(at), &blocks, &cls);
@@ -423,11 +440,7 @@ extern "C" CC_API int cc_matmul_vec(cc_device* dev, const cc_view* w, const cc_v
         const uint8_t* act = blocks ? (const uint8_t*)blocks : at == CC_F32 ? (const uint8_t*)xf : (const uint8_t*)dev->act_scratch;
         if (!rc) rc = cc_launch_matvec_exact(dev, wt, wraw, act, (float*)c->base, m, k, b);
         if (blocks) cc_pool_free(dev, blocks, cls);
-    } else if (!rc && b == 1 && cc_stream_supported(wt, k)) {
-        rc = cc_launch_matvec_stream_plain(dev, w->buf, dev->act_scratch, (float*)c->base, m, k);     // decode hot path
-    } else if (!rc && dense) {
-        rc = cc_launch_prefill_matmul(dev, w->buf, dev->act_scratch, at == CC_Q8_0 ? xf : nullptr, (float*)c->base, m, k, b);       // prefill: dense, tensor cores
-    } else if (!rc) rc = cc_launch_matvec(dev, w->buf, dev->act_scratch, xf, (float*)c->base, m, k, b);
+    } else rc = cc_launch_matmul_vec(dev, w->buf, xf, (float*)c->base, m, k, b);
     if (rc) { cc_tensor_release(c); return rc; }
     *out = c;
     return CC_OK;

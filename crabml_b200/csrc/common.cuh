@@ -305,16 +305,24 @@ void cc_comm_destroy(cc_device* dev);
 int cc_launch_all_reduce(cc_device* dev, float* x, int64_t n, const float* residual);
 int cc_launch_all_gather(cc_device* dev, const float* src, int64_t n, float* dst);
 extern "C" CC_API int cc_test_mega_barrier_floor(cc_device* dev, int n, float* us_per_phase);
-int cc_launch_mega(cc_device* dev, const MkPhase* phases_dev, int n_phases, const uint8_t* dyn_dev, unsigned* bar_dev, size_t smem_work, size_t smem_wstage,
-                   unsigned long long* prof, bool sample);
+// the persistent kernel that runs a phase table; the values are those of cc_lazy_mega_variant
+enum MegaVariant { MEGA_NONE = 0, MEGA_REGISTER = 1, MEGA_RING = 2 };     // CUDA-graph mode ; mega_kernel (mega.cu) ; mega_ring_kernel (mega_ring.cu)
+struct MegaLaunch {                 // launch description of one phase table (lazy.cu choose_mega)
+    MegaVariant variant = MEGA_NONE;
+    size_t smem = 1024, wstage = 0;  // working area (largest phase) ; norm-weight stage on top of it (largest n * 4 of a fused-norm phase)
+    int slot_bytes = 0, nslots = 0, at_ch = 64;  // MEGA_RING: weight-ring slot size and count (cc_mega_ring_slots), attention chunk
+    bool generic = false, sample = false;        // the instantiation that carries the generic (K-quant) MATVEC phase / the sampler's call
+};
+int cc_launch_mega(cc_device* dev, const MkPhase* phases_dev, int n_phases, const uint8_t* dyn_dev, unsigned* bar_dev, const MegaLaunch& L,
+                   unsigned long long* prof);
 bool cc_mega_test_stall();
 // mega_ring.cu: the same phase table run by the kernel whose weights arrive through a TMA-fed shared-memory ring
 bool cc_mega_ring_phase_ok(const MkPhase& ph);
 int cc_mega_ring_at_ch(const MkPhase& ph);
 size_t cc_mega_ring_smem_for_phase(const MkPhase& ph);
-bool cc_mega_ring_fits(size_t smem_work, size_t smem_wstage, int slot_bytes, bool generic);
-int cc_launch_mega_ring(cc_device* dev, const MkPhase* phases_dev, int n_phases, const uint8_t* dyn_dev, unsigned* bar_dev, size_t smem_work, size_t smem_wstage,
-                        unsigned long long* prof, const CommDev* comm, bool generic, bool sample, int slot_bytes, int at_ch);
+int cc_mega_ring_slots(const MegaLaunch& L);
+int cc_launch_mega_ring(cc_device* dev, const MkPhase* phases_dev, int n_phases, const uint8_t* dyn_dev, unsigned* bar_dev, const MegaLaunch& L,
+                        unsigned long long* prof, const CommDev* comm);
 int cc_check_async_error(cc_device* dev);     // after a stream synchronize: did a persistent kernel give up on a barrier?
 int cc_launch_normq(cc_device* dev, float* x, float* orig, const float* norm_w, float eps, int64_t n, void* act_scratch, bool write_back);
 int cc_launch_attn_decode(cc_device* dev, const AttnArgs& a);
@@ -327,6 +335,7 @@ bool cc_stream_supported(int type, int64_t k);
 bool cc_mega_generic_supported(int type, int64_t k);      // K-quant weights: generic MATVEC phase of the megakernel (mega.cu)
 int cc_launch_matvec_stream(cc_device* dev, int type, const StreamArgs& A);
 int cc_launch_matvec_stream_plain(cc_device* dev, const cc_buf* w, const void* act, float* out, int64_t m, int64_t k);
+int cc_launch_matmul_vec(cc_device* dev, const cc_buf* w, const float* x, float* out, int64_t m, int64_t k, int64_t b);     // capi.cu
 
 // ---- exact.cu (exact_order verification mode) -------------------------------------------------------
 int cc_launch_matvec_exact(cc_device* dev, int t, const uint8_t* w_gguf, const uint8_t* act_blocks, float* out,

@@ -38,7 +38,7 @@ struct LOp {
 // one captured token graph.  The cache key is a 64-bit fold of the launch signature; `sig` is the signature itself and is compared
 // on every hit (a colliding key must re-capture, never replay another plan's baked pointers); `last_use` drives the LRU bound.
 struct GraphEntry { cudaGraphExec_t exec = nullptr; size_t dyn_bytes = 0; uint64_t launches = 0; MkPhase* phases_dev = nullptr;
-                    std::vector<uint64_t> sig; uint64_t last_use = 0; int mega_variant = 0; };
+                    std::vector<uint64_t> sig; uint64_t last_use = 0; MegaVariant mega_variant = MEGA_NONE; };
 #define LZ_MAX_GRAPHS 64                             // cached token graphs per device (a decode loop needs 2-4)
 
 struct LazyState {
@@ -58,7 +58,7 @@ struct LazyState {
     std::unordered_map<uint64_t, GraphEntry> cache;
     uint64_t flushes = 0, graph_hits = 0, captures = 0, uncached = 0, evictions = 0, collisions = 0;
     uint64_t ns_record = 0, ns_fuse = 0, ns_submit = 0, n_ops = 0;      // host-side cost accounting
-    int mega_variant = 0;            // persistent kernel of the last megakernel flush: 1 mega_kernel, 2 mega_ring_kernel
+    MegaVariant mega_variant = MEGA_NONE;     // persistent kernel of the last megakernel flush
 };
 
 static LView mkview(const cc_view* v) {
@@ -136,11 +136,6 @@ struct Plan {
     bool cacheable = true;
     std::vector<MkPhase> phases;     // megakernel form of the same plan (valid while mega_ok)
     bool mega_ok = true;
-    size_t mega_smem = 1024, mega_wstage = 0;
-    bool mega_ring = false;          // weights through the shared-memory ring (mega_ring.cu)
-    int ring_slot = 0, ring_at_ch = 64;
-    bool mega_generic = false;       // some MATVEC phase is generic (K-quant weights): launch the instantiation that carries that code
-    bool mega_sample = false;        // the table ends with a SAMPLE phase: launch the instantiation that carries the sampler's call
     void S(uint64_t v) { sig.push_back(v); }
     void SP(const void* p) { sig.push_back((uint64_t)(uintptr_t)p); }
     size_t dyn_put(const void* p, size_t n) {
@@ -174,12 +169,12 @@ struct Fuser {
             if (q[j].out) last_use[q[j].out] = j;
         }
     }
-    // no op at or after `from` touches buf, and nobody outside the queue holds it
     // may an op of this flush write b?  (`a` is the destination of every in-place op; conservative for the others)
     bool written(const cc_buf* b) const {
         for (const LOp& op : q) if (op.a.buf == b || op.out == b) return true;
         return false;
     }
+    // no op at or after `from` touches buf, and nobody outside the queue holds it
     bool dead_after(cc_buf* b, size_t from) const {
         auto lu = last_use.find(b);
         if (lu != last_use.end() && lu->second >= from) return false;
@@ -243,88 +238,94 @@ struct Fuser {
                 if (cudaMemcpyAsync(d->dev_idx, op.rows.data(), (size_t)n * 8, cudaMemcpyHostToDevice, d->stream) != cudaSuccess) return cc_fail(d, CC_ERR_CUDA, "row index upload failed");
                 return cc_launch_dequant_rows(d, b.buf, (const int64_t*)d->dev_idx, n, a.shape[a.ndim - 1], a.buf->plane[0], a.buf->dtype);
             }
-            case L_MATVEC: {
-                const int64_t m = a.shape[0], k = a.shape[1], bb = b.ndim == 1 ? 1 : b.shape[0];
-                const int wt = a.buf->dtype, at = cc_partner_type(wt);
-                const float* xf = (const float*)b.buf->plane[0];
-                int rc = CC_OK;
-                const bool dense = !(bb == 1 && cc_stream_supported(wt, k)) && cc_prefill_supported(wt, m, k, bb);
-                if (at != CC_F32 && !(dense && at == CC_Q8_0)) rc = cc_launch_quantize(d, xf, bb * k, at, d->act_scratch);
-                if (rc) return rc;
-                if (bb == 1 && cc_stream_supported(wt, k)) return cc_launch_matvec_stream_plain(d, a.buf, d->act_scratch, (float*)op.out->base, m, k);
-                if (dense) return cc_launch_prefill_matmul(d, a.buf, d->act_scratch, at == CC_Q8_0 ? xf : nullptr, (float*)op.out->base, m, k, bb);
-                return cc_launch_matvec(d, a.buf, d->act_scratch, xf, (float*)op.out->base, m, k, bb);
-            }
+            case L_MATVEC:
+                return cc_launch_matmul_vec(d, a.buf, (const float*)b.buf->plane[0], (float*)op.out->base, a.shape[0], a.shape[1], b.ndim == 1 ? 1 : b.shape[0]);
             }
             return cc_fail(d, CC_ERR_UNSUPPORTED, "lazy: unknown op kind %d", op.kind);
         });
         q[i].done = true;
     }
 
-    // ---- pattern: [DUP] RMS_NORM MUL -> normq ; returns number of ops consumed (0 = no match) ---------------------------------
-    // On success *act_sel receives the scratch index that now holds quantize(x).
-    size_t try_normq(size_t i, int act_sel, cc_buf** xbuf) {
+    // ---- matchers shared by the patterns below -------------------------------------------------------------------------------
+    // [DUP] RMS_NORM MUL on one contiguous f32 row x (1 x n) with an f32 weight row: len = ops consumed, 0 = no match
+    struct NormMatch { size_t len = 0; cc_buf* orig = nullptr; cc_buf* x = nullptr; cc_buf* w = nullptr; int64_t n = 0; float eps = 0.0f; };
+    NormMatch match_norm(size_t i) const {
+        NormMatch m;
         size_t j = i;
-        cc_buf* orig = nullptr;
-        if (is(j, L_DUP) && is(j + 1, L_RMS_NORM) && q[j + 1].a.buf == q[j].a.buf) { orig = q[j].out; j++; }
-        if (!(is(j, L_RMS_NORM) && is(j + 1, L_MUL))) return 0;
+        if (is(j, L_DUP) && is(j + 1, L_RMS_NORM) && q[j + 1].a.buf == q[j].a.buf) { m.orig = q[j].out; j++; }
+        if (!(is(j, L_RMS_NORM) && is(j + 1, L_MUL))) return NormMatch();
         const LOp &rn = q[j], &mu = q[j + 1];
-        if (mu.a.buf != rn.a.buf) return 0;
+        if (mu.a.buf != rn.a.buf) return NormMatch();
         const int64_t n = vlen(rn.a);
-        if (rn.a.ndim > 2 || (rn.a.ndim == 2 && rn.a.shape[0] != 1) || !vcontig(rn.a) || n % 32) return 0;
-        if (vlen(mu.b) != n || mu.b.buf->dtype != CC_F32 || !vcontig(mu.b)) return 0;
-        if (n > 65536) return 0;
-        float* x = (float*)rn.a.buf->plane[0];
-        float* og = orig ? (float*)orig->base : nullptr;
-        const float* w = (const float*)mu.b.buf->plane[0];
-        float eps = rn.f;
+        if (rn.a.ndim > 2 || (rn.a.ndim == 2 && rn.a.shape[0] != 1) || !vcontig(rn.a)) return NormMatch();
+        if (vlen(mu.b) != n || mu.b.buf->dtype != CC_F32 || !vcontig(mu.b)) return NormMatch();
+        m.len = j + 2 - i; m.x = rn.a.buf; m.w = mu.b.buf; m.n = n; m.eps = rn.f;
+        return m;
+    }
+    // does the streaming kernel take the MATVEC at t on row x?
+    bool streams(size_t t, const cc_buf* x) const {
+        if (!is(t, L_MATVEC)) return false;
+        const LOp& mv = q[t];
+        return mv.b.buf == x && cc_stream_supported(mv.a.buf->dtype, mv.a.shape[1]) && vlen(mv.b) == mv.a.shape[1] && vcontig(mv.b);
+    }
+    // the MATVEC at j (weight type wt, k columns) and up to two more of the same type and k on row x, with the epilogue that follows:
+    // gate/up + silu + mul (llama2.rs:620-630) or x = matvec + residual (llama2.rs:266,636).  n matrices, `used` ops consumed.
+    struct GroupMatch { size_t n = 1, used = 1; int epilogue = 0; cc_buf* residual = nullptr; };
+    GroupMatch match_group(size_t j, const cc_buf* x, int wt, int64_t k) const {
+        GroupMatch g;
+        while (g.n < 3 && is(j + g.n, L_MATVEC) && q[j + g.n].b.buf == x && q[j + g.n].a.buf->dtype == wt && q[j + g.n].a.shape[1] == k &&
+               vlen(q[j + g.n].b) == k) g.n++;
+        g.used = g.n;
+        const LOp& m0 = q[j];
+        if (g.n >= 2 && is(j + 2, L_SILU) && is(j + 3, L_MUL) && q[j + 2].a.buf == m0.out && q[j + 3].a.buf == m0.out && q[j + 3].b.buf == q[j + 1].out &&
+            m0.a.shape[0] == q[j + 1].a.shape[0] && vlen(q[j + 3].b) == m0.a.shape[0] && dead_after(q[j + 1].out, j + 4)) {
+            g.n = 2; g.epilogue = 2; g.used = 4;
+        } else if (g.n == 1 && is(j + 1, L_ADD) && q[j + 1].a.buf == m0.out && vlen(q[j + 1].b) == m0.a.shape[0] && q[j + 1].b.buf->dtype == CC_F32 &&
+                   vcontig(q[j + 1].b)) {
+            g.epilogue = 1; g.residual = q[j + 1].b.buf; g.used = 2;
+        } else if (g.n > 1 && is(j + g.n, L_SILU)) {
+            g.n = 1; g.used = 1;                   // do not swallow a gate/up pair we could not fuse as a pair
+        }
+        return g;
+    }
+
+    // ---- pattern: [DUP] RMS_NORM MUL -> normq ; returns number of ops consumed (0 = no match) ---------------------------------
+    // On success *xbuf receives the normalised row, whose quantisation is now in scratch act_sel.
+    size_t try_normq(size_t i, int act_sel, cc_buf** xbuf) {
+        const NormMatch nm = match_norm(i);
+        if (!nm.len || nm.n % 32 || nm.n > 65536) return 0;
+        const int64_t n = nm.n; const float eps = nm.eps;
+        float* x = (float*)nm.x->plane[0];
+        float* og = nm.orig ? (float*)nm.orig->base : nullptr;
+        const float* w = (const float*)nm.w->plane[0];
         void* act = lz->act[act_sel];
         cc_device* d = dev;
         // the normalised f32 row only has to be materialised if something other than the following matvecs reads it
         // (only matvecs the streaming kernel will take consume the quantised scratch; any other reader -- a K-quant or batched
         // matvec falling back to its eager kernel -- needs the f32 row)
-        size_t end = j + 2;
-        while (is(end, L_MATVEC) && q[end].b.buf == rn.a.buf && cc_stream_supported(q[end].a.buf->dtype, q[end].a.shape[1]) &&
-               vlen(q[end].b) == q[end].a.shape[1] && vcontig(q[end].b)) end++;
-        const bool write_back = !dead_after(rn.a.buf, end);
+        size_t end = i + nm.len;
+        while (streams(end, nm.x)) end++;
+        const bool write_back = !dead_after(nm.x, end);
         P.S(0x2001); P.SP(x); P.SP(og); P.SP(w); P.SP(act); P.S((uint64_t)n); uint32_t eb; memcpy(&eb, &eps, 4); P.S(eb); P.S(write_back);
         P.steps.push_back([=](uint8_t*) { return cc_launch_normq(d, x, og, w, eps, n, act, write_back); });
         { MkPhase ph = {}; ph.type = MK_NORMQ; ph.write_back = write_back; ph.x = x; ph.orig = og; ph.norm_w = w; ph.eps = eps; ph.n = (int)n; ph.act = cc_act_q8_0(act, n);
-          ph.norm_ahead = !written(mu.b.buf); P.phases.push_back(ph); }
-        *xbuf = rn.a.buf;
-        size_t used = (j + 2) - i;
-        for (size_t t = i; t < i + used; t++) q[t].done = true;
-        return used;
+          ph.norm_ahead = !written(nm.w); P.phases.push_back(ph); }
+        *xbuf = nm.x;
+        for (size_t t = i; t < i + nm.len; t++) q[t].done = true;
+        return nm.len;
     }
 
     // ---- pattern: 1-3 MATVECs on the same activation through the streaming kernel (+ optional epilogues) ------------------------------
     // `act_sel` >= 0: scratch already holds quantize(x) ; < 0: emit a plain quantise first.
     size_t try_stream(size_t i, cc_buf* xbuf, int act_sel) {
-        if (!is(i, L_MATVEC)) return 0;
+        if (!streams(i, xbuf)) return 0;
         const LOp& m0 = q[i];
-        const int wt = m0.a.buf->dtype;
-        const int64_t k = m0.a.shape[1];
-        if (!cc_stream_supported(wt, k) || m0.b.buf != xbuf || vlen(m0.b) != k || !vcontig(m0.b)) return 0;
-        // count consecutive matvecs sharing x / type / k
-        size_t n = 1;
-        while (n < 3 && is(i + n, L_MATVEC) && q[i + n].b.buf == xbuf && q[i + n].a.buf->dtype == wt && q[i + n].a.shape[1] == k && vlen(q[i + n].b) == k) n++;
+        const int wt = m0.a.buf->dtype; const int64_t k = m0.a.shape[1];
+        const GroupMatch g = match_group(i, xbuf, wt, k);
+        size_t n = g.n, used = g.used;
         StreamArgs A = {};
-        A.k = (int)k;
-        A.exp_lut = dev->exp_lut;
-        size_t used = n;
-        // gate/up + silu + mul (llama2.rs:620-630)
-        if (n >= 2 && is(i + 2, L_SILU) && is(i + 3, L_MUL) && q[i + 2].a.buf == q[i].out && q[i + 3].a.buf == q[i].out && q[i + 3].b.buf == q[i + 1].out &&
-            q[i].a.shape[0] == q[i + 1].a.shape[0] && vlen(q[i + 3].b) == q[i].a.shape[0] && dead_after(q[i + 1].out, i + 4)) {
-            n = 2;
-            A.epilogue = 2;
-            used = 4;
-        } else if (n == 1 && is(i + 1, L_ADD) && q[i + 1].a.buf == m0.out && vlen(q[i + 1].b) == m0.a.shape[0] && q[i + 1].b.buf->dtype == CC_F32 && vcontig(q[i + 1].b)) {
-            A.epilogue = 1;                    // x = matvec + residual (llama2.rs:266,636)
-            A.residual = (const float*)q[i + 1].b.buf->plane[0];
-            used = 2;
-        } else if (n > 1 && is(i + n, L_SILU)) {
-            n = 1; used = 1;                   // do not swallow a gate/up pair we could not fuse as a pair
-        }
+        A.k = (int)k; A.exp_lut = dev->exp_lut; A.epilogue = g.epilogue;
+        A.residual = g.residual ? (const float*)g.residual->plane[0] : nullptr;
         // sharded path: column-split matvec -> allreduce [-> + residual]  /  row-split classifier -> allgather (comm.cu)
         int xchg = 0; float* xdst = nullptr; const float* xres = nullptr;
         if (A.epilogue == 0 && is(i + 1, L_ALLREDUCE) && q[i + 1].a.buf == m0.out && q[i + 1].i0 == m0.a.shape[0]) {
@@ -496,7 +497,6 @@ struct Fuser {
         P.steps.push_back([=](uint8_t* dyn_dev) { return cc_launch_sample(d, x, n, nullptr, (const SampleDyn*)(dyn_dev + off), slot, hist); });
         { MkPhase ph = {}; ph.type = MK_SAMPLE; ph.x = (float*)x; ph.n = (int)n; ph.dyn_off = off; ph.slot_dev = (long long*)slot; ph.hist_dev = (long long*)hist;
           ph.dst = scratch; P.phases.push_back(ph); }
-        P.mega_sample = true;
         q[i].done = true;
         return 1;
     }
@@ -507,43 +507,26 @@ struct Fuser {
     // the whole group is ONE phase: fused prologue (norm + Q8_K quantisation of x) + T::row_dot rows + epilogue -- the same
     // arithmetic as the eager kernels, so the two modes agree bit for bit.
     size_t try_generic(size_t i) {
-        size_t j = i;
-        cc_buf* orig = nullptr; cc_buf* xb = nullptr;
-        const float* norm_w = nullptr; float eps = 0.0f;
-        if (is(j, L_DUP) && is(j + 1, L_RMS_NORM) && q[j + 1].a.buf == q[j].a.buf) { orig = q[j].out; j++; }
-        if (is(j, L_RMS_NORM) && is(j + 1, L_MUL) && q[j + 1].a.buf == q[j].a.buf) {
-            const LOp &rn = q[j], &mu = q[j + 1];
-            const int64_t n = vlen(rn.a);
-            if (rn.a.ndim > 2 || (rn.a.ndim == 2 && rn.a.shape[0] != 1) || !vcontig(rn.a)) return 0;
-            if (vlen(mu.b) != n || mu.b.buf->dtype != CC_F32 || !vcontig(mu.b)) return 0;
-            xb = rn.a.buf; norm_w = (const float*)mu.b.buf->plane[0]; eps = rn.f;
-            j += 2;
-        } else if (orig) return 0;
+        const NormMatch nm = match_norm(i);
+        const size_t j = i + nm.len;           // a DUP or RMS_NORM that is not a whole norm prefix leaves j on an op that is no MATVEC
         if (!is(j, L_MATVEC)) return 0;
         const LOp& m0 = q[j];
-        const int wt = m0.a.buf->dtype;
-        const int64_t k = m0.a.shape[1];
+        const int wt = m0.a.buf->dtype; const int64_t k = m0.a.shape[1];
         if (!cc_mega_generic_supported(wt, k)) return 0;
-        if (!xb) xb = m0.b.buf;
+        cc_buf* xb = nm.len ? nm.x : m0.b.buf;
         if (m0.b.buf != xb || xb->dtype != CC_F32 || vlen(m0.b) != k || !vcontig(m0.b) || (m0.b.ndim == 2 && m0.b.shape[0] != 1) || m0.b.ndim > 2) return 0;
-        size_t n = 1;
-        while (n < 3 && is(j + n, L_MATVEC) && q[j + n].b.buf == xb && q[j + n].a.buf->dtype == wt && q[j + n].a.shape[1] == k && vlen(q[j + n].b) == k) n++;
-        StreamArgs A = {};
-        A.k = (int)k; A.exp_lut = dev->exp_lut;
-        size_t used_mv = n;
-        if (n >= 2 && is(j + 2, L_SILU) && is(j + 3, L_MUL) && q[j + 2].a.buf == q[j].out && q[j + 3].a.buf == q[j].out && q[j + 3].b.buf == q[j + 1].out &&
-            q[j].a.shape[0] == q[j + 1].a.shape[0] && vlen(q[j + 3].b) == q[j].a.shape[0] && dead_after(q[j + 1].out, j + 4)) {
-            n = 2; A.epilogue = 2; used_mv = 4;
-        } else if (n == 1 && is(j + 1, L_ADD) && q[j + 1].a.buf == m0.out && vlen(q[j + 1].b) == m0.a.shape[0] && q[j + 1].b.buf->dtype == CC_F32 && vcontig(q[j + 1].b) &&
-                   q[j + 1].b.buf != xb) {
-            A.epilogue = 1; A.residual = (const float*)q[j + 1].b.buf->plane[0]; used_mv = 2;
-        } else if (n > 1 && is(j + n, L_SILU)) { n = 1; used_mv = 1; }
-        if (is(j + used_mv, L_ALLREDUCE) || is(j + used_mv, L_ALLGATHER)) return 0;      // sharded K-quant models run in the CUDA-graph mode
-        const size_t end = j + used_mv;
+        GroupMatch g = match_group(j, xb, wt, k);
+        // the generic phase never writes a normalised row back (below), so a residual that is x itself would read the wrong row;
+        // the residual add then runs as its own op, with or without a norm
+        if (g.epilogue == 1 && g.residual == xb) g = GroupMatch();
+        if (is(j + g.used, L_ALLREDUCE) || is(j + g.used, L_ALLGATHER)) return 0;      // sharded K-quant models run in the CUDA-graph mode
+        const size_t end = j + g.used;
         // the normalised row is overwritten in place by the eager ops; the fused prologue never materialises it: nobody else may read it
-        if (norm_w && !dead_after(xb, end)) return 0;
-        A.mats.n = (int)n;
-        for (size_t t = 0; t < n; t++) {
+        if (nm.len && !dead_after(xb, end)) return 0;
+        StreamArgs A = {};
+        A.k = (int)k; A.exp_lut = dev->exp_lut; A.epilogue = g.epilogue; A.residual = g.residual ? (const float*)g.residual->plane[0] : nullptr;
+        A.mats.n = (int)g.n;
+        for (size_t t = 0; t < g.n; t++) {
             const cc_buf* w = q[j + t].a.buf;
             if (w->cols != k) return 0;
             A.mats.qs[t] = w->plane[0]; A.mats.d[t] = (const uint16_t*)w->plane[1]; A.mats.p2[t] = w->plane[2]; A.mats.p3[t] = w->plane[3];
@@ -552,14 +535,14 @@ struct Fuser {
         }
         MkPhase ph = {};
         ph.type = MK_MATVEC; ph.wtype = wt; ph.act_type = CC_Q8_K; ph.mv = A;
-        ph.x = (float*)xb->plane[0]; ph.orig = orig ? (float*)orig->base : nullptr; ph.norm_w = norm_w; ph.eps = eps; ph.n = (int)k;
-        ph.norm_ahead = norm_w && !written(q[j - 1].b.buf);
+        ph.x = (float*)xb->plane[0]; ph.orig = nm.orig ? (float*)nm.orig->base : nullptr; ph.eps = nm.eps; ph.n = (int)k;
+        ph.norm_w = nm.len ? (const float*)nm.w->plane[0] : nullptr;
+        ph.norm_ahead = nm.len && !written(nm.w);
         // eager steps for the CUDA-graph mode, op by op, without disqualifying the megakernel form
         covered_by_phase = true;
         for (size_t t = i; t < end; t++) fallback(t);
         covered_by_phase = false;
         P.phases.push_back(ph);
-        P.mega_generic = true;
         return end - i;
     }
 
@@ -619,11 +602,48 @@ struct Fuser {
     }
 };
 
-int cc_lazy_flush(cc_device* dev) {
-    LazyState* lz = dev->lz;
-    if (!lz || lz->q.empty()) return CC_OK;
-    lz->flushes++;
-    // scratch for the quantised activations (largest k in the queue)
+// The persistent kernel that runs a phase table and its launch geometry (MEGA_NONE: the CUDA-graph mode); on success the phases get
+// their links to the next MATVEC phase and to the next fused-norm weights the kernel may stage early.  A table with a streaming (Q8_0 /
+// Q4_0) MATVEC phase runs mega_ring.cu when every such phase can be fed by bulk copies and the ring gets enough slots beside the working
+// area; any other table runs mega.cu when its working area fits.  At head_dim 128 the attention phase's working area (the score row +
+// its chunk buffers) decides this at long contexts; past 50 808 positions the fuser leaves attention to the per-op kernels.
+static MegaLaunch choose_mega(const cc_device* dev, bool mega_ok, std::vector<MkPhase>& phs) {
+    MegaLaunch L;
+    if (!dev->mega || !mega_ok || phs.empty()) return L;
+    bool stream = false, ring_ok = true;
+    int n_sample = 0;
+    for (auto& ph : phs) {
+        if (ph.type == MK_MATVEC) (ph.act_type == CC_Q8_K ? L.generic : stream) = true;
+        if (!cc_mega_ring_phase_ok(ph)) ring_ok = false;
+        n_sample += ph.type == MK_SAMPLE;
+    }
+    // the megakernel runs ONE SAMPLE phase, after its phase loop (mega.cu): a table with more than one, or with anything queued
+    // behind the sampler (several tokens submitted before one flush), runs in the CUDA-graph mode
+    L.sample = n_sample > 0;
+    if (n_sample > 1 || (n_sample == 1 && phs.back().type != MK_SAMPLE)) return L;
+    for (auto& ph : phs) {
+        L.smem = std::max(L.smem, stream ? cc_mega_ring_smem_for_phase(ph) : cc_mega_smem_for_phase(ph));
+        if (ph.type == MK_MATVEC && ph.x && ph.norm_w) L.wstage = std::max(L.wstage, (size_t)ph.n * 4);
+        if (stream && ph.type == MK_MATVEC && ph.act_type != CC_Q8_K) L.slot_bytes = std::max(L.slot_bytes, ph.wtype == CC_Q8_0 ? 4352 : 2304);
+        if (stream && ph.type == MK_ATTN) L.at_ch = cc_mega_ring_at_ch(ph);
+    }
+    if (stream ? !ring_ok || !(L.nslots = cc_mega_ring_slots(L)) : L.smem + L.wstage + 4096 > 227 * 1024) return L;
+    L.variant = stream ? MEGA_RING : MEGA_REGISTER;
+    int nxt = -1, nxn = -1;
+    for (int t = (int)phs.size() - 1; t >= 0; t--) {
+        MkPhase& ph = phs[t];
+        ph.next_matvec = nxt;
+        ph.next_norm_w = nxn >= 0 && phs[nxn].norm_ahead ? phs[nxn].norm_w : nullptr;
+        ph.next_norm_n = ph.next_norm_w ? phs[nxn].n : 0;
+        if (ph.type == MK_MATVEC) nxt = t;
+        if (ph.type == MK_MATVEC && ph.x && ph.norm_w) nxn = t;
+    }
+    return L;
+}
+
+// scratch the queued ops need, at its final size before anything is captured: graphs bake the pointers in
+static int size_scratch(cc_device* dev, LazyState* lz) {
+    // quantised activations (largest k in the queue)
     int64_t max_k = 0;
     for (auto& op : lz->q) if (op.kind == L_MATVEC) max_k = std::max<int64_t>(max_k, std::max<int64_t>(op.a.shape[1], 0));
     // the fused attention quantises its OUTPUT row (n_heads * head_dim = the PV product's a_batch * n) into act[1]; QK^T products
@@ -639,14 +659,98 @@ int cc_lazy_flush(cc_device* dev) {
         for (int i = 0; i < 2; i++) if (cudaMalloc(&lz->act[i], cap) != cudaSuccess) return cc_fail(dev, CC_ERR_CUDA, "lazy: scratch alloc failed");
         lz->act_cap = cap;
     }
-    // eager matvec fallbacks use dev->act_scratch: make sure it is large enough BEFORE any capture
+    // eager matvec fallbacks (cc_launch_matmul_vec) use dev->act_scratch
     for (auto& op : lz->q) if (op.kind == L_MATVEC) {
         int at = cc_partner_type(op.a.buf->dtype);
         int64_t bb = op.b.ndim == 1 ? 1 : op.b.shape[0];
         if (at != CC_F32 && (rc = cc_ensure_act_scratch(dev, cc_act_bytes(at, bb * op.a.shape[1])))) return rc;
     }
-    // the sampler's scratch is baked into captured graphs: it must have its final size before any capture
     for (auto& op : lz->q) if (op.kind == L_SAMPLE && (rc = cc_ensure_sample_scratch(dev, vlen(op.a)))) return rc;
+    return CC_OK;
+}
+
+// per-token values: pinned slot -> device block, as an ordinary stream copy in front of the launches / the graph
+static int upload_dyn(cc_device* dev, LazyState* lz, const Plan& P) {
+    if (P.dyn.size() > lz->dyn_cap) return cc_fail(dev, CC_ERR_UNSUPPORTED, "lazy: dynamic argument block too large");
+    if (P.dyn.empty()) return CC_OK;
+    int rc = CC_OK; const int s = lz->dyn_slot;
+    lz->dyn_slot = (s + 1) % LZ_DYN_SLOTS;
+    cudaEventSynchronize(lz->dyn_ev[s]);          // the copy that last read this slot (LZ_DYN_SLOTS flushes ago) is long done
+    memcpy(lz->dyn_host[s], P.dyn.data(), P.dyn.size());
+    if (cudaMemcpyAsync(lz->dyn_dev, lz->dyn_host[s], P.dyn.size(), cudaMemcpyHostToDevice, dev->stream) != cudaSuccess) rc = cc_fail(dev, CC_ERR_CUDA, "lazy: dyn upload failed");
+    cudaEventRecord(lz->dyn_ev[s], dev->stream);
+    return rc;
+}
+
+static int run_steps(const Plan& P, uint8_t* dyn_dev) {
+    for (auto& st : P.steps) if (int r = st(dyn_dev)) return r;
+    return CC_OK;
+}
+
+// the cached graph of this signature, or end() after making room for a new one
+using GraphCache = std::unordered_map<uint64_t, GraphEntry>;
+static GraphCache::iterator find_graph(cc_device* dev, LazyState* lz, uint64_t key, const std::vector<uint64_t>& sig) {
+    auto it = lz->cache.find(key);
+    if (it != lz->cache.end() && it->second.sig != sig) {          // 64-bit key collision: never replay the other plan's graph
+        lz->collisions++;
+        cudaStreamSynchronize(dev->stream);
+        graph_entry_free(it->second);
+        lz->cache.erase(it);
+        it = lz->cache.end();
+    }
+    if (it == lz->cache.end() && lz->cache.size() >= LZ_MAX_GRAPHS) {   // LRU bound: evict the entry replayed longest ago
+        auto victim = lz->cache.begin();
+        for (auto c = lz->cache.begin(); c != lz->cache.end(); ++c) if (c->second.last_use < victim->second.last_use) victim = c;
+        cudaStreamSynchronize(dev->stream);          // its last launch may still be running
+        graph_entry_free(victim->second);
+        lz->cache.erase(victim);
+        lz->evictions++;
+    }
+    return it;
+}
+
+// capture the plan -- one persistent kernel, or its steps -- into a new cache entry
+static int capture(cc_device* dev, LazyState* lz, Plan& P, uint64_t key, GraphCache::iterator* out) {
+    int rc = CC_OK; lz->captures++;
+    uint64_t l0 = dev->launches; cudaGraph_t graph = nullptr; GraphEntry ge;
+    const MegaLaunch L = choose_mega(dev, P.mega_ok, P.phases);
+    if (L.variant != MEGA_NONE) {       // phase table lives in device memory for the lifetime of the graph
+        if (cudaMalloc(&ge.phases_dev, P.phases.size() * sizeof(MkPhase)) != cudaSuccess ||
+            cudaMemcpy(ge.phases_dev, P.phases.data(), P.phases.size() * sizeof(MkPhase), cudaMemcpyHostToDevice) != cudaSuccess)
+            rc = cc_fail(dev, CC_ERR_CUDA, "lazy: phase table upload failed");
+    }
+    cudaError_t e = rc ? cudaSuccess : cudaStreamBeginCapture(dev->stream, cudaStreamCaptureModeRelaxed);
+    if (!rc && e != cudaSuccess) rc = cc_fail(dev, CC_ERR_CUDA, "lazy: begin capture: %s", cudaGetErrorString(e));
+    if (!rc) {
+        if (L.variant != MEGA_NONE && lz->prof_dev && P.phases.size() < 4000) { lz->prof_types.clear(); for (auto& ph : P.phases) lz->prof_types.push_back(ph.type * 16 + (ph.type == MK_MATVEC ? ph.mv.mats.n + 4 * ph.mv.epilogue + 1024 * (ph.mv.k >> 10) : 0)); }
+        unsigned long long* prof = P.phases.size() < 4000 ? lz->prof_dev : nullptr;
+        if (L.variant == MEGA_NONE) rc = run_steps(P, lz->dyn_dev);
+        else if (L.variant == MEGA_RING) rc = cc_launch_mega_ring(dev, ge.phases_dev, (int)P.phases.size(), lz->dyn_dev, lz->bar_dev, L, prof, cc_comm_dev(dev));
+        else rc = cc_launch_mega(dev, ge.phases_dev, (int)P.phases.size(), lz->dyn_dev, lz->bar_dev, L, prof);
+        e = cudaStreamEndCapture(dev->stream, &graph);
+        if (!rc && e != cudaSuccess) rc = cc_fail(dev, CC_ERR_CUDA, "lazy: end capture: %s", cudaGetErrorString(e));
+    }
+    if (!rc) {
+        e = cudaGraphInstantiate(&ge.exec, graph, 0);
+        if (e != cudaSuccess) rc = cc_fail(dev, CC_ERR_CUDA, "lazy: graph instantiate: %s", cudaGetErrorString(e));
+    }
+    if (graph) cudaGraphDestroy(graph);
+    if (!rc) {
+        ge.mega_variant = L.variant;
+        ge.dyn_bytes = P.dyn.size();
+        ge.sig = P.sig;
+        ge.launches = dev->launches - l0;
+        dev->launches = l0;            // counted when the graph is launched
+        *out = lz->cache.emplace(key, ge).first;
+    }
+    return rc;
+}
+
+int cc_lazy_flush(cc_device* dev) {
+    LazyState* lz = dev->lz;
+    if (!lz || lz->q.empty()) return CC_OK;
+    lz->flushes++;
+    int rc = size_scratch(dev, lz); if (rc) return rc;
     auto t_f0 = std::chrono::steady_clock::now();
     Plan P;
     Fuser F{dev, lz, lz->q, P};
@@ -654,127 +758,20 @@ int cc_lazy_flush(cc_device* dev) {
     auto t_f1 = std::chrono::steady_clock::now();
     lz->ns_fuse += (uint64_t)std::chrono::duration_cast<std::chrono::nanoseconds>(t_f1 - t_f0).count();
     if (P.dyn.size() > lz->dyn_cap) P.cacheable = false;
-
-    auto run_steps = [&](uint8_t* dyn_dev) -> int {
-        for (auto& st : P.steps) { int r = st(dyn_dev); if (r) return r; }
-        return CC_OK;
-    };
-    // per-token values: pinned slot -> device block, as an ordinary stream copy in front of the launches / the graph
-    if (P.dyn.size() > lz->dyn_cap) rc = cc_fail(dev, CC_ERR_UNSUPPORTED, "lazy: dynamic argument block too large");
-    if (!rc && !P.dyn.empty()) {
-        const int s = lz->dyn_slot;
-        lz->dyn_slot = (s + 1) % LZ_DYN_SLOTS;
-        cudaEventSynchronize(lz->dyn_ev[s]);          // the copy that last read this slot (LZ_DYN_SLOTS flushes ago) is long done
-        memcpy(lz->dyn_host[s], P.dyn.data(), P.dyn.size());
-        if (cudaMemcpyAsync(lz->dyn_dev, lz->dyn_host[s], P.dyn.size(), cudaMemcpyHostToDevice, dev->stream) != cudaSuccess) rc = cc_fail(dev, CC_ERR_CUDA, "lazy: dyn upload failed");
-        cudaEventRecord(lz->dyn_ev[s], dev->stream);
-    }
+    rc = upload_dyn(dev, lz, P);
     if (rc) {
     } else if (!P.cacheable) {
         lz->uncached++;
-        rc = run_steps(lz->dyn_dev);
+        rc = run_steps(P, lz->dyn_dev);
     } else {
         P.S(P.dyn.size());
         uint64_t key = hash_sig(P.sig);
-        auto it = lz->cache.find(key);
-        if (it != lz->cache.end() && it->second.sig != P.sig) {          // 64-bit key collision: never replay the other plan's graph
-            lz->collisions++;
-            cudaStreamSynchronize(dev->stream);
-            graph_entry_free(it->second);
-            lz->cache.erase(it);
-            it = lz->cache.end();
-        }
-        if (it == lz->cache.end() && lz->cache.size() >= LZ_MAX_GRAPHS) {   // LRU bound: evict the entry replayed longest ago
-            auto victim = lz->cache.begin();
-            for (auto c = lz->cache.begin(); c != lz->cache.end(); ++c) if (c->second.last_use < victim->second.last_use) victim = c;
-            cudaStreamSynchronize(dev->stream);          // its last launch may still be running
-            graph_entry_free(victim->second);
-            lz->cache.erase(victim);
-            lz->evictions++;
-        }
-        if (it == lz->cache.end()) {
-            lz->captures++;
-            uint64_t l0 = dev->launches;
-            cudaGraph_t graph = nullptr;
-            GraphEntry ge;
-            bool use_mega = dev->mega && P.mega_ok && !P.phases.empty();
-            // the megakernel runs ONE SAMPLE phase, after its phase loop (mega.cu): a table with more than one, or with anything queued
-            // behind the sampler (several tokens submitted before one flush), runs in the CUDA-graph mode
-            if (use_mega && P.mega_sample) {
-                int n_sample = 0;
-                for (auto& ph : P.phases) n_sample += ph.type == MK_SAMPLE;
-                if (n_sample != 1 || P.phases.back().type != MK_SAMPLE) use_mega = false;
-            }
-            // A table with a streaming (Q8_0 / Q4_0) MATVEC phase runs mega_ring.cu when every such phase can be fed by bulk copies and the
-            // ring gets enough slots beside the working area; any other table runs mega.cu when its working area fits.  Otherwise: the
-            // CUDA-graph mode.  At head_dim 128 the attention phase's working area (the score row + its chunk buffers) decides this at
-            // long contexts; past 50 808 positions the fuser leaves attention to the per-op kernels (try_attention).
-            if (use_mega) {
-                bool stream = false, ring_ok = true;
-                for (auto& ph : P.phases) {
-                    if (ph.type == MK_MATVEC && ph.act_type != CC_Q8_K) stream = true;
-                    if (!cc_mega_ring_phase_ok(ph)) ring_ok = false;
-                }
-                P.mega_ring = stream;
-                for (auto& ph : P.phases) {
-                    if (P.mega_ring) {
-                        P.mega_smem = std::max(P.mega_smem, cc_mega_ring_smem_for_phase(ph));
-                        if (ph.type == MK_MATVEC && ph.x && ph.norm_w) P.mega_wstage = std::max(P.mega_wstage, (size_t)ph.n * 4);
-                        if (ph.type == MK_MATVEC && ph.act_type != CC_Q8_K) P.ring_slot = std::max(P.ring_slot, ph.wtype == CC_Q8_0 ? 4352 : 2304);
-                        if (ph.type == MK_ATTN) P.ring_at_ch = cc_mega_ring_at_ch(ph);
-                    } else {
-                        P.mega_smem = std::max(P.mega_smem, cc_mega_smem_for_phase(ph));
-                        if (ph.type == MK_MATVEC && ph.x && ph.norm_w) P.mega_wstage = std::max(P.mega_wstage, (size_t)ph.n * 4);
-                    }
-                }
-                if (P.mega_ring) use_mega = ring_ok && cc_mega_ring_fits(P.mega_smem, P.mega_wstage, P.ring_slot, P.mega_generic);
-                else use_mega = P.mega_smem + P.mega_wstage + 4096 <= 227 * 1024;
-            }
-            if (use_mega) {       // phase table lives in device memory for the lifetime of the graph
-                int nxt = -1, nxn = -1;
-                for (int t = (int)P.phases.size() - 1; t >= 0; t--) {
-                    MkPhase& ph = P.phases[t];
-                    ph.next_matvec = nxt;
-                    ph.next_norm_w = nxn >= 0 && P.phases[nxn].norm_ahead ? P.phases[nxn].norm_w : nullptr;
-                    ph.next_norm_n = ph.next_norm_w ? P.phases[nxn].n : 0;
-                    if (ph.type == MK_MATVEC) nxt = t;
-                    if (ph.type == MK_MATVEC && ph.x && ph.norm_w) nxn = t;
-                }
-                if (cudaMalloc(&ge.phases_dev, P.phases.size() * sizeof(MkPhase)) != cudaSuccess ||
-                    cudaMemcpy(ge.phases_dev, P.phases.data(), P.phases.size() * sizeof(MkPhase), cudaMemcpyHostToDevice) != cudaSuccess)
-                    rc = cc_fail(dev, CC_ERR_CUDA, "lazy: phase table upload failed");
-            }
-            cudaError_t e = rc ? cudaSuccess : cudaStreamBeginCapture(dev->stream, cudaStreamCaptureModeRelaxed);
-            if (!rc && e != cudaSuccess) rc = cc_fail(dev, CC_ERR_CUDA, "lazy: begin capture: %s", cudaGetErrorString(e));
-            if (!rc) {
-                if (use_mega && lz->prof_dev && P.phases.size() < 4000) { lz->prof_types.clear(); for (auto& ph : P.phases) lz->prof_types.push_back(ph.type * 16 + (ph.type == MK_MATVEC ? ph.mv.mats.n + 4 * ph.mv.epilogue + 1024 * (ph.mv.k >> 10) : 0)); }
-                unsigned long long* prof = P.phases.size() < 4000 ? lz->prof_dev : nullptr;
-                if (!use_mega) rc = run_steps(lz->dyn_dev);
-                else if (P.mega_ring) rc = cc_launch_mega_ring(dev, ge.phases_dev, (int)P.phases.size(), lz->dyn_dev, lz->bar_dev, P.mega_smem, P.mega_wstage, prof, cc_comm_dev(dev),
-                                                               P.mega_generic, P.mega_sample, P.ring_slot, P.ring_at_ch);
-                else rc = cc_launch_mega(dev, ge.phases_dev, (int)P.phases.size(), lz->dyn_dev, lz->bar_dev, P.mega_smem, P.mega_wstage, prof, P.mega_sample);
-                e = cudaStreamEndCapture(dev->stream, &graph);
-                if (!rc && e != cudaSuccess) rc = cc_fail(dev, CC_ERR_CUDA, "lazy: end capture: %s", cudaGetErrorString(e));
-            }
-            if (!rc) {
-                e = cudaGraphInstantiate(&ge.exec, graph, 0);
-                if (e != cudaSuccess) rc = cc_fail(dev, CC_ERR_CUDA, "lazy: graph instantiate: %s", cudaGetErrorString(e));
-            }
-            if (graph) cudaGraphDestroy(graph);
-            if (!rc) {
-                ge.mega_variant = use_mega ? (P.mega_ring ? 2 : 1) : 0;
-                ge.dyn_bytes = P.dyn.size();
-                ge.sig = P.sig;
-                ge.launches = dev->launches - l0;
-                dev->launches = l0;            // counted when the graph is launched
-                it = lz->cache.emplace(key, ge).first;
-            }
-        } else {
-            lz->graph_hits++;
-        }
+        auto it = find_graph(dev, lz, key, P.sig);
+        if (it != lz->cache.end()) lz->graph_hits++;
+        else rc = capture(dev, lz, P, key, &it);
         if (!rc) {
             it->second.last_use = lz->flushes;
-            if (it->second.mega_variant) lz->mega_variant = it->second.mega_variant;
+            if (it->second.mega_variant != MEGA_NONE) lz->mega_variant = it->second.mega_variant;
             cudaError_t e = cudaGraphLaunch(it->second.exec, dev->stream);
             if (e != cudaSuccess) rc = cc_fail(dev, CC_ERR_CUDA, "lazy: graph launch: %s", cudaGetErrorString(e));
             else dev->launches += it->second.launches;

@@ -134,7 +134,7 @@ __global__ void __launch_bounds__(MK_THREADS, MK_CTAS_PER_SM) mega_kernel(const 
     if (prof && blockIdx.x == 0 && threadIdx.x == 0) prof[n_phases * MK_PROF_SLOTS] = globaltimer_ns();
 }
 
-// working shared memory of one phase (the staging area of the norm weights comes on top, see cc_launch_mega); a MATVEC phase here is
+// working shared memory of one phase (the staging area of the norm weights comes on top: MegaLaunch::wstage); a MATVEC phase here is
 // generic (K-quant weights): the streaming ones run mega_ring.cu, whose working areas are cc_mega_ring_smem_for_phase
 size_t cc_mega_smem_for_phase(const MkPhase& ph) {
     if (ph.type == MK_MATVEC) return (size_t)(((TKBase::smem_bytes(ph.mv.k) + 15) & ~15) + 256) + (size_t)ph.mv.k * 4;
@@ -158,7 +158,9 @@ extern "C" CC_API int cc_test_mega_barrier_floor(cc_device* dev, int n, float* u
     for (int rep = 0; rep < 4; rep++) {
         CC_CUDA(dev, cudaMemsetAsync(d_bar, 0, 4096, dev->stream));
         cudaEventRecord(e0, dev->stream);
-        int rc = cc_launch_mega(dev, d_tab, n, nullptr, d_bar, 1024, 0, nullptr, false);
+        MegaLaunch L;
+        L.variant = MEGA_REGISTER;
+        int rc = cc_launch_mega(dev, d_tab, n, nullptr, d_bar, L, nullptr);
         if (rc) return rc;
         cudaEventRecord(e1, dev->stream);
         CC_CUDA(dev, cudaEventSynchronize(e1));
@@ -180,32 +182,18 @@ bool cc_mega_test_stall() {
     return on;
 }
 
-int cc_launch_mega(cc_device* dev, const MkPhase* phases_dev, int n_phases, const uint8_t* dyn_dev, unsigned* bar_dev, size_t smem_work, size_t smem_wstage,
-                   unsigned long long* prof, bool sample) {
+int cc_launch_mega(cc_device* dev, const MkPhase* phases_dev, int n_phases, const uint8_t* dyn_dev, unsigned* bar_dev, const MegaLaunch& L,
+                   unsigned long long* prof) {
     int max_ctas_per_sm = 0;
-    const size_t wtop = (smem_work + 15) & ~(size_t)15;
-    const size_t smem = wtop + smem_wstage;
+    const size_t wtop = (L.smem + 15) & ~(size_t)15;
+    const size_t smem = wtop + L.wstage;
     CC_REQUIRE(dev, smem <= 227 * 1024, "megakernel: a phase needs %zu bytes of shared memory", smem);
-    auto kern = sample ? mega_kernel<true> : mega_kernel<false>;
+    auto kern = L.sample ? mega_kernel<true> : mega_kernel<false>;
     if (smem > 48 * 1024) CC_CUDA(dev, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     CC_CUDA(dev, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&max_ctas_per_sm, kern, MK_THREADS, smem));
     CC_REQUIRE(dev, max_ctas_per_sm >= 1, "megakernel does not fit on an SM");
     int per_sm = max_ctas_per_sm < MK_CTAS_PER_SM ? max_ctas_per_sm : MK_CTAS_PER_SM;
-    int grid = dev->sm_count * per_sm;          // all CTAs co-resident: required by the grid barrier
-    // The grid barrier needs every CTA resident at once.  On a GPU this process owns, a plain launch of sm_count CTAs (1 per SM)
-    // is co-resident by construction.  With another tenant on the same GPU (a second process, MPS) a partially scheduled grid
-    // cannot finish a barrier: every spin in the kernel is bounded (MkSpin) and ends in CC_ERR_CUDA "megakernel barrier timeout"
-    // instead of a hang; CRABML_MEGA_COOP=1 adds the cooperative launch attribute (all-or-nothing placement).  That is opt-in
-    // because a cooperative kernel node in a CUDA graph is much slower to launch than a plain one.
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3((unsigned)grid); cfg.blockDim = dim3(MK_THREADS); cfg.dynamicSmemBytes = smem; cfg.stream = dev->stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeCooperative;
-    attr[0].val.cooperative = getenv("CRABML_MEGA_COOP") ? 1 : 0;
-    cfg.attrs = attr; cfg.numAttrs = 1;
     const uint16_t* lut = dev->exp_lut;
-    CC_CUDA(dev, cudaLaunchKernelEx(&cfg, kern, phases_dev, n_phases, dyn_dev, bar_dev, lut, prof, cc_mega_test_stall(), (int)wtop, dev->err_host));
-    CC_LAUNCH_CHECK(dev);
-    return CC_OK;
+    return mk_launch(dev, kern, dev->sm_count * per_sm, MK_THREADS, smem, phases_dev, n_phases, dyn_dev, bar_dev, lut, prof, cc_mega_test_stall(),
+                     (int)wtop, dev->err_host);
 }

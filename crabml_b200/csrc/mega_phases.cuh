@@ -565,3 +565,22 @@ static __device__ void phase_reduce(const MkPhase& ph, const CommDev& comm, unsi
                              // 6-7 ring consumer counters, 8 norm weights available (mega_ring.cu)
 
 #define MK_F_TESTSTALL 128     // test hook: the last CTA leaves before barrier 2 -> every other CTA must time out, not hang (cc_mega_test_stall)
+
+// Launch of a persistent kernel (mega.cu, mega_ring.cu).  The grid barrier needs every CTA resident at once.  On a GPU this process
+// owns, a plain launch of one CTA per SM is co-resident by construction.  With another tenant on the same GPU (a second process, MPS)
+// a partially scheduled grid cannot finish a barrier: every spin in the kernel is bounded (MkSpin) and ends in CC_ERR_CUDA "megakernel
+// barrier timeout" instead of a hang; CRABML_MEGA_COOP=1 adds the cooperative launch attribute (all-or-nothing placement).  That is
+// opt-in because a cooperative kernel node in a CUDA graph is much slower to launch than a plain one.
+template <typename... P, typename... A>
+static int mk_launch(cc_device* dev, void (*kern)(P...), int grid, int threads, size_t smem, A... args) {
+    cudaLaunchConfig_t cfg;
+    memset(&cfg, 0, sizeof(cfg));
+    cfg.gridDim = dim3((unsigned)grid); cfg.blockDim = dim3(threads); cfg.dynamicSmemBytes = smem; cfg.stream = dev->stream;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeCooperative;
+    attr[0].val.cooperative = getenv("CRABML_MEGA_COOP") ? 1 : 0;
+    cfg.attrs = attr; cfg.numAttrs = 1;
+    CC_CUDA(dev, cudaLaunchKernelEx(&cfg, kern, args...));
+    CC_LAUNCH_CHECK(dev);
+    return CC_OK;
+}

@@ -25,7 +25,7 @@
 #define MR_PRODUCER_WARPS 4        // 20 warps: five per SM sub-partition, still 96 registers per thread
 #define MR_THREADS (MK_THREADS + 32 * MR_PRODUCER_WARPS)
 #define MR_MAX_SLOTS 112
-#define MR_Q8_SLOTS 24             // ring depth for Q8_0 entries (cc_launch_mega_ring)
+#define MR_Q8_SLOTS 24             // ring depth for Q8_0 entries (cc_mega_ring_slots)
 #define MR_DESC_WORDS ((int)(sizeof(MkPhase) / 4))
 #define MR_DESC_PER_LANE ((MR_DESC_WORDS + 31) / 32)
 
@@ -640,37 +640,35 @@ size_t cc_mega_ring_smem_for_phase(const MkPhase& ph) {
     if (ph.type == MK_SAMPLE) return SMP_SMEM_BYTES;
     return 1024;
 }
-// slots the ring would get beside a working area of `smem_work` bytes and the norm-weight stage of `smem_wstage` bytes (the largest
-// n * 4 of a fused-norm phase); lazy.cu runs the table in the CUDA-graph mode
-// below MR_MIN_SLOTS -- e.g. a 32 K-token context, whose attention phase needs 128 KB for the score row alone
+// Ring layout, for the fit decision (lazy.cu choose_mega) and the launch alike: the ring starts at mr_ring_off, after the working area
+// and the norm-weight stage, and takes what is left of the SM's shared memory.  Returns the slot count, or 0 when fewer than
+// MR_MIN_SLOTS fit -- e.g. a 32 K-token context, whose attention phase needs 128 KB for the score row alone -- and lazy.cu runs the
+// table in the CUDA-graph mode.
+// Ring depth: a Q8_0 ring (4352-byte slots) is faster SHALLOW -- 24 slots = 104 KB per SM decode a Llama-2-7B token in 3.88 ms
+// against 4.04 ms with the ~40 that fit, and 20 / 16 / 12 slots are slower again (NVIDIA H100 80GB HBM3, 400 W).  Retuned with the
+// prologue inputs staged early: 16-24 slots within the spread, 28 and 32 are 4-6 % slower (same card, 700 W).  The Q4_0 consumer is
+// ALU-bound and keeps every slot that fits: a 55 KB ring (24 of its slots) cost it 2-4 %, 46 KB 9 %.
 #define MR_MIN_SLOTS 12
-static size_t mr_ring_off(size_t smem_work, size_t smem_wstage) { return ((((smem_work + 15) & ~(size_t)15) + smem_wstage) + 127) & ~(size_t)127; }
-int cc_mega_ring_slots(size_t smem_work, size_t smem_wstage, int slot_bytes, bool generic) {
-    cudaFuncAttributes fa;
-    if (cudaFuncGetAttributes(&fa, generic ? mega_ring_kernel<true, false> : mega_ring_kernel<false, false>) != cudaSuccess) { cudaGetLastError(); return 0; }
-    const size_t cap = 227 * 1024 - fa.sharedSizeBytes, off = mr_ring_off(smem_work, smem_wstage);
-    if (slot_bytes <= 0 || off >= cap) return 0;
-    const size_t n = (cap - off) / (size_t)slot_bytes;
-    return (int)(n > MR_MAX_SLOTS ? MR_MAX_SLOTS : n);
+static size_t mr_ring_off(const MegaLaunch& L) { return ((((L.smem + 15) & ~(size_t)15) + L.wstage) + 127) & ~(size_t)127; }
+static auto mr_kernel(const MegaLaunch& L) {
+    return L.generic ? (L.sample ? mega_ring_kernel<true, true> : mega_ring_kernel<true, false>) : (L.sample ? mega_ring_kernel<false, true> : mega_ring_kernel<false, false>);
 }
-bool cc_mega_ring_fits(size_t smem_work, size_t smem_wstage, int slot_bytes, bool generic) { return cc_mega_ring_slots(smem_work, smem_wstage, slot_bytes, generic) >= MR_MIN_SLOTS; }
-
-int cc_launch_mega_ring(cc_device* dev, const MkPhase* phases_dev, int n_phases, const uint8_t* dyn_dev, unsigned* bar_dev, size_t smem_work, size_t smem_wstage,
-                        unsigned long long* prof, const CommDev* comm, bool generic, bool sample, int slot_bytes, int at_ch) {
-    auto kern = generic ? (sample ? mega_ring_kernel<true, true> : mega_ring_kernel<true, false>) : (sample ? mega_ring_kernel<false, true> : mega_ring_kernel<false, false>);
+int cc_mega_ring_slots(const MegaLaunch& L) {
     cudaFuncAttributes fa;
-    CC_CUDA(dev, cudaFuncGetAttributes(&fa, kern));
-    const size_t wtop = (smem_work + 15) & ~(size_t)15;
-    const size_t ring_off = (wtop + smem_wstage + 127) & ~(size_t)127;
-    const size_t cap = 227 * 1024 - fa.sharedSizeBytes;
-    CC_REQUIRE(dev, ring_off + 4 * (size_t)slot_bytes <= cap, "megakernel: the phases leave no room for the weight ring (%zu bytes of working area)", ring_off);
-    const int fit = std::min((int)((cap - ring_off) / (size_t)slot_bytes), MR_MAX_SLOTS);
-    // Ring depth: a Q8_0 ring (4352-byte slots) is faster SHALLOW -- 24 slots = 104 KB per SM decode a Llama-2-7B token in 3.88 ms
-    // against 4.04 ms with the ~40 that fit, and 20 / 16 / 12 slots are slower again (NVIDIA H100 80GB HBM3, 400 W).  Retuned with the
-    // prologue inputs staged early: 16-24 slots within the spread, 28 and 32 are 4-6 % slower (same card, 700 W).  The Q4_0 consumer is
-    // ALU-bound and keeps every slot that fits: a 55 KB ring (24 of its slots) cost it 2-4 %, 46 KB 9 %.
-    const int nslots = slot_bytes >= 4352 ? std::min(fit, MR_Q8_SLOTS) : fit;
-    const size_t smem = ring_off + (size_t)nslots * slot_bytes;
+    if (cudaFuncGetAttributes(&fa, mr_kernel(L)) != cudaSuccess) { cudaGetLastError(); return 0; }
+    const size_t cap = 227 * 1024 - fa.sharedSizeBytes, off = mr_ring_off(L);
+    if (L.slot_bytes <= 0 || off >= cap) return 0;
+    const int fit = (int)std::min((cap - off) / (size_t)L.slot_bytes, (size_t)MR_MAX_SLOTS);
+    if (fit < MR_MIN_SLOTS) return 0;
+    return L.slot_bytes >= 4352 ? std::min(fit, MR_Q8_SLOTS) : fit;
+}
+
+int cc_launch_mega_ring(cc_device* dev, const MkPhase* phases_dev, int n_phases, const uint8_t* dyn_dev, unsigned* bar_dev, const MegaLaunch& L,
+                        unsigned long long* prof, const CommDev* comm) {
+    auto kern = mr_kernel(L);
+    const size_t wtop = (L.smem + 15) & ~(size_t)15;
+    const size_t ring_off = mr_ring_off(L);
+    const size_t smem = ring_off + (size_t)L.nslots * L.slot_bytes;
     CC_CUDA(dev, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     int max_ctas_per_sm = 0;
     CC_CUDA(dev, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&max_ctas_per_sm, kern, MR_THREADS, smem));
@@ -679,16 +677,8 @@ int cc_launch_mega_ring(cc_device* dev, const MkPhase* phases_dev, int n_phases,
     memset(&cd, 0, sizeof(cd));
     if (comm) cd = *comm;
     MrRing R;
-    R.ring_off = (int)ring_off; R.slot_bytes = slot_bytes; R.nslots = nslots; R.at_ch = at_ch;
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3((unsigned)dev->sm_count); cfg.blockDim = dim3(MR_THREADS); cfg.dynamicSmemBytes = smem; cfg.stream = dev->stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeCooperative;
-    attr[0].val.cooperative = getenv("CRABML_MEGA_COOP") ? 1 : 0;          // see cc_launch_mega
-    cfg.attrs = attr; cfg.numAttrs = 1;
+    R.ring_off = (int)ring_off; R.slot_bytes = L.slot_bytes; R.nslots = L.nslots; R.at_ch = L.at_ch;
     const uint16_t* lut = dev->exp_lut;
-    CC_CUDA(dev, cudaLaunchKernelEx(&cfg, kern, phases_dev, n_phases, dyn_dev, bar_dev, lut, prof, cc_mega_test_stall(), (int)wtop, dev->err_host, (const CommDev)cd, (const MrRing)R));
-    CC_LAUNCH_CHECK(dev);
-    return CC_OK;
+    return mk_launch(dev, kern, dev->sm_count, MR_THREADS, smem, phases_dev, n_phases, dyn_dev, bar_dev, lut, prof, cc_mega_test_stall(), (int)wtop,
+                     dev->err_host, (const CommDev)cd, (const MrRing)R);
 }

@@ -1,0 +1,182 @@
+"""Which ops the lazy fuser (lazy.cu) fuses, and which persistent kernel runs them.  Bit-identity alone cannot see a fusion that
+silently stops happening, since an unfused op gives the same bits through its eager kernel.  So each case pins, besides eager logits:
+lazy mode 1's kernel launches per token and its uncached flushes, and lazy mode 2's kernel variant and phase table fingerprint.  A
+fingerprint lists the type codes of cc_lazy_mega_profile: 16 * type (0 NORMQ, 1 MATVEC, 2 ATTN, 3 ROWS, 4 REDUCE, 5 GATHER,
+6 ARGMAX, 7 SAMPLE), plus for a MATVEC phase its matrix count + 4 * epilogue + 1024 * (k >> 10)."""
+import ctypes as C
+
+import numpy as np
+import pytest
+
+from oracle import oracle as oc
+from tests.gpu_common import make_device
+
+pytestmark = pytest.mark.gpu
+
+PROMPT = [1, 365, 2354]
+L7B = (32, 32, 1, 4096, 11008, 64, 32000, 1e-5, 128)
+
+
+def _fingerprint(dev):
+    cap = 9 * 4097
+    ts, ty, n = (C.c_uint64 * cap)(), (C.c_int32 * cap)(), C.c_int32(0)
+    dev.check(dev.lib.cc_lazy_mega_profile(dev.handle, ts, ty, cap, C.byref(n)))
+    return tuple(ty[:n.value])
+
+
+def _history(dev, count):
+    out = (C.c_int64 * count)()
+    dev.check(dev.lib.cc_read_history(dev.handle, 0, count, out))
+    return np.array(out[:], np.int64)
+
+
+def _decode(weights, sample=False):
+    """Decode from a slot (ROWS phase first, ARGMAX or SAMPLE last): launches of one generated token, and the logits."""
+    def case(dev):
+        from crabml_b200 import runner as R
+        conf, w = weights(dev)
+        counts, logits = [], None
+        for steps in (3, 4):
+            r = R.LlamaRunner(dev, conf, w, 16)
+            l0 = dev.launch_count()
+            if sample:
+                _, logits = r.generate_logits(PROMPT, steps, 1.0, 0.9, 7)
+            else:
+                _, logits = r.generate_greedy_logits(PROMPT, steps)
+            counts.append(dev.launch_count() - l0)
+            r.close()
+        return counts[1] - counts[0], logits
+    return case
+
+
+def _synth(wt, ct):
+    def weights(dev):
+        from crabml_b200 import runner as R
+        conf = R.LlamaConfig(*L7B)
+        return conf, R.synthetic_weights(dev, conf, wt, ct, seed=0xF5)
+    return weights
+
+
+def _fixture(path):
+    def weights(dev):
+        from crabml_b200 import runner as R
+        conf, w, _ = R.load_gguf(path, dev)
+        return conf, w
+    return weights
+
+
+def _ops(body, comm=False, rounds=3):
+    """Replay an op sequence `rounds` times; each round ends in an export (one flush).  Launches of the last round, and its outputs."""
+    def case(dev):
+        from crabml_b200 import CudaTensor, capi
+        from crabml_b200.runner import synth_scale
+        if comm:
+            dev.init_comm(0, 1)
+        rng, weights = np.random.default_rng(9), {}
+
+        def W(m, k, t, i):                 # made in the first round, which the measured last round does not see
+            if (m, k, t, i) not in weights:
+                weights[m, k, t, i] = CudaTensor.synth([m, k], t, dev, 3, i, synth_scale(t, k))
+            return weights[m, k, t, i]
+        T = lambda v: CudaTensor.new(np.asarray(v, np.float32), [len(v)], dev)                           # noqa: E731
+        env = dict(dev=dev, rng=rng, T=T, W=W, capi=capi, CudaTensor=CudaTensor)
+        for _ in range(rounds):
+            l0 = dev.launch_count()
+            out = body(env)
+            n = dev.launch_count() - l0
+        return n, out
+    return case
+
+
+def _gate_up_no_silu(e):            # two matvecs on one row, nothing after them
+    x = e["T"](e["rng"].standard_normal(512))
+    ys = [e["W"](256, 512, e["capi"].Q8_0, i).matmul_vec(x) for i in (1, 2)]
+    return np.concatenate([y.export() for y in ys])
+
+
+def _three_then_silu(e):            # q, k, v on one row, then silu on the first
+    x = e["T"](e["rng"].standard_normal(512))
+    ys = [e["W"](256, 512, e["capi"].Q8_0, i).matmul_vec(x) for i in (1, 2, 3)]
+    ys[0].silu_inplace()
+    return np.concatenate([y.export() for y in ys])
+
+
+def _kquant_self_residual(e):       # K-quant matvec + its own input row
+    x = e["T"](e["rng"].standard_normal(512))
+    return e["W"](512, 512, e["capi"].Q4_K, 1).matmul_vec(x).add_inplace(x).export()
+
+
+def _norm_weight_written(e):        # the fused norm's weight row is the output of an earlier matvec of the same flush
+    z, x = e["T"](e["rng"].standard_normal(512)), e["T"](e["rng"].standard_normal(512))
+    nw = e["W"](512, 512, e["capi"].Q8_0, 1).matmul_vec(z)
+    x.rms_norm_inplace(1e-5)
+    x.mul_inplace(nw)
+    return e["W"](256, 512, e["capi"].Q8_0, 2).matmul_vec(x).export()
+
+
+def _exchange(gather):              # world of one: matvec -> all_reduce -> + residual, or matvec -> all_gather
+    def body(e):
+        x, r = e["T"](e["rng"].standard_normal(4096)), e["T"](e["rng"].standard_normal(1024))
+        y = e["W"](1024, 4096, e["capi"].Q8_0, 5).matmul_vec(x)
+        if gather:
+            return e["CudaTensor"].alloc([1024], e["capi"].F32, e["dev"]).all_gather_from(y).export()
+        return y.all_reduce_sum_inplace().add_inplace(r).export()
+    return body
+
+
+def _samplers(n):
+    def body(e):
+        t = e["T"](2.0 * e["rng"].standard_normal(64))
+        for i in range(n):
+            t.sample_to_slot(1.0, 0.9, 5, i, i, i)
+        return _history(e["dev"], n)
+    return body
+
+
+def _tinyllamas(fixture_path):
+    return _decode(_fixture(fixture_path("tinyllamas-stories-15m-q8_0.gguf")))
+
+
+# id: (case, mode-1 launches per token, mode-1 uncached flushes, mode-2 variant (0: CUDA graph), mode-2 fingerprint).  Codes: 48 ROWS (a
+# CudaTensor.new upload, too), 32 ATTN, 0 NORMQ, 96 ARGMAX, 112 SAMPLE, 64 REDUCE, 80 GATHER; 16 + n + 4 * epilogue + 1024 * (k >> 10) MATVEC.
+DECODE_7B = (48, 4115, 32, 4117, 4122, 10261, 0, 48, 4113, 96)     # embedding row; qkv + prologue, attn, wo + res, gate/up + prologue,
+#                                          down (k 11008) + res; final norm, a row copy, classifier + prologue, argmax
+TINY_LAYER = (19, 32, 0, 21, 26, 21)      # head_dim 48: qkv + prologue, attn, plain quantise of its output, wo + res, gate/up, down + res
+CASES = {
+    "7b-q8_0": (lambda fp: _decode(_synth(oc.Q8_0, oc.Q8_0)), 14, 0, 2, DECODE_7B),          # ring kernel
+    "7b-q4_0-q6k": (lambda fp: _decode(_synth(oc.Q4_0, oc.Q6_K)), 14, 0, 2, DECODE_7B),      # Q6_K classifier: a generic phase in the ring table
+    "7b-q4_k": (lambda fp: _decode(_synth(oc.Q4_K, oc.Q6_K)), 29, 0, 1, DECODE_7B),          # mega_kernel; mode 1 runs K-quant ops eagerly
+    "tinyllamas-q8_0": (_tinyllamas, 60, 0, 2, (48,) + TINY_LAYER * 6 + (0, 48, 17, 96)),
+    "7b-q8_0-sampled": (lambda fp: _decode(_synth(oc.Q8_0, oc.Q8_0), sample=True), 14, 0, 2, DECODE_7B[:-1] + (112,)),
+    "two-samplers": (lambda fp: _ops(_samplers(2)), 3, 0, 0, ()),                             # upload + 2 samplers, in the graph
+    "allreduce-add": (lambda fp: _ops(_exchange(False), comm=True), 5, 0, 2, (48, 48, 4125, 64)),   # x, r; matvec into the exchange, reduce + r
+    "allgather": (lambda fp: _ops(_exchange(True), comm=True), 5, 0, 2, (48, 48, 4125, 80)),
+    "gate-up-no-silu": (lambda fp: _ops(_gate_up_no_silu), 3, 0, 2, (48, 18)),               # x; one 2-matrix phase with a plain quantise
+    "three-then-silu": (lambda fp: _ops(_three_then_silu), 8, 0, 0, ()),                      # silu is an eager op: no persistent kernel
+    "kquant-self-residual": (lambda fp: _ops(_kquant_self_residual), 4, 0, 0, ()),             # the add is an eager op
+    "norm-weight-written": (lambda fp: _ops(_norm_weight_written), 6, 0, 2, (48, 48, 17, 0, 17)),    # z, x; nw; norm written back (x lives on), matvec
+}
+
+
+def run_case(name, lazy, fixture_path):
+    """(launches per token, uncached flushes, variant, fingerprint, output) of one case in one lazy mode, on a fresh device."""
+    dev = make_device(lazy=lazy)
+    try:
+        launches, out = CASES[name][0](fixture_path)(dev)
+        st = dev.lazy_stats() if lazy else {"uncached": 0}
+        return launches, st["uncached"], dev.mega_variant(), _fingerprint(dev) if lazy == 2 else (), np.asarray(out).copy()
+    finally:
+        dev.close()
+
+
+@pytest.mark.parametrize("name", list(CASES))
+def test_fusion_plan(name, fixture_path, monkeypatch):
+    monkeypatch.setenv("CRABML_MEGA_PROF", "1")
+    _, launches, uncached, variant, fingerprint = CASES[name]
+    _, _, _, _, ref = run_case(name, 0, fixture_path)
+    got1 = run_case(name, 1, fixture_path)
+    got2 = run_case(name, 2, fixture_path)
+    assert (got1[0], got1[1]) == (launches, uncached)
+    assert (got2[2], got2[3]) == (variant, fingerprint)
+    for got in (got1[4], got2[4]):
+        np.testing.assert_array_equal(got.view(np.uint32) if got.dtype == np.float32 else got, ref.view(np.uint32) if ref.dtype == np.float32 else ref)
