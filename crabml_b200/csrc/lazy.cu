@@ -183,6 +183,9 @@ struct Fuser {
         return b->refs.load() == held;
     }
     static bool same_dense_1xN(const LView& v, int64_t n) { return vcontig(v) && vlen(v) == n; }
+    // an ADD / MUL that covers all n elements: the recorded counts are those capi.cu's binary() kept after chunks_exact(4), which
+    // skips the tail of an rhs longer than 1 (arithmetic.rs:5-68) -- a fused epilogue or norm would apply it to every element
+    bool covers(const LOp& op, int64_t n) const { return op.i0 == n && op.i1 == n; }
 
     // ---- eager fallback for one op -----------------------------------------------------------------------------
     bool covered_by_phase = false;     // set while try_generic emits the eager steps of ops its megakernel phase covers
@@ -258,7 +261,7 @@ struct Fuser {
         if (mu.a.buf != rn.a.buf) return NormMatch();
         const int64_t n = vlen(rn.a);
         if (rn.a.ndim > 2 || (rn.a.ndim == 2 && rn.a.shape[0] != 1) || !vcontig(rn.a)) return NormMatch();
-        if (vlen(mu.b) != n || mu.b.buf->dtype != CC_F32 || !vcontig(mu.b)) return NormMatch();
+        if (vlen(mu.b) != n || mu.b.buf->dtype != CC_F32 || !vcontig(mu.b) || !covers(mu, n)) return NormMatch();
         m.len = j + 2 - i; m.x = rn.a.buf; m.w = mu.b.buf; m.n = n; m.eps = rn.f;
         return m;
     }
@@ -278,10 +281,10 @@ struct Fuser {
         g.used = g.n;
         const LOp& m0 = q[j];
         if (g.n >= 2 && is(j + 2, L_SILU) && is(j + 3, L_MUL) && q[j + 2].a.buf == m0.out && q[j + 3].a.buf == m0.out && q[j + 3].b.buf == q[j + 1].out &&
-            m0.a.shape[0] == q[j + 1].a.shape[0] && vlen(q[j + 3].b) == m0.a.shape[0] && dead_after(q[j + 1].out, j + 4)) {
+            m0.a.shape[0] == q[j + 1].a.shape[0] && vlen(q[j + 3].b) == m0.a.shape[0] && covers(q[j + 3], m0.a.shape[0]) && dead_after(q[j + 1].out, j + 4)) {
             g.n = 2; g.epilogue = 2; g.used = 4;
-        } else if (g.n == 1 && is(j + 1, L_ADD) && q[j + 1].a.buf == m0.out && vlen(q[j + 1].b) == m0.a.shape[0] && q[j + 1].b.buf->dtype == CC_F32 &&
-                   vcontig(q[j + 1].b)) {
+        } else if (g.n == 1 && is(j + 1, L_ADD) && q[j + 1].a.buf == m0.out && vlen(q[j + 1].b) == m0.a.shape[0] && covers(q[j + 1], m0.a.shape[0]) &&
+                   q[j + 1].b.buf->dtype == CC_F32 && vcontig(q[j + 1].b)) {
             g.epilogue = 1; g.residual = q[j + 1].b.buf; g.used = 2;
         } else if (g.n > 1 && is(j + g.n, L_SILU)) {
             g.n = 1; g.used = 1;                   // do not swallow a gate/up pair we could not fuse as a pair
@@ -330,7 +333,8 @@ struct Fuser {
         int xchg = 0; float* xdst = nullptr; const float* xres = nullptr;
         if (A.epilogue == 0 && is(i + 1, L_ALLREDUCE) && q[i + 1].a.buf == m0.out && q[i + 1].i0 == m0.a.shape[0]) {
             n = 1; xchg = 1; used = 2; xdst = (float*)m0.out->base;
-            if (is(i + 2, L_ADD) && q[i + 2].a.buf == m0.out && vlen(q[i + 2].b) == m0.a.shape[0] && q[i + 2].b.buf->dtype == CC_F32 && vcontig(q[i + 2].b)) {
+            if (is(i + 2, L_ADD) && q[i + 2].a.buf == m0.out && vlen(q[i + 2].b) == m0.a.shape[0] && covers(q[i + 2], m0.a.shape[0]) &&
+                q[i + 2].b.buf->dtype == CC_F32 && vcontig(q[i + 2].b)) {
                 xres = (const float*)q[i + 2].b.buf->plane[0];
                 used = 3;
             }

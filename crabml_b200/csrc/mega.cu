@@ -67,9 +67,11 @@ __global__ void __launch_bounds__(MK_THREADS, MK_CTAS_PER_SM) mega_kernel(const 
         const bool look = nx > p && nx < n_phases;
         int desc_w = 0, next_w = 0;
         if (p + 1 < n_phases && threadIdx.x < sizeof(MkPhase) / 4) desc_w = ((const int*)(phases + p + 1))[threadIdx.x];
+        // only weights no phase of the table writes (norm_ahead): they are requested before the barrier, i.e. before the phases in
+        // between have finished on every CTA
         if (look && threadIdx.x < 3) {
             const MkPhase* ph = phases + nx;
-            next_w = threadIdx.x < 2 ? ((const int*)&ph->norm_w)[threadIdx.x] : ph->x && ph->norm_w ? ph->n : 0;
+            next_w = threadIdx.x < 2 ? ((const int*)&ph->norm_w)[threadIdx.x] : ph->x && ph->norm_w && ph->norm_ahead ? ph->n : 0;
         }
         switch (s_ph.type) {
         case MK_NORMQ: phase_normq(s_ph, s_red); break;

@@ -57,6 +57,17 @@ def _synth(wt, ct):
     return weights
 
 
+def _synth_q4_k_m(dev):
+    """the 7B-shaped Q4_K layer laid out like llama.cpp's Q4_K_M: wv and ffn_down in Q6_K"""
+    from crabml_b200 import CudaTensor
+    from crabml_b200 import runner as R
+    conf, w = _synth(oc.Q4_K, oc.Q6_K)(dev)
+    for tid, key in enumerate(("wv", "ffn_down"), 100):
+        rows, cols = w[key][0].shape()
+        w[key][0] = CudaTensor.synth([rows, cols], oc.Q6_K, dev, 0xF5, tid, R.synth_scale(oc.Q6_K, cols))
+    return conf, w
+
+
 def _fixture(path):
     def weights(dev):
         from crabml_b200 import runner as R
@@ -146,6 +157,9 @@ CASES = {
     "7b-q8_0": (lambda fp: _decode(_synth(oc.Q8_0, oc.Q8_0)), 14, 0, 2, DECODE_7B),          # ring kernel
     "7b-q4_0-q6k": (lambda fp: _decode(_synth(oc.Q4_0, oc.Q6_K)), 14, 0, 2, DECODE_7B),      # Q6_K classifier: a generic phase in the ring table
     "7b-q4_k": (lambda fp: _decode(_synth(oc.Q4_K, oc.Q6_K)), 29, 0, 1, DECODE_7B),          # mega_kernel; mode 1 runs K-quant ops eagerly
+    # mixed q/k/v (wv Q6_K): the norm cannot fold into the wq/wk phase while wv still reads its row, so it is written back by a NORMQ
+    # phase, then wq + wk (2 matrices) and wv (1) run as separate generic phases
+    "7b-q4_k_m": (lambda fp: _decode(_synth_q4_k_m), 28, 0, 1, (48, 0, 4114, 4113) + DECODE_7B[2:]),
     "tinyllamas-q8_0": (_tinyllamas, 60, 0, 2, (48,) + TINY_LAYER * 6 + (0, 48, 17, 96)),
     "7b-q8_0-sampled": (lambda fp: _decode(_synth(oc.Q8_0, oc.Q8_0), sample=True), 14, 0, 2, DECODE_7B[:-1] + (112,)),
     "two-samplers": (lambda fp: _ops(_samplers(2)), 3, 0, 0, ()),                             # upload + 2 samplers, in the graph

@@ -16,6 +16,23 @@ def gdev():
     d.close()
 
 
+def gemv_budget(t, raw, m, k, x):
+    """Error budget of a matvec against oc.gemv: f32 summation-order noise, 1e-6 * sum_i |w_i a_i| per output (the integer block dots
+    are exact), with a the quantised activation the kernel multiplies.  x: [k] or [b, k] -> [b * m] (row-major like the output).
+    The weights are dequantised a slab of rows at a time, so that large matrices stay cheap in host memory."""
+    at = oc.rhs_type(t)
+    xb = np.asarray(x, np.float32).reshape(-1, k)
+    ad = np.stack([np.abs(oc.dequantize(at, oc.quantize(at, r), k)) for r in xb]).astype(np.float64)
+    rows_per = max(1, (1 << 22) // k)
+    row_bytes = raw.size // m
+    sums = np.empty((xb.shape[0], m), np.float64)
+    for r0 in range(0, m, rows_per):
+        r1 = min(m, r0 + rows_per)
+        wd = np.abs(oc.dequantize(t, raw[r0 * row_bytes:r1 * row_bytes], (r1 - r0) * k).reshape(r1 - r0, k)).astype(np.float64)
+        sums[:, r0:r1] = ad @ wd.T
+    return sums.reshape(-1) * 1e-6 + 1e-30
+
+
 def run_case(gdev, t, m, k, b=None, seed=0, scale=0.02):
     from crabml_b200 import CudaTensor
     rng = np.random.default_rng(seed)
@@ -26,12 +43,7 @@ def run_case(gdev, t, m, k, b=None, seed=0, scale=0.02):
     got = gw.matmul_vec(CudaTensor.new(x, xs, gdev))
     assert got.shape() == ([m] if b is None else [b, m])
     want = oc.gemv(t, raw, m, k, x.reshape(xs))
-    # error budget: f32 summation-order noise relative to sum |w_i a_i| (the integer block dots are exact)
-    at = oc.rhs_type(t)
-    wd = np.abs(oc.dequantize(t, raw, m * k).reshape(m, k)).astype(np.float64)
-    xb = x.reshape(-1, k)
-    ad = np.stack([np.abs(oc.dequantize(at, oc.quantize(at, r), k)) for r in xb]).astype(np.float64)
-    budget = (ad @ wd.T).reshape(got.export().shape) * 1e-6 + 1e-30
+    budget = gemv_budget(t, raw, m, k, x)
     if t in (oc.Q4_1, oc.Q5_1):
         budget = budget * 1.0          # same f16-rounded products as the reference; no extra slack
     diff = np.abs(got.export().astype(np.float64) - want.reshape(-1).astype(np.float64))

@@ -92,7 +92,7 @@ FINE = ["x0", "xn", "q", "k", "v", "att", "o", "x1", "hn", "g", "u", "h", "y", "
 COARSE = ["x0", "q", "k", "v", "x1", "h", "x2"]
 
 
-@pytest.mark.parametrize("wt", [oc.Q8_0, oc.Q4_0, oc.Q4_K])
+@pytest.mark.parametrize("wt", [oc.Q8_0, oc.Q4_0, oc.Q2_K, oc.Q3_K, oc.Q4_K, oc.Q5_K, oc.Q6_K, oc.Q8_K])
 def test_megakernel_phase_taps_vs_oracle_on_the_same_inputs(wt):
     from crabml_b200 import runner as R
     tokens = [1, 31999, 777]

@@ -152,12 +152,12 @@ def test_lazy_mode_matches_eager_ops_through_python_mirror(fixture_path):
         dev.close()
 
 
-@pytest.mark.parametrize("wt,ct", [(oc.Q8_0, oc.Q8_0), (oc.Q4_0, oc.Q6_K), (oc.Q4_K, oc.Q6_K)])
+@pytest.mark.parametrize("wt,ct", [(oc.Q8_0, oc.Q8_0), (oc.Q4_0, oc.Q6_K), (oc.Q4_K, oc.Q6_K), (oc.Q5_K, oc.Q6_K), (oc.Q2_K, oc.Q6_K)])
 def test_lazy_7b_shaped_layer(wt, ct):
     """Every execution mode on the same model.  The K-quant rows do not take the streaming kernel: they check that the fuser
     hands the f32 normalised row (not only the Q8_0 scratch) to matvecs that fall back to their eager kernels.  Lazy mode 2 runs
     both persistent kernels here: the ring kernel (mega_ring.cu) for the tables with Q8_0 / Q4_0 phases, mega_kernel (mega.cu)
-    for the all-K-quant one."""
+    for the all-K-quant ones (Q4_K and Q6_K segmented, Q5_K and Q2_K row by row)."""
     from crabml_b200 import runner as R
     conf = R.LlamaConfig(32, 32, 2, 4096, 11008, 4096, 32000, 1e-5, 128)
     res = {}
@@ -171,7 +171,8 @@ def test_lazy_7b_shaped_layer(wt, ct):
                 st = dev.lazy_stats()
                 assert st["uncached"] == 0 and st["graph_replays"] >= 2, st
             if lazy == 2:
-                assert dev.mega_variant() == (1 if wt == oc.Q4_K else 2), dev.mega_variant()
+                streaming = wt in (oc.Q8_0, oc.Q4_0) or ct in (oc.Q8_0, oc.Q4_0)      # a table with no Q8_0 / Q4_0 matvec runs mega_kernel
+                assert dev.mega_variant() == (2 if streaming else 1), dev.mega_variant()
             r.close()
         finally:
             dev.close()
