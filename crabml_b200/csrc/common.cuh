@@ -297,6 +297,8 @@ struct MkPhase {
                                         // SAMPLE: as ARGMAX, with a SampleDyn at dyn_off and the sampler scratch at dst
     int norm_ahead, pad2;               // fused norm: no op of the table writes norm_w (model weights), so it may be staged before earlier phases end
 };
+#define MK_PROF_SLOTS 9      // developer profiling: u64 stamps per phase (CTA 0 / thread 0): 0 start, 1 activation ready, 2 rows done, 3 arrived, 4 x staged, 5 rms known,
+                             // 6-7 ring consumer counters, 8 norm weights available (mega_ring.cu); read by tools/mega_profile*.py
 size_t cc_mega_smem_for_phase(const MkPhase& ph);      // working area, without the norm-weight staging area on top of it
 const CommDev* cc_comm_dev(cc_device* dev);
 bool cc_comm_is_nccl(cc_device* dev);
@@ -347,8 +349,9 @@ int cc_launch_rope_exact(cc_device* dev, float* x, int64_t n_batch, int64_t batc
 int cc_launch_bmm_kcontig_exact(cc_device* dev, const float* a, const void* b, int b_dtype, float* c, int64_t ab, int64_t bb,
                                 int64_t m, int64_t k, int64_t n, int64_t sb0, int64_t sb2);
 
-// one segment of a weight row in registers: 8 x 16-byte loads + 4 f16 scales per lane (the megakernel's weight pipe; Q8_0 / Q4_0:
-// two half-group runs a, b of 4 groups; Q4_K: a = block headers, b = quants; Q6_K: a = ql, b = qh, s = d)
+// one segment (16 super-blocks) of a K-quant weight row in registers, loaded as one batch by T::seg_load (vecdot.cuh) so that the
+// generic MATVEC phase keeps the next segment in flight: 8 x 16-byte loads + 4 f16 scales per lane (Q4_K: a = block headers,
+// b = quants; Q6_K: a = ql, b = qh, s = d)
 struct KSeg { int4 a[4], b[4]; uint16_t s[4]; };
 
 // ---- small device helpers -------------------------------------------------------------------------

@@ -93,7 +93,7 @@ LazyState* cc_lazy_create(cc_device* dev) {
     for (int i = 0; i < LZ_DYN_SLOTS; i++)
         if (cudaMallocHost(&lz->dyn_host[i], lz->dyn_cap) != cudaSuccess || cudaEventCreateWithFlags(&lz->dyn_ev[i], cudaEventDisableTiming) != cudaSuccess) { delete lz; return nullptr; }
     if (cudaMalloc(&lz->dyn_dev, lz->dyn_cap) != cudaSuccess) { delete lz; return nullptr; }
-    if (getenv("CRABML_MEGA_PROF") && cudaMalloc(&lz->prof_dev, 9 * 8 * 4097) == cudaSuccess) cudaMemset(lz->prof_dev, 0, 9 * 8 * 4097);    // stamps a kernel never takes read 0
+    if (getenv("CRABML_MEGA_PROF") && cudaMalloc(&lz->prof_dev, MK_PROF_SLOTS * 8 * 4097) == cudaSuccess) cudaMemset(lz->prof_dev, 0, MK_PROF_SLOTS * 8 * 4097);    // stamps a kernel never takes read 0
     if (cudaMalloc(&lz->bar_dev, 4096) != cudaSuccess || cudaMemset(lz->bar_dev, 0, 4096) != cudaSuccess) { delete lz; return nullptr; }
     return lz;
 }
@@ -813,8 +813,8 @@ extern "C" CC_API int cc_lazy_mega_profile(cc_device* dev, unsigned long long* t
     if (!dev || !dev->lz || !dev->lz->prof_dev || !ts || !types || !n_out) return CC_ERR_ARG;
     cudaStreamSynchronize(dev->stream);
     int n = (int)dev->lz->prof_types.size();
-    if ((n + 1) * 9 > cap) return CC_ERR_ARG;          // 9 stamps per phase (mega_phases.cuh MK_PROF_SLOTS)
-    if (cudaMemcpy(ts, dev->lz->prof_dev, (size_t)(n + 1) * 9 * 8, cudaMemcpyDeviceToHost) != cudaSuccess) return CC_ERR_CUDA;
+    if ((n + 1) * MK_PROF_SLOTS > cap) return CC_ERR_ARG;
+    if (cudaMemcpy(ts, dev->lz->prof_dev, (size_t)(n + 1) * MK_PROF_SLOTS * 8, cudaMemcpyDeviceToHost) != cudaSuccess) return CC_ERR_CUDA;
     for (int i = 0; i < n; i++) types[i] = dev->lz->prof_types[i];
     *n_out = n;
     return CC_OK;

@@ -98,7 +98,7 @@ __global__ void __launch_bounds__(MK_THREADS, MK_CTAS_PER_SM) mega_kernel(const 
         if (look && threadIdx.x < 3) ((int*)&s_next)[threadIdx.x] = next_w;
         const bool more = p + 1 < n_phases;
         // test hook (tests/test_gpu_robustness.py): one CTA deserts before the third barrier, as if it had never become resident
-        if (test_stall && p == 2 && blockIdx.x == gridDim.x - 1) return;
+        if (test_stall && p == 2 && blockIdx.x == gridDim.x - 1) { if (threadIdx.x == 0) s_abort = 1; break; }
         if (more) grid_barrier_arrive(bar, gridDim.x, gen);       // its bar.sync also publishes s_next (written just above)
         // immutable norm weights of the next fused prologue, requested before waiting at the barrier: one L2 trip less after it
         if (look && s_next.norm_n > 0) {
@@ -127,6 +127,7 @@ __global__ void __launch_bounds__(MK_THREADS, MK_CTAS_PER_SM) mega_kernel(const 
             }
         }
     }
+    asm volatile("cp.async.wait_all;" ::: "memory");      // a launch that gave up may still have norm-weight or x-row copies in flight
     // the SAMPLE phase (lazy.cu: the only one, and the last): called after the loop, so the call saves nothing around itself (the
     // barrier before it was the last iteration's)
     if constexpr (SMP) {

@@ -561,9 +561,6 @@ static __device__ void phase_reduce(const MkPhase& ph, const CommDev& comm, unsi
 }
 
 
-#define MK_PROF_SLOTS 9      // developer profiling: u64 stamps per phase (CTA 0 / thread 0): 0 start, 1 activation ready, 2 rows done, 3 arrived, 4 x staged, 5 rms known,
-                             // 6-7 ring consumer counters, 8 norm weights available (mega_ring.cu)
-
 #define MK_F_TESTSTALL 128     // test hook: the last CTA leaves before barrier 2 -> every other CTA must time out, not hang (cc_mega_test_stall)
 
 // Launch of a persistent kernel (mega.cu, mega_ring.cu).  The grid barrier needs every CTA resident at once.  On a GPU this process

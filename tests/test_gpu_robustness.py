@@ -39,7 +39,7 @@ def test_deserting_cta_is_a_timeout_error_not_a_hang(wt):
     never become resident (another tenant on the GPU).  Every other CTA must give up after the spin bound, the kernel must drain
     (ring kernel: the producer warps stop, bulk copies in flight land before the CTA's shared memory goes away), and the host must
     see CC_ERR_CUDA 'megakernel barrier timeout' -- within seconds."""
-    env = dict(os.environ, CRABML_MEGA_FLAGS=str(0x44C | 0x80))          # the default flag word + the hook
+    env = dict(os.environ, CRABML_MEGA_FLAGS=str(0x80))          # the only bit of the word that has an effect
     t0 = time.time()
     p = subprocess.run([sys.executable, "-c", CHILD, wt], env=env, capture_output=True, text=True, timeout=120)
     out = p.stdout + p.stderr

@@ -27,7 +27,7 @@ for i in range(40):
     r.forward([100 + i], pos, export=False); pos += 1
 ms = dev.timer_end()
 print(f"40 tokens back to back: {ms / 40 * 1e3:.1f} us per token by CUDA events (kernel time below + inter-launch gap)")
-SL = 9                                      # stamps per phase (mega_phases.cuh MK_PROF_SLOTS)
+SL = 9                                      # stamps per phase (common.cuh MK_PROF_SLOTS)
 CAP = SL * 4097
 ts = (C.c_uint64 * CAP)(); ty = (C.c_int32 * CAP)(); n = C.c_int32(0)
 dev.check(dev.lib.cc_lazy_mega_profile(dev.handle, ts, ty, CAP, C.byref(n)))
