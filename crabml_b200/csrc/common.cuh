@@ -333,6 +333,7 @@ struct LazyState;
 LazyState* cc_lazy_create(cc_device* dev);
 void cc_lazy_destroy(cc_device* dev);
 int cc_lazy_flush(cc_device* dev);
+int cc_lazy_invalidate(cc_device* dev);        // drop the cached graphs, reset the grid barrier (no-op without lazy state); stream idle
 bool cc_stream_supported(int type, int64_t k);
 bool cc_mega_generic_supported(int type, int64_t k);      // K-quant weights: generic MATVEC phase of the megakernel (mega.cu)
 int cc_launch_matvec_stream(cc_device* dev, int type, const StreamArgs& A);

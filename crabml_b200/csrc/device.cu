@@ -151,6 +151,10 @@ extern "C" CC_API int cc_device_set_sm_limit(cc_device* dev, int32_t n) {
     CC_CUDA(dev, cudaGetDeviceProperties(&prop, dev->ordinal));
     CC_REQUIRE(dev, n >= 1 && n <= prop.multiProcessorCount, "sm_limit %d out of range (1..%d)", n, prop.multiProcessorCount);
     if (dev->lz) { int rc = cc_lazy_flush(dev); if (rc) return rc; }
+    if (dev->lz && n != dev->sm_count) {         // cached graphs keep the grid they were captured with
+        CC_CUDA(dev, cudaStreamSynchronize(dev->stream));
+        if (int rc = cc_lazy_invalidate(dev)) return rc;
+    }
     dev->sm_count = n;
     return CC_OK;
 }
@@ -233,6 +237,7 @@ int cc_ensure_act_scratch(cc_device* dev, size_t bytes) {
     if (bytes <= dev->act_scratch_bytes) return CC_OK;
     if (dev->act_scratch) {
         CC_CUDA(dev, cudaStreamSynchronize(dev->stream));
+        if (int rc = cc_lazy_invalidate(dev)) return rc;      // the lazy modes' cached graphs of eager matvec steps hold the old pointer
         CC_CUDA(dev, cudaFree(dev->act_scratch));
     }
     size_t nb = size_class(bytes);

@@ -87,6 +87,18 @@ static void graph_cache_clear(LazyState* lz) {
     for (auto& kv : lz->cache) graph_entry_free(kv.second);
     lz->cache.clear();
 }
+// the same, for what a graph bakes in outside the lazy state: the eager matvec steps' dev->act_scratch (cc_ensure_act_scratch) and the
+// grid of every persistent or streaming kernel (cc_device_set_sm_limit).  Both change rarely, so the next flush of every plan
+// re-captures rather than each signature carrying a scratch generation and the SM count.  The grid barrier restarts from zero too, as
+// on a new device: its arrival counter holds (barriers so far) x (grid size), which a launch with another grid cannot continue
+// (mega_phases.cuh grid_barrier_wait).  The stream must be idle.
+int cc_lazy_invalidate(cc_device* dev) {
+    LazyState* lz = dev->lz;
+    if (!lz) return CC_OK;
+    graph_cache_clear(lz);
+    if (cudaMemsetAsync(lz->bar_dev, 0, 4096, dev->stream) != cudaSuccess) return cc_fail(dev, CC_ERR_CUDA, "lazy: barrier reset failed");
+    return CC_OK;
+}
 
 LazyState* cc_lazy_create(cc_device* dev) {
     LazyState* lz = new LazyState();
@@ -195,6 +207,9 @@ struct Fuser {
         cc_device* d = dev;
         P.S(0x1000 + op.kind); P.SP(op.a.buf ? op.a.buf->plane[0] : nullptr); P.SP(op.b.buf ? op.b.buf->plane[0] : nullptr);
         P.SP(op.out ? op.out->plane[0] : nullptr);
+        // the pool hands an f32 and an f16 buffer of one size class the same address, and a weight re-created at a freed address may
+        // have another type: the kernels a step launches depend on the types
+        P.S(op.a.buf ? op.a.buf->dtype : -1); P.S(op.b.buf ? op.b.buf->dtype : -1); P.S(op.out ? op.out->dtype : -1);
         for (int k = 0; k < CC_MAX_DIMS; k++) { P.S(op.a.shape[k]); P.S(op.a.strides[k]); P.S(op.b.shape[k]); P.S(op.b.strides[k]); }
         P.S(op.i0); P.S(op.i1); P.S(op.i2); uint32_t fb; memcpy(&fb, &op.f, 4); P.S(fb);
         switch (op.kind) {
@@ -455,7 +470,7 @@ struct Fuser {
         int n = slot >= 0 ? 1 : (int)op.rows.size();
         size_t off = slot >= 0 ? 0 : P.dyn_put(op.rows.data(), op.rows.size() * 8);
         const int64_t* rows_dev = slot >= 0 ? dev->slots + slot : nullptr;
-        P.S(0x2005); P.SP(src->plane[0]); P.SP(dst); P.S(dt); P.S(n); P.S(cols); P.S(off); P.SP(rows_dev);
+        P.S(0x2005); P.SP(src->plane[0]); P.SP(dst); P.S(dt); P.S(n); P.S(cols); P.S(off); P.SP(rows_dev); P.S(src->dtype); P.S(src->cols);   // (types: fallback())
         P.steps.push_back([=](uint8_t* dyn_dev) { return cc_launch_dequant_rows(d, src, rows_dev ? rows_dev : (const int64_t*)(dyn_dev + off), n, cols, dst, dt); });
         { MkPhase ph = {}; ph.type = MK_ROWS; ph.dyn_off = off; for (int t = 0; t < CC_MAX_PLANES; t++) ph.planes.p[t] = src->plane[t];
           ph.planes.cols = src->cols > 0 ? src->cols : cols; ph.src_dtype = src->dtype; ph.dst_dtype = dt; ph.n_rows = n; ph.cols = cols; ph.dst = dst;
@@ -663,7 +678,7 @@ static int size_scratch(cc_device* dev, LazyState* lz) {
         for (int i = 0; i < 2; i++) if (cudaMalloc(&lz->act[i], cap) != cudaSuccess) return cc_fail(dev, CC_ERR_CUDA, "lazy: scratch alloc failed");
         lz->act_cap = cap;
     }
-    // eager matvec fallbacks (cc_launch_matmul_vec) use dev->act_scratch
+    // eager matvec fallbacks (cc_launch_matmul_vec) use dev->act_scratch; growing it drops the cached graphs (cc_ensure_act_scratch)
     for (auto& op : lz->q) if (op.kind == L_MATVEC) {
         int at = cc_partner_type(op.a.buf->dtype);
         int64_t bb = op.b.ndim == 1 ? 1 : op.b.shape[0];

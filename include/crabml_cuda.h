@@ -97,7 +97,8 @@ CC_API int cc_lazy_mega_profile(cc_device* dev, unsigned long long* ts, int* typ
 CC_API int cc_lazy_mega_variant(cc_device* dev);
 /* counters: kernels launched by this library since creation (bench.py "gpu_launches") */
 CC_API uint64_t cc_device_launch_count(cc_device* dev);
-/* persistent kernels of this device use at most n SMs (test / co-tenancy hook: two devices of one process side by side on one GPU) */
+/* persistent kernels of this device use at most n SMs (test / co-tenancy hook: two devices of one process side by side on one GPU).
+ * In lazy mode a change waits for the queued work and drops the graphs captured at the old grid. */
 CC_API int cc_device_set_sm_limit(cc_device* dev, int32_t n);
 /* raw cudaStream_t of the device, for event timing by the caller */
 CC_API void* cc_device_stream(cc_device* dev);
