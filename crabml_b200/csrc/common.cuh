@@ -277,7 +277,16 @@ struct AttnArgs {            // fused decode attention (fused.cu)
     int n_heads, n_kv, hd, rope_dim, max_len, kv_f16;
     int64_t seq_stride;
     float scale;
+    int split;               // megakernels: CTAs per head (lazy.cu: the most the score scratch allows, then cc_attn_split); the fused kernel ignores it
 };
+// Attention phase of the megakernels split over `split` CTAs per head: CTA c scores its own range of the head's positions and
+// accumulates PV for its hd / split output dimensions; the score rows meet in MegaLaunch::scores ([n_heads][max_len + 1] f32).  Head h's CTAs count their arrivals in
+// word AT_ARRIVE_WORD + 8 h of the grid-barrier block (4096 bytes), AT_SPLIT_MAX per phase whatever the split.
+#define AT_SPLIT_MAX 4
+#define AT_SPLIT_MIN_KV 320       // below this many cached positions the exchange costs more than the split saves: one CTA per head
+#define AT_ARRIVE_WORD 128
+#define AT_SPLIT_MAX_HEADS ((1024 - AT_ARRIVE_WORD) / 8)
+int cc_attn_split(const AttnArgs& a, int grid);
 struct DeqPlanes { const uint8_t* p[CC_MAX_PLANES]; int64_t cols; };
 // megakernel phase descriptor (mega.cu); built by lazy.cu
 enum { MK_NORMQ = 0, MK_MATVEC = 1, MK_ATTN = 2, MK_ROWS = 3, MK_REDUCE = 4, MK_GATHER = 5, MK_ARGMAX = 6, MK_SAMPLE = 7 };
@@ -314,6 +323,7 @@ struct MegaLaunch {                 // launch description of one phase table (la
     size_t smem = 1024, wstage = 0;  // working area (largest phase) ; norm-weight stage on top of it (largest n * 4 of a fused-norm phase)
     int slot_bytes = 0, nslots = 0, at_ch = 64;  // MEGA_RING: weight-ring slot size and count (cc_mega_ring_slots), attention chunk
     bool generic = false, sample = false;        // the instantiation that carries the generic (K-quant) MATVEC phase / the sampler's call
+    float* scores = nullptr;                     // the attention phase's score rows (AttnArgs::split > 1)
 };
 int cc_launch_mega(cc_device* dev, const MkPhase* phases_dev, int n_phases, const uint8_t* dyn_dev, unsigned* bar_dev, const MegaLaunch& L,
                    unsigned long long* prof);

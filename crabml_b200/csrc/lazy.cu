@@ -51,7 +51,9 @@ struct LazyState {
     uint8_t* dyn_dev = nullptr;
     size_t dyn_cap = 1 << 16;
     void* act[2] = {nullptr, nullptr};
-    unsigned* bar_dev = nullptr;     // megakernel grid barrier {count, generation}
+    float* scores = nullptr;         // megakernels' attention phase: the score rows the CTAs of a head exchange (cc_attn_split)
+    size_t scores_cap = 0;
+    unsigned* bar_dev = nullptr;     // megakernel grid barrier {count, generation}, attention arrival words (AT_ARRIVE_WORD)
     unsigned long long* prof_dev = nullptr;   // CRABML_MEGA_PROF=1: per-phase start timestamps of the last megakernel run
     std::vector<int> prof_types;
     size_t act_cap = 0;
@@ -107,6 +109,8 @@ LazyState* cc_lazy_create(cc_device* dev) {
     if (cudaMalloc(&lz->dyn_dev, lz->dyn_cap) != cudaSuccess) { delete lz; return nullptr; }
     if (getenv("CRABML_MEGA_PROF") && cudaMalloc(&lz->prof_dev, MK_PROF_SLOTS * 8 * 4097) == cudaSuccess) cudaMemset(lz->prof_dev, 0, MK_PROF_SLOTS * 8 * 4097);    // stamps a kernel never takes read 0
     if (cudaMalloc(&lz->bar_dev, 4096) != cudaSuccess || cudaMemset(lz->bar_dev, 0, 4096) != cudaSuccess) { delete lz; return nullptr; }
+    lz->scores_cap = (size_t)1 << 20;                // 32 heads x 8K positions before the first regrowth (size_scratch)
+    if (cudaMalloc(&lz->scores, lz->scores_cap) != cudaSuccess) { delete lz; return nullptr; }
     return lz;
 }
 void cc_lazy_destroy(cc_device* dev) {
@@ -119,6 +123,7 @@ void cc_lazy_destroy(cc_device* dev) {
     for (int i = 0; i < LZ_DYN_SLOTS; i++) { if (lz->dyn_host[i]) cudaFreeHost(lz->dyn_host[i]); if (lz->dyn_ev[i]) cudaEventDestroy(lz->dyn_ev[i]); }
     if (lz->dyn_dev) cudaFree(lz->dyn_dev);
     for (int i = 0; i < 2; i++) if (lz->act[i]) cudaFree(lz->act[i]);
+    if (lz->scores) cudaFree(lz->scores);
     delete lz;
     dev->lz = nullptr;
 }
@@ -440,9 +445,11 @@ struct Fuser {
         A.n_heads = (int)n_heads; A.n_kv = (int)n_kv; A.hd = (int)hd; A.rope_dim = (int)rope_dim;
         A.max_len = (int)(seq_stride / hd); A.kv_f16 = kc->dtype == CC_F16;
         A.seq_stride = seq_stride; A.scale = sc.f;
+        // the most CTAs per head the score scratch allows; the persistent kernel's split is chosen with its grid (choose_mega)
+        A.split = (size_t)n_heads * (size_t)(A.max_len + 1) * 4 <= lz->scores_cap ? AT_SPLIT_MAX : 1;
         cc_device* d = dev;
         size_t roff = rope_off;
-        P.S(0x2004); P.SP(A.q); P.SP(A.k); P.SP(A.v); P.SP(A.kcache); P.SP(A.vcache); P.SP(A.out); P.SP(A.act_scratch);
+        P.S(0x2004); P.SP(A.q); P.SP(A.k); P.SP(A.v); P.SP(A.kcache); P.SP(A.vcache); P.SP(A.out); P.SP(A.act_scratch); P.S(A.split); P.SP(lz->scores);
         P.S(n_heads); P.S(n_kv); P.S(hd); P.S(rope_dim); P.S(seq_stride); P.S(A.kv_f16); uint32_t sb; memcpy(&sb, &A.scale, 4); P.S(sb); P.S(dyn_off); P.S(roff);
         P.steps.push_back([=](uint8_t* dyn_dev) {
             AttnArgs B = A;
@@ -648,6 +655,8 @@ static MegaLaunch choose_mega(const cc_device* dev, bool mega_ok, std::vector<Mk
     }
     if (stream ? !ring_ok || !(L.nslots = cc_mega_ring_slots(L)) : L.smem + L.wstage + 4096 > 227 * 1024) return L;
     L.variant = stream ? MEGA_RING : MEGA_REGISTER;
+    for (auto& ph : phs) if (ph.type == MK_ATTN) ph.at.split = cc_attn_split(ph.at, dev->sm_count);      // both kernels: one CTA per SM
+    L.scores = dev->lz->scores;
     int nxt = -1, nxn = -1;
     for (int t = (int)phs.size() - 1; t >= 0; t--) {
         MkPhase& ph = phs[t];
@@ -677,6 +686,20 @@ static int size_scratch(cc_device* dev, LazyState* lz) {
         size_t cap = (size_t)1 << 20; while (cap < need) cap <<= 1;      // generous from the start: growing means cudaFree (context-wide wait)
         for (int i = 0; i < 2; i++) if (cudaMalloc(&lz->act[i], cap) != cudaSuccess) return cc_fail(dev, CC_ERR_CUDA, "lazy: scratch alloc failed");
         lz->act_cap = cap;
+    }
+    // the megakernels' attention score rows [heads][max_len + 1] (MegaLaunch::scores), from the QK^T products: the K^T view of the cache
+    // has row stride hd and batch stride max_len * hd
+    size_t score_need = 0;
+    for (auto& op : lz->q)
+        if (op.kind == L_BMM && op.b.ndim == 3 && op.b.strides[1] == 1 && op.b.strides[2] > 0 && op.b.strides[0] > 0)
+            score_need = std::max(score_need, (size_t)op.a.shape[0] * (size_t)(op.b.strides[0] / op.b.strides[2] + 1) * 4);
+    if (score_need > lz->scores_cap) {
+        cudaStreamSynchronize(dev->stream);
+        graph_cache_clear(lz);
+        cudaFree(lz->scores); lz->scores = nullptr; lz->scores_cap = 0;
+        size_t cap = (size_t)1 << 20; while (cap < score_need) cap <<= 1;
+        if (cudaMalloc(&lz->scores, cap) != cudaSuccess) return cc_fail(dev, CC_ERR_CUDA, "lazy: score scratch alloc failed");
+        lz->scores_cap = cap;
     }
     // eager matvec fallbacks (cc_launch_matmul_vec) use dev->act_scratch; growing it drops the cached graphs (cc_ensure_act_scratch)
     for (auto& op : lz->q) if (op.kind == L_MATVEC) {

@@ -9,7 +9,7 @@
 //     MATVEC  K-quant matvec over 1-3 matrices + epilogue, with a fused prologue ([dup] + rms_norm * w + Q8_K quantisation of the
 //             input row, recomputed by every CTA)
 //     NORMQ   normalise + Q8_0 quantise as a phase of its own
-//     ATTN    rope + KV append + attention + output quantise    (one CTA per head, K/V chunks through a TMA pipeline)
+//     ATTN    rope + KV append + attention + output quantise    (up to 4 CTAs per head, K/V chunks through a TMA pipeline)
 //     ROWS    copy_rows_from (embedding row dequantisation)
 //     ARGMAX / SAMPLE   the next token on the device
 // The per-phase time breakdown: tools/mega_profile.py.
@@ -26,7 +26,7 @@ struct MkNextNorm { const float* norm_w; int norm_n; };
 template <bool SMP>
 __global__ void __launch_bounds__(MK_THREADS, MK_CTAS_PER_SM) mega_kernel(const MkPhase* __restrict__ phases, int n_phases, const uint8_t* dyn,
                                                                          unsigned* bar, const uint16_t* exp_lut, unsigned long long* prof, bool test_stall, int wtop_off,
-                                                                         unsigned* err_host) {
+                                                                         unsigned* err_host, float* scores) {
     extern __shared__ __align__(16) uint8_t smem[];
     __shared__ float s_red[MK_WARPS];
     __shared__ MkPhase s_phs[2];             // phase descriptors, double-buffered: p+1 is fetched while p runs
@@ -88,7 +88,8 @@ __global__ void __launch_bounds__(MK_THREADS, MK_CTAS_PER_SM) mega_kernel(const 
             break;
         }
         case MK_ATTN:
-            if (s_ph.at.kv_f16) phase_attn<true>(s_ph, (float*)work, s_red, dyn, exp_lut, abar0, apar, AT_CH); else phase_attn<false>(s_ph, (float*)work, s_red, dyn, exp_lut, abar0, apar, AT_CH);
+            if (s_ph.at.kv_f16) phase_attn<true>(s_ph, (float*)work, s_red, dyn, exp_lut, abar0, apar, AT_CH, bar, err_host, &s_abort, scores);
+            else phase_attn<false>(s_ph, (float*)work, s_red, dyn, exp_lut, abar0, apar, AT_CH, bar, err_host, &s_abort, scores);
             break;
         case MK_ROWS: phase_rows(s_ph, dyn); break;
         case MK_ARGMAX: phase_argmax(s_ph, dyn, s_red); break;
@@ -175,6 +176,17 @@ extern "C" CC_API int cc_test_mega_barrier_floor(cc_device* dev, int n, float* u
     return CC_OK;
 }
 
+// CTAs per head of the attention phase (mega_phases.cuh phase_attn) in a grid of `grid` CTAs: the largest of 4, 2, 1 for which every
+// CTA owns whole Q8_0 blocks of the head's output (hd % (32 S) == 0) and every CTA serves one head at most (n_heads S <= grid), so no CTA
+// waits for a peer that is still busy with another head.  a.split is the most the score scratch allows (1: none); with more heads than
+// arrival words, one CTA per head.
+int cc_attn_split(const AttnArgs& a, int grid) {
+    if (a.split <= 1 || a.n_heads > AT_SPLIT_MAX_HEADS) return 1;
+    for (int S = AT_SPLIT_MAX; S > 1; S >>= 1)
+        if (a.hd % (32 * S) == 0 && a.n_heads * S <= grid) return S;
+    return 1;
+}
+
 bool cc_mega_generic_supported(int type, int64_t k) {
     return (type == CC_Q2_K || type == CC_Q3_K || type == CC_Q4_K || type == CC_Q5_K || type == CC_Q6_K || type == CC_Q8_K) && k % 256 == 0 && k <= 32768;
 }
@@ -198,5 +210,5 @@ int cc_launch_mega(cc_device* dev, const MkPhase* phases_dev, int n_phases, cons
     int per_sm = max_ctas_per_sm < MK_CTAS_PER_SM ? max_ctas_per_sm : MK_CTAS_PER_SM;
     const uint16_t* lut = dev->exp_lut;
     return mk_launch(dev, kern, dev->sm_count * per_sm, MK_THREADS, smem, phases_dev, n_phases, dyn_dev, bar_dev, lut, prof, cc_mega_test_stall(),
-                     (int)wtop, dev->err_host);
+                     (int)wtop, dev->err_host, L.scores);
 }

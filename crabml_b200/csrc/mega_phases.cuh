@@ -326,13 +326,15 @@ static __device__ MK_GENERIC_ATTR void phase_matvec_generic(const MkPhase& ph, u
     flush_pending();
 }
 
-// ---- ATTN phase: arithmetic of fused.cu attn_decode_kernel, heads dealt to CTAs.  The K (then V) rows of the head are
-// staged in shared memory in chunks of AT_CH positions with ALL loads of a chunk in flight at once: at decode the cost of
-// this phase is HBM/L2 latency, not bandwidth, so round trips are what matters.
+// ---- ATTN phase: arithmetic of fused.cu attn_decode_kernel, heads dealt to CTAs (phase_attn_one) or each head to a.split = S CTAs
+// (phase_attn_split, cc_attn_split).  The K (then V) rows a CTA reads are staged in shared memory in chunks with ALL loads of a chunk in
+// flight at once: at decode the cost of this phase is HBM/L2 latency and the one SM a head's history streams through, not bandwidth, so
+// round trips and SMs per head are what matter.
 #define AT_CH 64
 #define AT_NBUF 3
+// one CTA per head: the K (then V) rows of the head are contiguous in the cache, one bulk copy per chunk of at_ch rows
 template <bool KV_F16>
-static __device__ void phase_attn(const MkPhase& ph, float* sm, float* s_red, const uint8_t* dyn, const uint16_t* exp_lut, unsigned abar0, unsigned& apar, const int at_ch) {
+static __device__ void phase_attn_one(const MkPhase& ph, float* sm, float* s_red, const uint8_t* dyn, const uint16_t* exp_lut, unsigned abar0, unsigned& apar, const int at_ch) {
     const AttnArgs& a = ph.at;
     const int n_heads = a.n_heads, n_kv = a.n_kv, hd = a.hd, rope_dim = a.rope_dim;
     const int64_t seq_stride = a.seq_stride;
@@ -483,6 +485,234 @@ static __device__ void phase_attn(const MkPhase& ph, float* sm, float* s_red, co
         }
         MK_SYNC();
     }
+}
+
+// a called function in the ring kernel (MK_GENERIC_NOINLINE), as the generic phase: inlined there, it cost the phases every token runs
+// (Llama-2-7B Q8_0 at ~32-104 positions decoded 268 instead of 271 tok/s; called, 280: the kernel spills less than before the split;
+// NVIDIA H100 80GB HBM3, 700 W).  Inlined in mega.cu, where a call spills more (nvcc 12.9 -Xptxas -v).
+#if MK_GENERIC_NOINLINE
+#define MK_ATTN_SPLIT_ATTR __noinline__
+#else
+#define MK_ATTN_SPLIT_ATTR
+#endif
+__device__ __forceinline__ unsigned atom_add_release(unsigned* p, unsigned v) {
+    unsigned old;
+    asm volatile("atom.release.gpu.global.add.u32 %0, [%1], %2;" : "=r"(old) : "l"(p), "r"(v) : "memory");
+    return old;
+}
+// CTA c of head h scores the positions [c L / S, (c + 1) L / S) (the last range holds this token's own position, scored from s_q . s_k)
+// and publishes them in the head's row of the score scratch; once all S CTAs have arrived every CTA reads the whole row and runs the softmax over
+// it in the canonical order, so all of them hold the same p; CTA c then accumulates PV for the dimensions [c hd / S, (c + 1) hd / S),
+// sequentially over s, and quantises those hd / (32 S) Q8_0 blocks of the output.  Each score is an independent dot product and each
+// output element's PV sum keeps its order: the bits are those of phase_attn_one.
+template <bool KV_F16>
+static __device__ MK_ATTN_SPLIT_ATTR void phase_attn_split(const MkPhase& ph, float* sm, float* s_red, const uint8_t* dyn, const uint16_t* exp_lut, unsigned abar0, unsigned& apar, const int at_ch,
+                                        unsigned* bar, unsigned* err_host, int* s_abort, float* scores) {
+    const AttnArgs& a = ph.at;
+    const int n_heads = a.n_heads, n_kv = a.n_kv, hd = a.hd, rope_dim = a.rope_dim, S = a.split;
+    const int64_t seq_stride = a.seq_stride;
+    const int64_t* dynv = (const int64_t*)(dyn + ph.dyn_off);
+    const float* rope_tab = (const float*)(dyn + ph.rope_off);
+    const int kv_len = (int)dynv[1], L = kv_len + 1;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    float* s_q = sm; float* s_k = sm + hd; float* s_v = sm + 2 * hd; float* s_p = sm + 3 * hd;
+    // AT_NBUF chunk buffers of at_ch cache rows each (raw bytes: f32 or f16), filled by TMA bulk copies in a K-chunks-then-V-chunks job
+    // sequence with AT_NBUF jobs in flight; one mbarrier per buffer.  A K chunk is at_ch contiguous rows of the CTA's range; a V chunk is
+    // vch = S at_ch rows of the CTA's dw = hd / S columns (the same bytes: the working area does not depend on S), one copy per row.
+    uint8_t* s_buf = (uint8_t*)(sm + 3 * hd + ((a.max_len + 8 + 3) & ~3));
+    const unsigned s_buf_smem = (unsigned)__cvta_generic_to_shared(s_buf);
+    constexpr int ELT = KV_F16 ? 2 : 4;
+    const unsigned buf_bytes = (unsigned)(at_ch * hd * ELT);
+    const int pairs = rope_dim >> 1;
+    const int dw = hd / S, vch = at_ch * S;
+    const int NCV = (kv_len + vch - 1) / vch;                     // V chunks: every CTA of the head reads all kv_len rows (its columns)
+    for (int u = blockIdx.x; u < n_heads * S; u += gridDim.x) {
+        const int h = u % n_heads, part = u / n_heads;           // part-major: part 0 of every head on the CTA that has it without the split
+        const int g = KV_F16 ? h / (n_heads / n_kv) : h % n_kv;
+        const int p_lo = (int)((int64_t)part * L / S), p_hi = (int)((int64_t)(part + 1) * L / S), k_hi = min(p_hi, kv_len);
+        const int NCK = k_hi > p_lo ? (k_hi - p_lo + at_ch - 1) / at_ch : 0;      // K chunks of the cached positions in [p_lo, p_hi)
+        const int NJ = NCK + NCV;
+        int v_issued = 0;                                            // V chunks requested so far (one cp.async group each)
+        auto issue_job = [&](int j) {                                // all threads
+            const unsigned mb = abar0 + 8u * (unsigned)(j % AT_NBUF), dst = s_buf_smem + (unsigned)(j % AT_NBUF) * buf_bytes;
+            if (j < NCK) {                                           // contiguous K rows: one bulk copy
+                const int p0 = p_lo + j * at_ch, cnt = min(at_ch, k_hi - p0);
+                if (threadIdx.x == 0) {
+                    const uint8_t* src = (const uint8_t*)a.kcache + ((int64_t)g * seq_stride + (int64_t)p0 * hd) * ELT;
+                    const unsigned bytes = (unsigned)(cnt * hd * ELT);
+                    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(mb), "r"(bytes) : "memory");
+                    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst), "l"(src), "r"(bytes), "r"(mb) : "memory");
+                }
+            } else {
+                // this CTA's dw columns of vch rows: 16-byte cp.async pieces spread over all threads (a bulk copy per 64-128-byte row
+                // slice is a TMA request each, and the requests of a long context queue up behind each other)
+                const int p0 = (j - NCK) * vch, cnt = min(vch, kv_len - p0), pr = dw * ELT / 16;
+                const uint8_t* src = (const uint8_t*)a.vcache + ((int64_t)g * seq_stride + (int64_t)p0 * hd + part * dw) * ELT;
+                for (int i = threadIdx.x; i < cnt * pr; i += MK_THREADS) {
+                    const int r = i / pr, q = i - r * pr;
+                    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst + (unsigned)(r * pr + q) * 16u), "l"(src + (int64_t)r * hd * ELT + q * 16) : "memory");
+                }
+                asm volatile("cp.async.commit_group;" ::: "memory");
+                v_issued++;
+            }
+        };
+        auto wait_job = [&](int j) {                                // all threads, in job order
+            if (j >= NCK) {                                          // this thread's pieces of chunk j have landed (later chunks may still be in flight), then everybody's
+                const int newer = v_issued - (j - NCK) - 1;
+                if (newer >= 2) asm volatile("cp.async.wait_group 2;" ::: "memory");
+                else if (newer == 1) asm volatile("cp.async.wait_group 1;" ::: "memory");
+                else asm volatile("cp.async.wait_group 0;" ::: "memory");
+                MK_SYNC();
+                return;
+            }
+            const int bsel = j % AT_NBUF;
+            mbar_wait(abar0 + 8u * (unsigned)bsel, (apar >> bsel) & 1u);
+            apar ^= 1u << bsel;
+        };
+        auto ld_kv = [&](const uint8_t* buf, int idx) -> float { return KV_F16 ? __half2float(((const __half*)buf)[idx]) : ((const float*)buf)[idx]; };
+        // the first AT_NBUF jobs are requested up front; every later job is issued as soon as its buffer has been consumed
+        for (int j = 0; j < min(AT_NBUF, NJ); j++) issue_job(j);
+        for (int i = threadIdx.x; i < hd; i += MK_THREADS) {
+            float qv, kvv;
+            if (i < rope_dim) {
+                const int j = i >> 1;
+                const float c = rope_tab[j], s = rope_tab[pairs + j];
+                const float q0 = ldcg_f(a.q + h * hd + 2 * j), q1 = ldcg_f(a.q + h * hd + 2 * j + 1);
+                const float k0 = ldcg_f(a.k + g * hd + 2 * j), k1 = ldcg_f(a.k + g * hd + 2 * j + 1);
+                qv = (i & 1) ? q0 * s + q1 * c : q0 * c - q1 * s;
+                kvv = (i & 1) ? k0 * s + k1 * c : k0 * c - k1 * s;
+            } else {
+                qv = ldcg_f(a.q + h * hd + i);
+                kvv = ldcg_f(a.k + g * hd + i);
+            }
+            s_q[i] = qv * a.scale;
+            s_k[i] = kvv;
+            s_v[i] = ldcg_f(a.v + g * hd + i);
+        }
+        MK_SYNC();
+        // one CTA per kv group appends this token's row: no CTA reads cache row kv_len in this phase
+        const bool owner = part == 0 && (KV_F16 ? (h % (n_heads / n_kv) == 0) : (h < n_kv));
+        if (owner) {
+            for (int i = threadIdx.x; i < hd; i += MK_THREADS) {
+                const int64_t off = (int64_t)g * seq_stride + (int64_t)kv_len * hd + i;
+                if (KV_F16) { ((__half*)a.kcache)[off] = __float2half_rn(s_k[i]); ((__half*)a.vcache)[off] = __float2half_rn(s_v[i]); }
+                else { ((float*)a.kcache)[off] = s_k[i]; ((float*)a.vcache)[off] = s_v[i]; }
+            }
+        }
+        float* srow = scores + (size_t)h * (size_t)(a.max_len + 1);
+        // scores, chunk by chunk; per-lane summation order i = lane, lane+32, ... as in fused.cu
+        for (int j = 0; j < NCK; j++) {
+            const int p0 = p_lo + j * at_ch, cnt = min(at_ch, k_hi - p0);
+            const uint8_t* kb = s_buf + (size_t)(j % AT_NBUF) * buf_bytes;
+            wait_job(j);
+            for (int s = warp; s < cnt; s += MK_WARPS) {
+                float acc = 0.0f;
+                for (int i = lane; i < hd; i += 32) acc += (KV_F16 ? __half2float(__float2half_rn(s_q[i])) : s_q[i]) * ld_kv(kb, s * hd + i);
+                acc = warp_sum(acc);
+                if (lane == 0) { s_p[p0 + s] = acc; srow[p0 + s] = acc; }
+            }
+            MK_SYNC();                                       // buffer consumed by every warp -> refill it
+            if (j + AT_NBUF < NJ) issue_job(j + AT_NBUF);
+        }
+        if (warp == 0 && p_hi == L) {                              // this token's own position (the last range)
+            float acc = 0.0f;
+            for (int i = lane; i < hd; i += 32) {
+                if (KV_F16) acc += __half2float(__float2half_rn(s_q[i])) * __half2float(__float2half_rn(s_k[i]));
+                else acc += s_q[i] * s_k[i];
+            }
+            acc = warp_sum(acc);
+            if (lane == 0) { s_p[kv_len] = acc; srow[kv_len] = acc; }
+        }
+        MK_SYNC();
+        {
+            // score exchange: the MK_SYNC above orders the CTA's row stores before the release; the arrival word is monotonic across phases
+            // and launches (each phase adds AT_SPLIT_MAX in all), so the value it held before this CTA's add tells which phase this is
+            if (threadIdx.x == 0) {
+                unsigned* w = bar + AT_ARRIVE_WORD + 8 * h;
+                const unsigned old = atom_add_release(w, AT_SPLIT_MAX / S), target = (old & ~(unsigned)(AT_SPLIT_MAX - 1)) + AT_SPLIT_MAX;
+                MkSpin sp;
+                for (unsigned v = old + AT_SPLIT_MAX / S; (int)(v - target) < 0; v = ld_acquire_u32(w))      // the last to arrive does not poll
+                    if (sp.expired(bar, err_host, 1u)) { *s_abort = 1; break; }
+            }
+            MK_SYNC();
+            for (int s = threadIdx.x; s < L; s += MK_THREADS) if (s < p_lo || s >= p_hi) s_p[s] = ldcg_f(srow + s);
+            MK_SYNC();
+        }
+        float m = -INFINITY;
+        for (int s = threadIdx.x; s < L; s += MK_THREADS) m = fmaxf(m, s_p[s]);
+        m = warp_max(m);
+        if (lane == 0) s_red[warp] = m;
+        MK_SYNC();
+        m = s_red[0];
+#pragma unroll
+        for (int w = 1; w < MK_WARPS; w++) m = fmaxf(m, s_red[w]);
+        MK_SYNC();
+        float sum = 0.0f;
+        for (int s = threadIdx.x; s < L; s += MK_THREADS) {
+            float e = h2f_bits(exp_lut[f2h_bits(s_p[s] - m)]);
+            s_p[s] = e;
+            sum += e;
+        }
+        sum = warp_sum(sum);
+        if (lane == 0) s_red[warp] = sum;
+        MK_SYNC();
+        sum = 0.0f;
+#pragma unroll
+        for (int w = 0; w < MK_WARPS; w++) sum += s_red[w];
+        for (int s = threadIdx.x; s < L; s += MK_THREADS) s_p[s] = s_p[s] / sum;
+        MK_SYNC();
+        // out[d] = sum_s p[s] * V[s][d], sequential over s (batch_matmul.rs:60-68 order); F16: f16 accumulation (buf_f16.rs:152-163)
+        float accf = 0.0f;
+        __half acch = __float2half_rn(0.0f);
+        const int t = threadIdx.x, d = part * dw + t;
+        for (int j = NCK; j < NJ; j++) {
+            const int p0 = (j - NCK) * vch, cnt = min(vch, kv_len - p0);
+            const uint8_t* vb = s_buf + (size_t)(j % AT_NBUF) * buf_bytes;
+            wait_job(j);
+            if (t < dw) {
+                for (int s = 0; s < cnt; s++) {
+                    if (KV_F16) acch = __hadd(acch, __hmul(((const __half*)vb)[s * dw + t], __float2half_rn(s_p[p0 + s])));
+                    else accf += s_p[p0 + s] * ((const float*)vb)[s * dw + t];
+                }
+            }
+            MK_SYNC();
+            if (j + AT_NBUF < NJ) issue_job(j + AT_NBUF);
+        }
+        float* s_o = s_k;
+        MK_SYNC();
+        if (t < dw) {
+            float o;
+            if (KV_F16) { acch = __hadd(acch, __hmul(__float2half_rn(s_v[d]), __float2half_rn(s_p[kv_len]))); o = __half2float(acch); }
+            else { accf += s_p[kv_len] * s_v[d]; o = accf; }
+            a.out[h * hd + d] = o;
+            s_o[t] = o;
+        }
+        MK_SYNC();
+        if (a.act_scratch) {
+            ActQ8_0 act = ph.act;
+            for (int b = warp; b < (dw >> 5); b += MK_WARPS) {
+                float v = s_o[b * 32 + lane];
+                float amax = warp_max(fabsf(v));
+                float dd = amax / 127.0f;
+                int qq = __float2int_rz(v / dd);
+                const int gb = h * (hd >> 5) + part * (dw >> 5) + b;
+                act.qs[gb * 32 + lane] = (int8_t)qq;
+                int ss = warp_sum_i(qq);
+                if (lane == 0) { act.d[gb] = __half2float(__float2half_rn(dd)); act.isum[gb] = ss; }
+            }
+        }
+        MK_SYNC();
+    }
+}
+
+// below AT_SPLIT_MIN_KV cached positions the score exchange costs more than the split saves (Llama-2-7B, per layer, split against one
+// CTA per head: 10.4 / 8.8 us at ~60 positions, 14.3 / 12.9 at ~190, 22.3 / 23.1 at ~440, 70 / 88 at ~2040; NVIDIA H100 80GB HBM3,
+// 700 W): one CTA per head
+template <bool KV_F16>
+static __device__ __forceinline__ void phase_attn(const MkPhase& ph, float* sm, float* s_red, const uint8_t* dyn, const uint16_t* exp_lut, unsigned abar0, unsigned& apar,
+                                                  const int at_ch, unsigned* bar, unsigned* err_host, int* s_abort, float* scores) {
+    if (ph.at.split > 1 && ((const int64_t*)(dyn + ph.dyn_off))[1] >= AT_SPLIT_MIN_KV) phase_attn_split<KV_F16>(ph, sm, s_red, dyn, exp_lut, abar0, apar, at_ch, bar, err_host, s_abort, scores);
+    else phase_attn_one<KV_F16>(ph, sm, s_red, dyn, exp_lut, abar0, apar, at_ch);
 }
 
 // ---- ROWS phase: copy_rows_from with the row indices in dyn (embedding lookup / row pick) -----------------------------------

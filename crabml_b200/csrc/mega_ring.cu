@@ -503,7 +503,7 @@ __device__ void phase_matvec_ring(const MkPhase& ph, uint8_t* smem, float* s_wn,
 template <bool GEN, bool SMP>      // SMP: the table ends with its only SAMPLE phase (see mega.cu)
 __global__ void __launch_bounds__(MR_THREADS, 1) mega_ring_kernel(const MkPhase* __restrict__ phases, int n_phases, const uint8_t* dyn, unsigned* bar,
                                                                   const uint16_t* exp_lut, unsigned long long* prof, bool test_stall, int wtop_off, unsigned* err_host,
-                                                                  const CommDev comm, const MrRing R) {
+                                                                  const CommDev comm, const MrRing R, float* scores) {
     extern __shared__ __align__(128) uint8_t smem[];
     __shared__ float s_red[MK_WARPS];
     __shared__ MkPhase s_phs[2];             // phase descriptors of the compute warps, double-buffered
@@ -576,8 +576,8 @@ __global__ void __launch_bounds__(MR_THREADS, 1) mega_ring_kernel(const MkPhase*
             else phase_matvec_ring<CC_Q4_0>(s_ph, work, s_wn, wst, xstaged == p, exp_lut, RC, comm, xseq, st1);
             break;
         case MK_ATTN:
-            if (s_ph.at.kv_f16) phase_attn<true>(s_ph, (float*)work, s_red, dyn, exp_lut, abar0, apar, R.at_ch);
-            else phase_attn<false>(s_ph, (float*)work, s_red, dyn, exp_lut, abar0, apar, R.at_ch);
+            if (s_ph.at.kv_f16) phase_attn<true>(s_ph, (float*)work, s_red, dyn, exp_lut, abar0, apar, R.at_ch, bar, err_host, &s_abort, scores);
+            else phase_attn<false>(s_ph, (float*)work, s_red, dyn, exp_lut, abar0, apar, R.at_ch, bar, err_host, &s_abort, scores);
             break;
         case MK_ROWS: phase_rows(s_ph, dyn); break;
         case MK_REDUCE: phase_reduce(s_ph, comm, xseq, false); break;
@@ -630,7 +630,7 @@ bool cc_mega_ring_phase_ok(const MkPhase& ph) {
         if (((uintptr_t)ph.mv.mats.qs[t] | (uintptr_t)ph.mv.mats.d[t]) & 15u) return false;
     return true;
 }
-int cc_mega_ring_at_ch(const MkPhase& ph) {       // 48 KB of cache rows in flight per head either way
+int cc_mega_ring_at_ch(const MkPhase& ph) {       // 48 KB of cache rows in flight per CTA either way (a V chunk: S times the rows, 1 / S of the columns)
     return ph.at.kv_f16 ? 64 : 32;
 }
 size_t cc_mega_ring_smem_for_phase(const MkPhase& ph) {
@@ -680,5 +680,5 @@ int cc_launch_mega_ring(cc_device* dev, const MkPhase* phases_dev, int n_phases,
     R.ring_off = (int)ring_off; R.slot_bytes = L.slot_bytes; R.nslots = L.nslots; R.at_ch = L.at_ch;
     const uint16_t* lut = dev->exp_lut;
     return mk_launch(dev, kern, dev->sm_count, MR_THREADS, smem, phases_dev, n_phases, dyn_dev, bar_dev, lut, prof, cc_mega_test_stall(), (int)wtop,
-                     dev->err_host, (const CommDev)cd, (const MrRing)R);
+                     dev->err_host, (const CommDev)cd, (const MrRing)R, L.scores);
 }
