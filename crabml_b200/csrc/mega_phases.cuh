@@ -326,199 +326,38 @@ static __device__ MK_GENERIC_ATTR void phase_matvec_generic(const MkPhase& ph, u
     flush_pending();
 }
 
-// ---- ATTN phase: arithmetic of fused.cu attn_decode_kernel, heads dealt to CTAs (phase_attn_one) or each head to a.split = S CTAs
-// (phase_attn_split, cc_attn_split).  The K (then V) rows a CTA reads are staged in shared memory in chunks with ALL loads of a chunk in
-// flight at once: at decode the cost of this phase is HBM/L2 latency and the one SM a head's history streams through, not bandwidth, so
-// round trips and SMs per head are what matter.
+// ---- ATTN phase: arithmetic of fused.cu attn_decode_kernel, each head on S CTAs (phase_attn: S = 1 on a short history, else a.split
+// from cc_attn_split).  The K (then V) rows a CTA reads are staged in shared memory in chunks with ALL loads of a chunk in flight at once: at
+// decode the cost of this phase is HBM/L2 latency and the one SM a head's history streams through, not bandwidth, so round trips and SMs
+// per head are what matter.
 #define AT_CH 64
 #define AT_NBUF 3
-// one CTA per head: the K (then V) rows of the head are contiguous in the cache, one bulk copy per chunk of at_ch rows
-template <bool KV_F16>
-static __device__ void phase_attn_one(const MkPhase& ph, float* sm, float* s_red, const uint8_t* dyn, const uint16_t* exp_lut, unsigned abar0, unsigned& apar, const int at_ch) {
-    const AttnArgs& a = ph.at;
-    const int n_heads = a.n_heads, n_kv = a.n_kv, hd = a.hd, rope_dim = a.rope_dim;
-    const int64_t seq_stride = a.seq_stride;
-    const int64_t* dynv = (const int64_t*)(dyn + ph.dyn_off);
-    const float* rope_tab = (const float*)(dyn + ph.rope_off);
-    const int kv_len = (int)dynv[1], L = kv_len + 1;
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    float* s_q = sm; float* s_k = sm + hd; float* s_v = sm + 2 * hd; float* s_p = sm + 3 * hd;
-    // AT_NBUF chunk buffers of at_ch cache rows each (raw bytes: f32 or f16), filled by TMA bulk copies -- the rows of one kv head
-    // are contiguous -- in a K-chunks-then-V-chunks job sequence with AT_NBUF jobs in flight; one mbarrier per buffer.
-    uint8_t* s_buf = (uint8_t*)(sm + 3 * hd + ((a.max_len + 8 + 3) & ~3));
-    const unsigned s_buf_smem = (unsigned)__cvta_generic_to_shared(s_buf);
-    constexpr int ELT = KV_F16 ? 2 : 4;
-    const unsigned buf_bytes = (unsigned)(at_ch * hd * ELT);
-    const int pairs = rope_dim >> 1;
-    const int hd4 = hd >> 2;
-    const int NC = (kv_len + at_ch - 1) / at_ch;                  // chunks per pass; jobs 0..NC-1 = K chunks, NC..2NC-1 = V chunks
-    auto issue_job = [&](int g, int j) {                            // one elected thread
-        const int c = j < NC ? j : j - NC;
-        const int p0 = c * at_ch, cnt = min(at_ch, kv_len - p0);
-        const uint8_t* src = (const uint8_t*)(j < NC ? a.kcache : a.vcache) + ((int64_t)g * seq_stride + (int64_t)p0 * hd) * ELT;
-        const unsigned bytes = (unsigned)(cnt * hd * ELT), bar = abar0 + 8u * (unsigned)(j % AT_NBUF), dst = s_buf_smem + (unsigned)(j % AT_NBUF) * buf_bytes;
-        asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-        asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
-    };
-    auto wait_job = [&](int j) {                                    // all threads, in job order
-        const int bsel = j % AT_NBUF;
-        mbar_wait(abar0 + 8u * (unsigned)bsel, (apar >> bsel) & 1u);
-        apar ^= 1u << bsel;
-    };
-    auto ld_kv = [&](const uint8_t* buf, int idx) -> float { return KV_F16 ? __half2float(((const __half*)buf)[idx]) : ((const float*)buf)[idx]; };
-    for (int h = blockIdx.x; h < n_heads; h += gridDim.x) {
-        const int g = KV_F16 ? h / (n_heads / n_kv) : h % n_kv;
-        // the first AT_NBUF jobs are requested up front; every later job is issued as soon as its buffer has been consumed
-        if (threadIdx.x == 0) for (int j = 0; j < min(AT_NBUF, 2 * NC); j++) issue_job(g, j);
-        for (int i = threadIdx.x; i < hd; i += MK_THREADS) {
-            float qv, kvv;
-            if (i < rope_dim) {
-                const int j = i >> 1;
-                const float c = rope_tab[j], s = rope_tab[pairs + j];
-                const float q0 = ldcg_f(a.q + h * hd + 2 * j), q1 = ldcg_f(a.q + h * hd + 2 * j + 1);
-                const float k0 = ldcg_f(a.k + g * hd + 2 * j), k1 = ldcg_f(a.k + g * hd + 2 * j + 1);
-                qv = (i & 1) ? q0 * s + q1 * c : q0 * c - q1 * s;
-                kvv = (i & 1) ? k0 * s + k1 * c : k0 * c - k1 * s;
-            } else {
-                qv = ldcg_f(a.q + h * hd + i);
-                kvv = ldcg_f(a.k + g * hd + i);
-            }
-            s_q[i] = qv * a.scale;
-            s_k[i] = kvv;
-            s_v[i] = ldcg_f(a.v + g * hd + i);
-        }
-        MK_SYNC();
-        const bool owner = KV_F16 ? (h % (n_heads / n_kv) == 0) : (h < n_kv);
-        if (owner) {
-            for (int i = threadIdx.x; i < hd; i += MK_THREADS) {
-                const int64_t off = (int64_t)g * seq_stride + (int64_t)kv_len * hd + i;
-                if (KV_F16) { ((__half*)a.kcache)[off] = __float2half_rn(s_k[i]); ((__half*)a.vcache)[off] = __float2half_rn(s_v[i]); }
-                else { ((float*)a.kcache)[off] = s_k[i]; ((float*)a.vcache)[off] = s_v[i]; }
-            }
-        }
-        // scores, chunk by chunk; per-lane summation order i = lane, lane+32, ... as in fused.cu
-        for (int j = 0; j < NC; j++) {
-            const int p0 = j * at_ch, cnt = min(at_ch, kv_len - p0);
-            const uint8_t* kb = s_buf + (size_t)(j % AT_NBUF) * buf_bytes;
-            wait_job(j);
-            for (int s = warp; s < cnt; s += MK_WARPS) {
-                float acc = 0.0f;
-                for (int i = lane; i < hd; i += 32) acc += (KV_F16 ? __half2float(__float2half_rn(s_q[i])) : s_q[i]) * ld_kv(kb, s * hd + i);
-                acc = warp_sum(acc);
-                if (lane == 0) s_p[p0 + s] = acc;
-            }
-            MK_SYNC();                                       // buffer consumed by every warp -> refill it
-            if (threadIdx.x == 0 && j + AT_NBUF < 2 * NC) issue_job(g, j + AT_NBUF);
-        }
-        if (warp == 0) {                                           // this token's own position
-            float acc = 0.0f;
-            for (int i = lane; i < hd; i += 32) {
-                if (KV_F16) acc += __half2float(__float2half_rn(s_q[i])) * __half2float(__float2half_rn(s_k[i]));
-                else acc += s_q[i] * s_k[i];
-            }
-            acc = warp_sum(acc);
-            if (lane == 0) s_p[kv_len] = acc;
-        }
-        MK_SYNC();
-        float m = -INFINITY;
-        for (int s = threadIdx.x; s < L; s += MK_THREADS) m = fmaxf(m, s_p[s]);
-        m = warp_max(m);
-        if (lane == 0) s_red[warp] = m;
-        MK_SYNC();
-        m = s_red[0];
-#pragma unroll
-        for (int w = 1; w < MK_WARPS; w++) m = fmaxf(m, s_red[w]);
-        MK_SYNC();
-        float sum = 0.0f;
-        for (int s = threadIdx.x; s < L; s += MK_THREADS) {
-            float e = h2f_bits(exp_lut[f2h_bits(s_p[s] - m)]);
-            s_p[s] = e;
-            sum += e;
-        }
-        sum = warp_sum(sum);
-        if (lane == 0) s_red[warp] = sum;
-        MK_SYNC();
-        sum = 0.0f;
-#pragma unroll
-        for (int w = 0; w < MK_WARPS; w++) sum += s_red[w];
-        for (int s = threadIdx.x; s < L; s += MK_THREADS) s_p[s] = s_p[s] / sum;
-        MK_SYNC();
-        // out[d] = sum_s p[s] * V[s][d], sequential over s (batch_matmul.rs:60-68 order); F16: f16 accumulation (buf_f16.rs:152-163)
-        float accf = 0.0f;
-        __half acch = __float2half_rn(0.0f);
-        const int d = threadIdx.x;
-        for (int j = NC; j < 2 * NC; j++) {
-            const int p0 = (j - NC) * at_ch, cnt = min(at_ch, kv_len - p0);
-            const uint8_t* vb = s_buf + (size_t)(j % AT_NBUF) * buf_bytes;
-            wait_job(j);
-            if (d < hd) {
-                for (int s = 0; s < cnt; s++) {
-                    if (KV_F16) acch = __hadd(acch, __hmul(((const __half*)vb)[s * hd + d], __float2half_rn(s_p[p0 + s])));
-                    else accf += s_p[p0 + s] * ((const float*)vb)[s * hd + d];
-                }
-            }
-            MK_SYNC();
-            if (threadIdx.x == 0 && j + AT_NBUF < 2 * NC) issue_job(g, j + AT_NBUF);
-        }
-        float* s_o = s_k;
-        MK_SYNC();
-        if (d < hd) {
-            float o;
-            if (KV_F16) { acch = __hadd(acch, __hmul(__float2half_rn(s_v[d]), __float2half_rn(s_p[kv_len]))); o = __half2float(acch); }
-            else { accf += s_p[kv_len] * s_v[d]; o = accf; }
-            a.out[h * hd + d] = o;
-            s_o[d] = o;
-        }
-        MK_SYNC();
-        if (a.act_scratch) {
-            ActQ8_0 act = ph.act;
-            for (int b = warp; b < (hd >> 5); b += MK_WARPS) {
-                float v = s_o[b * 32 + lane];
-                float amax = warp_max(fabsf(v));
-                float dd = amax / 127.0f;
-                int qq = __float2int_rz(v / dd);
-                const int gb = h * (hd >> 5) + b;
-                act.qs[gb * 32 + lane] = (int8_t)qq;
-                int ss = warp_sum_i(qq);
-                if (lane == 0) { act.d[gb] = __half2float(__float2half_rn(dd)); act.isum[gb] = ss; }
-            }
-        }
-        MK_SYNC();
-    }
-}
-
-// a called function in the ring kernel (MK_GENERIC_NOINLINE), as the generic phase: inlined there, it cost the phases every token runs
-// (Llama-2-7B Q8_0 at ~32-104 positions decoded 268 instead of 271 tok/s; called, 280: the kernel spills less than before the split;
-// NVIDIA H100 80GB HBM3, 700 W).  Inlined in mega.cu, where a call spills more (nvcc 12.9 -Xptxas -v).
-#if MK_GENERIC_NOINLINE
-#define MK_ATTN_SPLIT_ATTR __noinline__
-#else
-#define MK_ATTN_SPLIT_ATTR
-#endif
 __device__ __forceinline__ unsigned atom_add_release(unsigned* p, unsigned v) {
     unsigned old;
     asm volatile("atom.release.gpu.global.add.u32 %0, [%1], %2;" : "=r"(old) : "l"(p), "r"(v) : "memory");
     return old;
 }
-// CTA c of head h scores the positions [c L / S, (c + 1) L / S) (the last range holds this token's own position, scored from s_q . s_k)
-// and publishes them in the head's row of the score scratch; once all S CTAs have arrived every CTA reads the whole row and runs the softmax over
-// it in the canonical order, so all of them hold the same p; CTA c then accumulates PV for the dimensions [c hd / S, (c + 1) hd / S),
-// sequentially over s, and quantises those hd / (32 S) Q8_0 blocks of the output.  Each score is an independent dot product and each
-// output element's PV sum keeps its order: the bits are those of phase_attn_one.
-template <bool KV_F16>
-static __device__ MK_ATTN_SPLIT_ATTR void phase_attn_split(const MkPhase& ph, float* sm, float* s_red, const uint8_t* dyn, const uint16_t* exp_lut, unsigned abar0, unsigned& apar, const int at_ch,
+// Each head on S CTAs: S = a.split when SPLIT, else 1.  CTA c of head h scores the positions [c L / S, (c + 1) L / S) (the last range
+// holds this token's own position, scored from s_q . s_k).  With SPLIT it publishes them in the head's row of the score scratch; once all
+// S CTAs have arrived every CTA reads the whole row and runs the softmax over it in the canonical order, so all of them hold the same p.
+// CTA c then accumulates PV for the dimensions [c hd / S, (c + 1) hd / S), sequentially over s, and quantises those hd / (32 S) Q8_0
+// blocks of the output.  Each score is an independent dot product and each output element's PV sum keeps its order, so the bits do not
+// depend on S.
+template <bool KV_F16, bool SPLIT>
+static __device__ void phase_attn_heads(const MkPhase& ph, float* sm, float* s_red, const uint8_t* dyn, const uint16_t* exp_lut, unsigned abar0, unsigned& apar, const int at_ch,
                                         unsigned* bar, unsigned* err_host, int* s_abort, float* scores) {
     const AttnArgs& a = ph.at;
-    const int n_heads = a.n_heads, n_kv = a.n_kv, hd = a.hd, rope_dim = a.rope_dim, S = a.split;
+    const int n_heads = a.n_heads, n_kv = a.n_kv, hd = a.hd, rope_dim = a.rope_dim, S = SPLIT ? a.split : 1;
     const int64_t seq_stride = a.seq_stride;
     const int64_t* dynv = (const int64_t*)(dyn + ph.dyn_off);
     const float* rope_tab = (const float*)(dyn + ph.rope_off);
     const int kv_len = (int)dynv[1], L = kv_len + 1;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     float* s_q = sm; float* s_k = sm + hd; float* s_v = sm + 2 * hd; float* s_p = sm + 3 * hd;
-    // AT_NBUF chunk buffers of at_ch cache rows each (raw bytes: f32 or f16), filled by TMA bulk copies in a K-chunks-then-V-chunks job
-    // sequence with AT_NBUF jobs in flight; one mbarrier per buffer.  A K chunk is at_ch contiguous rows of the CTA's range; a V chunk is
-    // vch = S at_ch rows of the CTA's dw = hd / S columns (the same bytes: the working area does not depend on S), one copy per row.
+    // AT_NBUF chunk buffers of at_ch cache rows each (raw bytes: f32 or f16), filled in a K-chunks-then-V-chunks job sequence with
+    // AT_NBUF jobs in flight; one mbarrier per buffer.  A K chunk is at_ch contiguous rows of the CTA's range, one TMA bulk copy.  A V
+    // chunk is vch = S at_ch rows of the CTA's dw = hd / S columns (the same bytes: the working area does not depend on S): with S = 1
+    // contiguous rows again, one bulk copy; with S > 1 a strided slice of every row.
     uint8_t* s_buf = (uint8_t*)(sm + 3 * hd + ((a.max_len + 8 + 3) & ~3));
     const unsigned s_buf_smem = (unsigned)__cvta_generic_to_shared(s_buf);
     constexpr int ELT = KV_F16 ? 2 : 4;
@@ -527,18 +366,20 @@ static __device__ MK_ATTN_SPLIT_ATTR void phase_attn_split(const MkPhase& ph, fl
     const int dw = hd / S, vch = at_ch * S;
     const int NCV = (kv_len + vch - 1) / vch;                     // V chunks: every CTA of the head reads all kv_len rows (its columns)
     for (int u = blockIdx.x; u < n_heads * S; u += gridDim.x) {
-        const int h = u % n_heads, part = u / n_heads;           // part-major: part 0 of every head on the CTA that has it without the split
+        const int part = SPLIT ? u / n_heads : 0, h = u - part * n_heads;      // part-major: part 0 of every head on the CTA that has it without the split
         const int g = KV_F16 ? h / (n_heads / n_kv) : h % n_kv;
-        const int p_lo = (int)((int64_t)part * L / S), p_hi = (int)((int64_t)(part + 1) * L / S), k_hi = min(p_hi, kv_len);
-        const int NCK = k_hi > p_lo ? (k_hi - p_lo + at_ch - 1) / at_ch : 0;      // K chunks of the cached positions in [p_lo, p_hi)
+        const int p_lo = (int)((int64_t)part * L / S), p_hi = (int)((int64_t)(part + 1) * L / S), k_hi = SPLIT ? min(p_hi, kv_len) : kv_len;
+        const int NCK = !SPLIT ? NCV : k_hi > p_lo ? (k_hi - p_lo + at_ch - 1) / at_ch : 0;      // K chunks of the cached positions in [p_lo, p_hi)
         const int NJ = NCK + NCV;
-        int v_issued = 0;                                            // V chunks requested so far (one cp.async group each)
-        auto issue_job = [&](int j) {                                // all threads
+        int v_issued = 0;                                            // SPLIT: V chunks requested so far (one cp.async group each)
+        const bool issuer = SPLIT || threadIdx.x == 0;               // who requests a job: all threads with cp.async V pieces, else thread 0
+        auto issue_job = [&](int j) {                                // the issuers
             const unsigned mb = abar0 + 8u * (unsigned)(j % AT_NBUF), dst = s_buf_smem + (unsigned)(j % AT_NBUF) * buf_bytes;
-            if (j < NCK) {                                           // contiguous K rows: one bulk copy
-                const int p0 = p_lo + j * at_ch, cnt = min(at_ch, k_hi - p0);
+            if (j < NCK || !SPLIT) {                                 // contiguous rows: one bulk copy
+                const bool kj = j < NCK;
+                const int p0 = kj ? p_lo + j * at_ch : (j - NCK) * at_ch, cnt = min(at_ch, (kj ? k_hi : kv_len) - p0);
                 if (threadIdx.x == 0) {
-                    const uint8_t* src = (const uint8_t*)a.kcache + ((int64_t)g * seq_stride + (int64_t)p0 * hd) * ELT;
+                    const uint8_t* src = (const uint8_t*)(kj ? a.kcache : a.vcache) + ((int64_t)g * seq_stride + (int64_t)p0 * hd) * ELT;
                     const unsigned bytes = (unsigned)(cnt * hd * ELT);
                     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(mb), "r"(bytes) : "memory");
                     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst), "l"(src), "r"(bytes), "r"(mb) : "memory");
@@ -557,7 +398,7 @@ static __device__ MK_ATTN_SPLIT_ATTR void phase_attn_split(const MkPhase& ph, fl
             }
         };
         auto wait_job = [&](int j) {                                // all threads, in job order
-            if (j >= NCK) {                                          // this thread's pieces of chunk j have landed (later chunks may still be in flight), then everybody's
+            if (SPLIT && j >= NCK) {                                 // this thread's pieces of chunk j have landed (later chunks may still be in flight), then everybody's
                 const int newer = v_issued - (j - NCK) - 1;
                 if (newer >= 2) asm volatile("cp.async.wait_group 2;" ::: "memory");
                 else if (newer == 1) asm volatile("cp.async.wait_group 1;" ::: "memory");
@@ -571,7 +412,7 @@ static __device__ MK_ATTN_SPLIT_ATTR void phase_attn_split(const MkPhase& ph, fl
         };
         auto ld_kv = [&](const uint8_t* buf, int idx) -> float { return KV_F16 ? __half2float(((const __half*)buf)[idx]) : ((const float*)buf)[idx]; };
         // the first AT_NBUF jobs are requested up front; every later job is issued as soon as its buffer has been consumed
-        for (int j = 0; j < min(AT_NBUF, NJ); j++) issue_job(j);
+        if (issuer) for (int j = 0; j < min(AT_NBUF, NJ); j++) issue_job(j);
         for (int i = threadIdx.x; i < hd; i += MK_THREADS) {
             float qv, kvv;
             if (i < rope_dim) {
@@ -599,7 +440,7 @@ static __device__ MK_ATTN_SPLIT_ATTR void phase_attn_split(const MkPhase& ph, fl
                 else { ((float*)a.kcache)[off] = s_k[i]; ((float*)a.vcache)[off] = s_v[i]; }
             }
         }
-        float* srow = scores + (size_t)h * (size_t)(a.max_len + 1);
+        float* srow = SPLIT ? scores + (size_t)h * (size_t)(a.max_len + 1) : nullptr;
         // scores, chunk by chunk; per-lane summation order i = lane, lane+32, ... as in fused.cu
         for (int j = 0; j < NCK; j++) {
             const int p0 = p_lo + j * at_ch, cnt = min(at_ch, k_hi - p0);
@@ -609,10 +450,10 @@ static __device__ MK_ATTN_SPLIT_ATTR void phase_attn_split(const MkPhase& ph, fl
                 float acc = 0.0f;
                 for (int i = lane; i < hd; i += 32) acc += (KV_F16 ? __half2float(__float2half_rn(s_q[i])) : s_q[i]) * ld_kv(kb, s * hd + i);
                 acc = warp_sum(acc);
-                if (lane == 0) { s_p[p0 + s] = acc; srow[p0 + s] = acc; }
+                if (lane == 0) { s_p[p0 + s] = acc; if (SPLIT) srow[p0 + s] = acc; }
             }
             MK_SYNC();                                       // buffer consumed by every warp -> refill it
-            if (j + AT_NBUF < NJ) issue_job(j + AT_NBUF);
+            if (issuer && j + AT_NBUF < NJ) issue_job(j + AT_NBUF);
         }
         if (warp == 0 && p_hi == L) {                              // this token's own position (the last range)
             float acc = 0.0f;
@@ -621,10 +462,10 @@ static __device__ MK_ATTN_SPLIT_ATTR void phase_attn_split(const MkPhase& ph, fl
                 else acc += s_q[i] * s_k[i];
             }
             acc = warp_sum(acc);
-            if (lane == 0) { s_p[kv_len] = acc; srow[kv_len] = acc; }
+            if (lane == 0) { s_p[kv_len] = acc; if (SPLIT) srow[kv_len] = acc; }
         }
         MK_SYNC();
-        {
+        if (SPLIT) {
             // score exchange: the MK_SYNC above orders the CTA's row stores before the release; the arrival word is monotonic across phases
             // and launches (each phase adds AT_SPLIT_MAX in all), so the value it held before this CTA's add tells which phase this is
             if (threadIdx.x == 0) {
@@ -676,7 +517,7 @@ static __device__ MK_ATTN_SPLIT_ATTR void phase_attn_split(const MkPhase& ph, fl
                 }
             }
             MK_SYNC();
-            if (j + AT_NBUF < NJ) issue_job(j + AT_NBUF);
+            if (issuer && j + AT_NBUF < NJ) issue_job(j + AT_NBUF);
         }
         float* s_o = s_k;
         MK_SYNC();
@@ -705,6 +546,24 @@ static __device__ MK_ATTN_SPLIT_ATTR void phase_attn_split(const MkPhase& ph, fl
     }
 }
 
+// SPLIT is a template parameter, and the one-CTA instantiation folds to the code of a one-CTA phase (thread 0 requests every job, K and V
+// chunks cover the same kv_len rows) and stays inline: both kernels then compile to the registers, frames, spills and instruction counts
+// of separate one-CTA and split functions (nvcc 12.9 -Xptxas -v).  One called function with a run-time S took 12.7 instead of 9.1 us per
+// layer at ~60 positions; folding less than this cost the K-quant kernel 4 % (Llama-2-7B; NVIDIA H100 80GB HBM3, 700 W).  The split
+// instantiation is a called function in the ring kernel (MK_GENERIC_NOINLINE), as the generic phase: inlined there, it cost the phases
+// every token runs (Llama-2-7B Q8_0 at ~32-104 positions decoded 268 instead of 271 tok/s; called, 280: the kernel spills
+// less than before the split; NVIDIA H100 80GB HBM3, 700 W).  Inlined in mega.cu, where a call spills more (nvcc 12.9 -Xptxas -v).
+#if MK_GENERIC_NOINLINE
+#define MK_ATTN_SPLIT_ATTR __noinline__
+#else
+#define MK_ATTN_SPLIT_ATTR
+#endif
+template <bool KV_F16>
+static __device__ MK_ATTN_SPLIT_ATTR void phase_attn_split(const MkPhase& ph, float* sm, float* s_red, const uint8_t* dyn, const uint16_t* exp_lut, unsigned abar0, unsigned& apar, const int at_ch,
+                                        unsigned* bar, unsigned* err_host, int* s_abort, float* scores) {
+    phase_attn_heads<KV_F16, true>(ph, sm, s_red, dyn, exp_lut, abar0, apar, at_ch, bar, err_host, s_abort, scores);
+}
+
 // below AT_SPLIT_MIN_KV cached positions the score exchange costs more than the split saves (Llama-2-7B, per layer, split against one
 // CTA per head: 10.4 / 8.8 us at ~60 positions, 14.3 / 12.9 at ~190, 22.3 / 23.1 at ~440, 70 / 88 at ~2040; NVIDIA H100 80GB HBM3,
 // 700 W): one CTA per head
@@ -712,7 +571,7 @@ template <bool KV_F16>
 static __device__ __forceinline__ void phase_attn(const MkPhase& ph, float* sm, float* s_red, const uint8_t* dyn, const uint16_t* exp_lut, unsigned abar0, unsigned& apar,
                                                   const int at_ch, unsigned* bar, unsigned* err_host, int* s_abort, float* scores) {
     if (ph.at.split > 1 && ((const int64_t*)(dyn + ph.dyn_off))[1] >= AT_SPLIT_MIN_KV) phase_attn_split<KV_F16>(ph, sm, s_red, dyn, exp_lut, abar0, apar, at_ch, bar, err_host, s_abort, scores);
-    else phase_attn_one<KV_F16>(ph, sm, s_red, dyn, exp_lut, abar0, apar, at_ch);
+    else phase_attn_heads<KV_F16, false>(ph, sm, s_red, dyn, exp_lut, abar0, apar, at_ch, bar, err_host, s_abort, scores);
 }
 
 // ---- ROWS phase: copy_rows_from with the row indices in dyn (embedding lookup / row pick) -----------------------------------
