@@ -263,22 +263,22 @@ struct StreamArgs {
     StreamMats mats;
     const void* act;         // ActQ8_0 scratch (quantize.cu layout) of k elements
     int k;
-    int epilogue;            // 0 store, 1 add residual, 2 silu(mat0 row) * (mat1 row), 3 store into every rank's exchange slot (megakernel)
-    const float* residual;
-    const uint16_t* exp_lut;
+    int epilogue;            // 0 store, 1 add residual[mat] (llama2.rs residual adds, qwen2 q/k/v biases), 2 silu(mat0 row) * (mat1 row),
+                             // 3 store into every rank's exchange slot (megakernel)
+    const float* residual[3];   // epilogue 1: out[mat][r] = dot + residual[mat][r], one f32 vector per matrix
 };
 struct AttnArgs {            // fused decode attention (fused.cu)
     const float *q, *k, *v;  // raw matvec outputs [n_heads*hd], [n_kv*hd], [n_kv*hd]
     void *kcache, *vcache;   // [n_kv, seq_max, hd] F32 or F16
     float* out;              // [n_heads*hd]
     void* act_scratch;       // Q8_0 quantisation of out
-    const int64_t* dyn;      // device: {pos, kv_len}
-    const float* rope_tab;   // device: cos[rope_dim/2], sin[rope_dim/2]
     int n_heads, n_kv, hd, rope_dim, max_len, kv_f16;
     int64_t seq_stride;
     float scale;
     int split;               // megakernels: CTAs per head (lazy.cu: the most the score scratch allows, then cc_attn_split); the fused kernel ignores it
+    int rope_neox;           // RoPE pairs: 0 llama (2j, 2j+1), 1 neox (j, j + hd/2), j < rope_dim/2 (rope.rs:47-80)
 };
+// MkPhase is 512 bytes: the persistent kernels keep ten copies of it in shared memory, so its size moves the weight ring's fit
 // Attention phase of the megakernels split over `split` CTAs per head: CTA c scores its own range of the head's positions and
 // accumulates PV for its hd / split output dimensions; the score rows meet in MegaLaunch::scores ([n_heads][max_len + 1] f32).  Head h's CTAs count their arrivals in
 // word AT_ARRIVE_WORD + 8 h of the grid-barrier block (4096 bytes), AT_SPLIT_MAX per phase whatever the split.
@@ -323,6 +323,7 @@ struct MegaLaunch {                 // launch description of one phase table (la
     size_t smem = 1024, wstage = 0;  // working area (largest phase) ; norm-weight stage on top of it (largest n * 4 of a fused-norm phase)
     int slot_bytes = 0, nslots = 0, at_ch = 64;  // MEGA_RING: weight-ring slot size and count (cc_mega_ring_slots), attention chunk
     bool generic = false, sample = false;        // the instantiation that carries the generic (K-quant) MATVEC phase / the sampler's call
+    bool qwen2 = false;                          // ... Neox attention phases and per-matrix epilogue vectors (MEGA_RING only)
     float* scores = nullptr;                     // the attention phase's score rows (AttnArgs::split > 1)
 };
 int cc_launch_mega(cc_device* dev, const MkPhase* phases_dev, int n_phases, const uint8_t* dyn_dev, unsigned* bar_dev, const MegaLaunch& L,
@@ -337,7 +338,7 @@ int cc_launch_mega_ring(cc_device* dev, const MkPhase* phases_dev, int n_phases,
                         unsigned long long* prof, const CommDev* comm);
 int cc_check_async_error(cc_device* dev);     // after a stream synchronize: did a persistent kernel give up on a barrier?
 int cc_launch_normq(cc_device* dev, float* x, float* orig, const float* norm_w, float eps, int64_t n, void* act_scratch, bool write_back);
-int cc_launch_attn_decode(cc_device* dev, const AttnArgs& a);
+int cc_launch_attn_decode(cc_device* dev, const AttnArgs& a, const int64_t* dyn /* {pos, kv_len} */, const float* rope_tab /* cos[pairs], sin[pairs] */);
 bool cc_attn_decode_fits(int64_t hd, int64_t max_len);      // can the single-pass attention kernel hold the score row of this cache?
 struct LazyState;
 LazyState* cc_lazy_create(cc_device* dev);
@@ -357,6 +358,9 @@ int cc_launch_rms_norm_exact(cc_device* dev, float* x, int64_t rows, int64_t col
 int cc_launch_softmax_exact(cc_device* dev, float* x, int64_t rows, int64_t cols);
 int cc_launch_rope_exact(cc_device* dev, float* x, int64_t n_batch, int64_t batch_stride, int64_t head_dim, int mode,
                          int64_t pos, int64_t rope_dim);
+// the cos / sin of the `pairs` rotation angles of one position, on the host with the reference's libm calls (rope.rs:47-80); read by the
+// eager rope kernel and by the fused attention of both lazy modes
+void cc_rope_table(int mode, int64_t pos, int64_t head_dim, int pairs, float* cos_out, float* sin_out);
 int cc_launch_bmm_kcontig_exact(cc_device* dev, const float* a, const void* b, int b_dtype, float* c, int64_t ab, int64_t bb,
                                 int64_t m, int64_t k, int64_t n, int64_t sb0, int64_t sb2);
 

@@ -308,6 +308,22 @@ int cc_launch_softmax_exact(cc_device* dev, float* x, int64_t rows, int64_t cols
 }
 
 // rope with HOST-evaluated cos/sin (glibc cosf/sinf, exactly what the reference calls): rope.rs:47-80
+// The base is 10000 in both modes, whatever a model file says (rope.rs:48,69 hard-code it; a GGUF `rope.freq_base` is not read):
+// llama: theta_j = pos * scale^j by the running product (rope.rs:48-53); neox: theta_j = pos / 10000^(2j / head_dim), one powf per j
+// (rope.rs:66-79).
+void cc_rope_table(int mode, int64_t pos, int64_t head_dim, int pairs, float* cos_out, float* sin_out) {
+    const float fpos = (float)pos;
+    if (mode == CC_ROPE_LLAMA) {
+        float theta_scale = powf(10000.0f, -2.0f / (float)head_dim), theta = fpos;
+        for (int j = 0; j < pairs; j++) { cos_out[j] = cosf(theta); sin_out[j] = sinf(theta); theta *= theta_scale; }
+    } else {
+        for (int j = 0; j < pairs; j++) {
+            float timescale = powf(10000.0f, 2.0f * (float)j / (float)head_dim);
+            float theta = fpos / timescale;
+            cos_out[j] = cosf(theta); sin_out[j] = sinf(theta);
+        }
+    }
+}
 struct RopeTable { float c[128], s[128]; };
 __global__ void rope_table_kernel(float* row, int64_t heads, int head_dim, int mode, int pairs, RopeTable tb) {
     int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -327,17 +343,7 @@ int cc_launch_rope_exact(cc_device* dev, float* x, int64_t n_batch, int64_t batc
     int64_t heads = batch_stride / head_dim;
     for (int64_t bi = 0; bi < n_batch; bi++) {
         RopeTable tb;
-        float fpos = (float)(pos + bi);
-        if (mode == CC_ROPE_LLAMA) {
-            float theta_scale = powf(10000.0f, -2.0f / (float)head_dim), theta = fpos;
-            for (int j = 0; j < pairs; j++) { tb.c[j] = cosf(theta); tb.s[j] = sinf(theta); theta *= theta_scale; }
-        } else {
-            for (int j = 0; j < pairs; j++) {
-                float timescale = powf(10000.0f, 2.0f * (float)j / (float)head_dim);
-                float theta = fpos / timescale;
-                tb.c[j] = cosf(theta); tb.s[j] = sinf(theta);
-            }
-        }
+        cc_rope_table(mode, pos + bi, head_dim, pairs, tb.c, tb.s);
         int64_t total = heads * pairs;
         rope_table_kernel<<<(unsigned)((total + 127) / 128), 128, 0, dev->stream>>>(x + bi * batch_stride, heads, (int)head_dim, mode, pairs, tb);
         CC_LAUNCH_CHECK(dev);

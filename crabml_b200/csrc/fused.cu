@@ -56,7 +56,7 @@ __global__ void __launch_bounds__(NQ_THREADS) normq_kernel(float* x, float* orig
 
 // ---------------------------------------------------------------------------------------------------------------
 // attn_decode: one CTA per query head, n_batch = 1.  Replaces (llama2.rs:252-256, 541-590):
-//   rope_inplace(q), rope_inplace(k)            rope.rs:47-63, cos/sin table evaluated on the host (same libm calls)
+//   rope_inplace(q), rope_inplace(k)            rope.rs:47-80 (llama or neox pairs), cos/sin table evaluated on the host (cc_rope_table)
 //   k_cache.concatenate(k), v_cache.concatenate(v)   concatenate.rs (F32 or F16 cache, f16::from_f32 on append)
 //   q.contiguous().scale_inplace(1/sqrt(hd))
 //   attn = q.batch_matmul(k_cache^T); softmax_inplace; out = attn.batch_matmul(v_cache)
@@ -66,7 +66,7 @@ __global__ void __launch_bounds__(NQ_THREADS) normq_kernel(float* x, float* orig
 // dyn: {pos, kv_len}; rope_tab: cos[pairs] then sin[pairs].
 // ---------------------------------------------------------------------------------------------------------------
 #define AT_THREADS CC_RED_THREADS            // canonical softmax order (common.cuh); also 16 score warps per head
-template <bool KV_F16>
+template <bool KV_F16, bool NEOX>
 __global__ void __launch_bounds__(AT_THREADS) attn_decode_kernel(const float* __restrict__ q_in, const float* __restrict__ k_in, const float* __restrict__ v_in,
                                                                  void* kcache, void* vcache, float* __restrict__ out, ActQ8_0 act,
                                                                  const int64_t* __restrict__ dyn, const float* __restrict__ rope_tab,
@@ -85,16 +85,21 @@ __global__ void __launch_bounds__(AT_THREADS) attn_decode_kernel(const float* __
     float* s_p = sm + 3 * hd;                       // [L] scores
     __shared__ float s_red[AT_THREADS / 32];
     const int pairs = rope_dim >> 1;
-    // rope (llama mode: pairs (2j, 2j+1)); q additionally scaled AFTER the rotation (scale_inplace, llama2.rs:565)
+    // rope, q additionally scaled AFTER the rotation (scale_inplace, llama2.rs:565); pairs as exact.cu rope_table_kernel (rope.rs:47-80):
+    //   llama: (2j, 2j+1) for j < rope_dim/2
+    //   neox: (j, j + hd/2) for j < rope_dim/2 -- half the HEAD dim even when rope_dim < hd, the reference's pairing
+    const int half = hd >> 1;
     for (int i = threadIdx.x; i < hd; i += AT_THREADS) {
         float qv, kvv;
-        if (i < rope_dim) {
-            const int j = i >> 1;
+        const bool second = NEOX ? i >= half : (i & 1);
+        const int j = NEOX ? (second ? i - half : i) : i >> 1;
+        if (j < pairs) {
+            const int lo = NEOX ? j : 2 * j, hi = NEOX ? j + half : 2 * j + 1;
             const float c = rope_tab[j], s = rope_tab[pairs + j];
-            const float q0 = q_in[h * hd + 2 * j], q1 = q_in[h * hd + 2 * j + 1];
-            const float k0 = k_in[g * hd + 2 * j], k1 = k_in[g * hd + 2 * j + 1];
-            qv = (i & 1) ? q0 * s + q1 * c : q0 * c - q1 * s;
-            kvv = (i & 1) ? k0 * s + k1 * c : k0 * c - k1 * s;
+            const float q0 = q_in[h * hd + lo], q1 = q_in[h * hd + hi];
+            const float k0 = k_in[g * hd + lo], k1 = k_in[g * hd + hi];
+            qv = second ? q0 * s + q1 * c : q0 * c - q1 * s;
+            kvv = second ? k0 * s + k1 * c : k0 * c - k1 * s;
         } else {
             qv = q_in[h * hd + i];
             kvv = k_in[g * hd + i];
@@ -229,21 +234,20 @@ int cc_launch_normq(cc_device* dev, float* x, float* orig, const float* norm_w, 
 static size_t attn_decode_smem(int64_t hd, int64_t max_len) { return (size_t)(3 * hd + max_len + 8) * sizeof(float); }
 bool cc_attn_decode_fits(int64_t hd, int64_t max_len) { return attn_decode_smem(hd, max_len) <= AT_SMEM_MAX; }
 
-int cc_launch_attn_decode(cc_device* dev, const AttnArgs& a) {
+template <bool KV_F16, bool NEOX>
+static cudaError_t launch_attn(cc_device* dev, const AttnArgs& a, ActQ8_0 act, const int64_t* dyn, const float* rope_tab, size_t smem) {
+    if (smem > 48 * 1024) cudaFuncSetAttribute(attn_decode_kernel<KV_F16, NEOX>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    return launch_pdl(attn_decode_kernel<KV_F16, NEOX>, dim3(a.n_heads), dim3(AT_THREADS), smem, dev->stream, dev->pdl, a.q, a.k, a.v, a.kcache, a.vcache, a.out, act,
+                      dyn, rope_tab, (const uint16_t*)dev->exp_lut, a.n_heads, a.n_kv, a.hd, a.rope_dim, a.seq_stride, a.scale);
+}
+
+int cc_launch_attn_decode(cc_device* dev, const AttnArgs& a, const int64_t* dyn, const float* rope_tab) {
     const size_t smem = attn_decode_smem(a.hd, a.max_len);
     CC_REQUIRE(dev, smem <= AT_SMEM_MAX, "attention: context %d too long for the single-pass kernel", a.max_len);
     ActQ8_0 act = cc_act_q8_0(a.act_scratch, (int64_t)a.n_heads * a.hd);
     if (!a.act_scratch) act.qs = nullptr;
-    cudaError_t e;
-    if (a.kv_f16) {
-        if (smem > 48 * 1024) cudaFuncSetAttribute(attn_decode_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        e = launch_pdl(attn_decode_kernel<true>, dim3(a.n_heads), dim3(AT_THREADS), smem, dev->stream, dev->pdl, a.q, a.k, a.v, a.kcache, a.vcache, a.out, act,
-                       a.dyn, a.rope_tab, (const uint16_t*)dev->exp_lut, a.n_heads, a.n_kv, a.hd, a.rope_dim, a.seq_stride, a.scale);
-    } else {
-        if (smem > 48 * 1024) cudaFuncSetAttribute(attn_decode_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        e = launch_pdl(attn_decode_kernel<false>, dim3(a.n_heads), dim3(AT_THREADS), smem, dev->stream, dev->pdl, a.q, a.k, a.v, a.kcache, a.vcache, a.out, act,
-                       a.dyn, a.rope_tab, (const uint16_t*)dev->exp_lut, a.n_heads, a.n_kv, a.hd, a.rope_dim, a.seq_stride, a.scale);
-    }
+    const cudaError_t e = a.kv_f16 ? (a.rope_neox ? launch_attn<true, true>(dev, a, act, dyn, rope_tab, smem) : launch_attn<true, false>(dev, a, act, dyn, rope_tab, smem))
+                                   : (a.rope_neox ? launch_attn<false, true>(dev, a, act, dyn, rope_tab, smem) : launch_attn<false, false>(dev, a, act, dyn, rope_tab, smem));
     if (e != cudaSuccess) return cc_fail(dev, CC_ERR_CUDA, "attention launch: %s", cudaGetErrorString(e));
     dev->launches++;
     return CC_OK;

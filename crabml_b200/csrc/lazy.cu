@@ -174,7 +174,7 @@ struct Fuser {
     LazyState* lz;
     std::vector<LOp>& q;
     Plan& P;
-    size_t rope_off = (size_t)-1; int64_t rope_pos = -1; int rope_hd = 0, rope_dim = 0;
+    size_t rope_off = (size_t)-1; int64_t rope_pos = -1; int rope_hd = 0, rope_dim = 0, rope_mode = -1;
 
     bool is(size_t i, int kind) const { return i < q.size() && !q[i].done && q[i].kind == kind; }
     std::unordered_map<cc_buf*, size_t> last_use;      // buffer -> index of the last queued op that touches it (built once per flush)
@@ -292,20 +292,29 @@ struct Fuser {
         return mv.b.buf == x && cc_stream_supported(mv.a.buf->dtype, mv.a.shape[1]) && vlen(mv.b) == mv.a.shape[1] && vcontig(mv.b);
     }
     // the MATVEC at j (weight type wt, k columns) and up to two more of the same type and k on row x, with the epilogue that follows:
-    // gate/up + silu + mul (llama2.rs:620-630) or x = matvec + residual (llama2.rs:266,636).  n matrices, `used` ops consumed.
-    struct GroupMatch { size_t n = 1, used = 1; int epilogue = 0; cc_buf* residual = nullptr; };
+    // gate/up + silu + mul (llama2.rs:620-630), or one ADD of an f32 vector per matrix, in matrix order: x = matvec + residual
+    // (llama2.rs:266,636) and qwen2's q/k/v biases (llama2.rs:315-317).  n matrices, `used` ops consumed.
+    struct GroupMatch { size_t n = 1, used = 1; int epilogue = 0; cc_buf* residual[3] = {nullptr, nullptr, nullptr}; };
+    // the ADD at `at` adds a whole contiguous f32 vector to the output of the MATVEC at t
+    bool adds_vector(size_t at, size_t t) const {
+        if (!is(at, L_ADD)) return false;
+        const LOp &mv = q[t], &ad = q[at];
+        return ad.a.buf == mv.out && vlen(ad.b) == mv.a.shape[0] && covers(ad, mv.a.shape[0]) && ad.b.buf->dtype == CC_F32 && vcontig(ad.b);
+    }
     GroupMatch match_group(size_t j, const cc_buf* x, int wt, int64_t k) const {
         GroupMatch g;
         while (g.n < 3 && is(j + g.n, L_MATVEC) && q[j + g.n].b.buf == x && q[j + g.n].a.buf->dtype == wt && q[j + g.n].a.shape[1] == k &&
                vlen(q[j + g.n].b) == k) g.n++;
         g.used = g.n;
         const LOp& m0 = q[j];
+        bool adds = true;
+        for (size_t t = 0; t < g.n; t++) adds = adds && adds_vector(j + g.n + t, j + t);
         if (g.n >= 2 && is(j + 2, L_SILU) && is(j + 3, L_MUL) && q[j + 2].a.buf == m0.out && q[j + 3].a.buf == m0.out && q[j + 3].b.buf == q[j + 1].out &&
             m0.a.shape[0] == q[j + 1].a.shape[0] && vlen(q[j + 3].b) == m0.a.shape[0] && covers(q[j + 3], m0.a.shape[0]) && dead_after(q[j + 1].out, j + 4)) {
             g.n = 2; g.epilogue = 2; g.used = 4;
-        } else if (g.n == 1 && is(j + 1, L_ADD) && q[j + 1].a.buf == m0.out && vlen(q[j + 1].b) == m0.a.shape[0] && covers(q[j + 1], m0.a.shape[0]) &&
-                   q[j + 1].b.buf->dtype == CC_F32 && vcontig(q[j + 1].b)) {
-            g.epilogue = 1; g.residual = q[j + 1].b.buf; g.used = 2;
+        } else if (adds) {
+            g.epilogue = 1; g.used = 2 * g.n;
+            for (size_t t = 0; t < g.n; t++) g.residual[t] = q[j + g.n + t].b.buf;
         } else if (g.n > 1 && is(j + g.n, L_SILU)) {
             g.n = 1; g.used = 1;                   // do not swallow a gate/up pair we could not fuse as a pair
         }
@@ -347,8 +356,8 @@ struct Fuser {
         const GroupMatch g = match_group(i, xbuf, wt, k);
         size_t n = g.n, used = g.used;
         StreamArgs A = {};
-        A.k = (int)k; A.exp_lut = dev->exp_lut; A.epilogue = g.epilogue;
-        A.residual = g.residual ? (const float*)g.residual->plane[0] : nullptr;
+        A.k = (int)k; A.epilogue = g.epilogue;
+        for (int t = 0; t < 3; t++) A.residual[t] = g.residual[t] ? (const float*)g.residual[t]->plane[0] : nullptr;
         // sharded path: column-split matvec -> allreduce [-> + residual]  /  row-split classifier -> allgather (comm.cu)
         int xchg = 0; float* xdst = nullptr; const float* xres = nullptr;
         if (A.epilogue == 0 && is(i + 1, L_ALLREDUCE) && q[i + 1].a.buf == m0.out && q[i + 1].i0 == m0.a.shape[0]) {
@@ -377,7 +386,7 @@ struct Fuser {
             P.steps.push_back([=](uint8_t*) { return cc_launch_normq(d, x, nullptr, nullptr, 0.0f, k, act, false); });
             { MkPhase ph = {}; ph.type = MK_NORMQ; ph.x = x; ph.n = (int)k; ph.act = cc_act_q8_0(act, k); P.phases.push_back(ph); }
         }
-        P.S(0x2003); P.S(wt); P.S(k); P.S(A.epilogue); P.SP(A.residual); P.SP(act);
+        P.S(0x2003); P.S(wt); P.S(k); P.S(A.epilogue); P.SP(A.residual[0]); P.SP(A.residual[1]); P.SP(A.residual[2]); P.SP(act);
         for (size_t t = 0; t < n; t++) { P.SP(A.mats.qs[t]); P.SP(A.mats.out[t]); P.S(A.mats.m[t]); }
         P.steps.push_back([=](uint8_t*) { return cc_launch_matvec_stream(d, wt, A); });
         { MkPhase ph = {}; ph.type = MK_MATVEC; ph.wtype = wt; ph.mv = A; if (xchg) { ph.mv.epilogue = 3; ph.xgpu = 1; }
@@ -396,14 +405,15 @@ struct Fuser {
         return used;
     }
 
-    // ---- pattern: rope q,k + kv append + attention (llama2.rs:252-256, 541-590), n_batch == 1 -----------------------------------------------
+    // ---- pattern: rope q,k (llama or neox) + kv append + attention (llama2.rs:252-256, 541-590), n_batch == 1 -----------------------------------------------
     size_t try_attention(size_t i, cc_buf** obuf, bool* quantized) {
         if (!(is(i, L_ROPE) && is(i + 1, L_ROPE) && is(i + 2, L_CONCAT) && is(i + 3, L_CONCAT) && is(i + 4, L_CONTIGUOUS) && is(i + 5, L_SCALE) &&
               is(i + 6, L_BMM) && is(i + 7, L_SOFTMAX) && is(i + 8, L_BMM))) return 0;
         const LOp &rq = q[i], &rk = q[i + 1], &ck = q[i + 2], &cv = q[i + 3], &ct = q[i + 4], &sc = q[i + 5], &b1 = q[i + 6], &sm = q[i + 7], &b2 = q[i + 8];
         if (rq.a.ndim != 3 || rk.a.ndim != 3 || rq.a.shape[0] != 1 || rk.a.shape[0] != 1) return 0;
         const int64_t n_heads = rq.a.shape[1], hd = rq.a.shape[2], n_kv = rk.a.shape[1];
-        if (rk.a.shape[2] != hd || (int)rq.f != CC_ROPE_LLAMA || (int)rk.f != CC_ROPE_LLAMA || rq.i0 != rk.i0 || rq.rows[0] != rk.rows[0]) return 0;
+        const int mode = (int)rq.f;
+        if (rk.a.shape[2] != hd || (mode != CC_ROPE_LLAMA && mode != CC_ROPE_NEOX) || (int)rk.f != mode || rq.i0 != rk.i0 || rq.rows[0] != rk.rows[0]) return 0;
         if (hd > 256 || n_heads % n_kv) return 0;
         *quantized = hd % 32 == 0;
         cc_buf *qb = rq.a.buf, *kb = rk.a.buf, *kc = ck.a.buf, *vc = cv.a.buf, *vb = cv.b.buf;
@@ -425,14 +435,13 @@ struct Fuser {
         if (!dead_after(ct.out, i + 9) || !dead_after(b1.out, i + 9) || !dead_after(qb, i + 9) || !dead_after(kb, i + 9) || !dead_after(vb, i + 9)) return 0;
         const int64_t pos = rq.i0, rope_dim = rq.rows[0];
         if (rope_dim > hd || rope_dim % 2) return 0;
-        // RoPE table: host libm, identical calls to the reference (rope.rs:47-63); shared by all layers of this flush
-        if (rope_off == (size_t)-1 || rope_pos != pos || rope_hd != hd || this->rope_dim != rope_dim) {
+        // RoPE table: host libm, identical calls to the reference and the eager kernel (cc_rope_table); shared by all layers of this flush
+        if (rope_off == (size_t)-1 || rope_pos != pos || rope_hd != hd || this->rope_dim != rope_dim || rope_mode != mode) {
             std::vector<float> tab((size_t)rope_dim);
             const int pairs = (int)rope_dim / 2;
-            float theta_scale = powf(10000.0f, -2.0f / (float)hd), theta = (float)pos;
-            for (int j = 0; j < pairs; j++) { tab[j] = cosf(theta); tab[pairs + j] = sinf(theta); theta *= theta_scale; }
+            cc_rope_table(mode, pos, hd, pairs, tab.data(), tab.data() + pairs);
             rope_off = P.dyn_put(tab.data(), tab.size() * 4);
-            rope_pos = pos; rope_hd = (int)hd; this->rope_dim = (int)rope_dim;
+            rope_pos = pos; rope_hd = (int)hd; this->rope_dim = (int)rope_dim; rope_mode = mode;
         }
         int64_t dynv[2] = {pos, kv_len};
         size_t dyn_off = P.dyn_put(dynv, sizeof(dynv));
@@ -443,6 +452,7 @@ struct Fuser {
         if (*quantized && is(i + 9, L_MATVEC) && !cc_stream_supported(q[i + 9].a.buf->dtype, q[i + 9].a.shape[1])) *quantized = false;   // K-quant wo quantises (Q8_K) itself
         A.act_scratch = *quantized ? lz->act[1] : nullptr;
         A.n_heads = (int)n_heads; A.n_kv = (int)n_kv; A.hd = (int)hd; A.rope_dim = (int)rope_dim;
+        A.rope_neox = mode == CC_ROPE_NEOX;
         A.max_len = (int)(seq_stride / hd); A.kv_f16 = kc->dtype == CC_F16;
         A.seq_stride = seq_stride; A.scale = sc.f;
         // the most CTAs per head the score scratch allows; the persistent kernel's split is chosen with its grid (choose_mega)
@@ -450,12 +460,9 @@ struct Fuser {
         cc_device* d = dev;
         size_t roff = rope_off;
         P.S(0x2004); P.SP(A.q); P.SP(A.k); P.SP(A.v); P.SP(A.kcache); P.SP(A.vcache); P.SP(A.out); P.SP(A.act_scratch); P.S(A.split); P.SP(lz->scores);
-        P.S(n_heads); P.S(n_kv); P.S(hd); P.S(rope_dim); P.S(seq_stride); P.S(A.kv_f16); uint32_t sb; memcpy(&sb, &A.scale, 4); P.S(sb); P.S(dyn_off); P.S(roff);
+        P.S(n_heads); P.S(n_kv); P.S(hd); P.S(rope_dim); P.S(A.rope_neox); P.S(seq_stride); P.S(A.kv_f16); uint32_t sb; memcpy(&sb, &A.scale, 4); P.S(sb); P.S(dyn_off); P.S(roff);
         P.steps.push_back([=](uint8_t* dyn_dev) {
-            AttnArgs B = A;
-            B.dyn = (const int64_t*)(dyn_dev + dyn_off);
-            B.rope_tab = (const float*)(dyn_dev + roff);
-            return cc_launch_attn_decode(d, B);
+            return cc_launch_attn_decode(d, A, (const int64_t*)(dyn_dev + dyn_off), (const float*)(dyn_dev + roff));
         });
         { MkPhase ph = {}; ph.type = MK_ATTN; ph.at = A; ph.dyn_off = dyn_off; ph.rope_off = roff; ph.act = cc_act_q8_0(lz->act[1], n_heads * hd);
           P.phases.push_back(ph); }
@@ -543,14 +550,15 @@ struct Fuser {
         if (m0.b.buf != xb || xb->dtype != CC_F32 || vlen(m0.b) != k || !vcontig(m0.b) || (m0.b.ndim == 2 && m0.b.shape[0] != 1) || m0.b.ndim > 2) return 0;
         GroupMatch g = match_group(j, xb, wt, k);
         // the generic phase never writes a normalised row back (below), so a residual that is x itself would read the wrong row;
-        // the residual add then runs as its own op, with or without a norm
-        if (g.epilogue == 1 && g.residual == xb) g = GroupMatch();
+        // the residual add then runs as its own op, with or without a norm.  Its epilogue adds one vector to one matrix: the bias adds
+        // of a q/k/v group run as their own ops too (and keep the table out of the persistent kernels)
+        if (g.epilogue == 1 && (g.residual[0] == xb || g.n > 1)) { const size_t n = g.n; g = GroupMatch(); g.n = g.used = n; }
         if (is(j + g.used, L_ALLREDUCE) || is(j + g.used, L_ALLGATHER)) return 0;      // sharded K-quant models run in the CUDA-graph mode
         const size_t end = j + g.used;
         // the normalised row is overwritten in place by the eager ops; the fused prologue never materialises it: nobody else may read it
         if (nm.len && !dead_after(xb, end)) return 0;
         StreamArgs A = {};
-        A.k = (int)k; A.exp_lut = dev->exp_lut; A.epilogue = g.epilogue; A.residual = g.residual ? (const float*)g.residual->plane[0] : nullptr;
+        A.k = (int)k; A.epilogue = g.epilogue; A.residual[0] = g.residual[0] ? (const float*)g.residual[0]->plane[0] : nullptr;
         A.mats.n = (int)g.n;
         for (size_t t = 0; t < g.n; t++) {
             const cc_buf* w = q[j + t].a.buf;
@@ -642,11 +650,13 @@ static MegaLaunch choose_mega(const cc_device* dev, bool mega_ok, std::vector<Mk
         if (ph.type == MK_MATVEC) (ph.act_type == CC_Q8_K ? L.generic : stream) = true;
         if (!cc_mega_ring_phase_ok(ph)) ring_ok = false;
         n_sample += ph.type == MK_SAMPLE;
+        if ((ph.type == MK_ATTN && ph.at.rope_neox) || (ph.type == MK_MATVEC && ph.mv.epilogue == 1 && ph.mv.mats.n > 1)) L.qwen2 = true;
     }
     // the megakernel runs ONE SAMPLE phase, after its phase loop (mega.cu): a table with more than one, or with anything queued
     // behind the sampler (several tokens submitted before one flush), runs in the CUDA-graph mode
     L.sample = n_sample > 0;
     if (n_sample > 1 || (n_sample == 1 && phs.back().type != MK_SAMPLE)) return L;
+    if (L.qwen2 && !stream) return L;          // qwen2 phases are in the ring kernel only (mega_ring.cu QWEN2)
     for (auto& ph : phs) {
         L.smem = std::max(L.smem, stream ? cc_mega_ring_smem_for_phase(ph) : cc_mega_smem_for_phase(ph));
         if (ph.type == MK_MATVEC && ph.x && ph.norm_w) L.wstage = std::max(L.wstage, (size_t)ph.n * 4);

@@ -14,7 +14,8 @@
 //         lane-relative immediates.  The first segment is requested BEFORE the activation is staged.
 //   * the quantised activation (Q8_0 blocks as SoA: qs | f32 scale | block sums) is copied global -> shared once per CTA;
 //   * up to 3 matrices that share the activation (wq,wk,wv / gate,up) run as one launch;
-//   * epilogues: store | + residual (llama2.rs:266,636) | silu(gate) * up (llama2.rs:620-630).
+//   * epilogues: store | + one f32 vector per matrix: the residual (llama2.rs:266,636) or qwen2's q/k/v biases
+//     (llama2.rs:315-317) | silu(gate) * up (llama2.rs:620-630).
 // Q8_0 device layout: inside each group of 32 blocks the 16-byte first halves of all blocks precede the second
 // halves, so lane l reads block 32g+l with two fully coalesced LDG.128 (512 B per warp request).
 #include "common.cuh"
@@ -91,7 +92,7 @@ __device__ __forceinline__ float seg_dot(const Seg<TYPE>& S, int seg, const int4
 }
 
 template <int TYPE>
-__global__ void __launch_bounds__(MS_THREADS, MS_CTAS_PER_SM) matvec_stream_kernel(StreamArgs A) {
+__global__ void __launch_bounds__(MS_THREADS, MS_CTAS_PER_SM) matvec_stream_kernel(StreamArgs A, const uint16_t* __restrict__ exp_lut) {
     extern __shared__ __align__(16) uint8_t smem[];
     const int k = A.k, nb = k >> 5, GR = (nb + 31) >> 5, NSEG = (GR + MS_SEG - 1) / MS_SEG;
     const int nbp = NSEG * MS_SEG * 32;                           // padded block count
@@ -163,7 +164,7 @@ __global__ void __launch_bounds__(MS_THREADS, MS_CTAS_PER_SM) matvec_stream_kern
             if ((i & 1) == 0) { first = r; return; }
             if (lane == 0) {                                       // silu.rs:6-13 then mul (llama2.rs:625-630)
                 float g = first;
-                float nexp = h2f_bits(A.exp_lut[f2h_bits(-g)]);
+                float nexp = h2f_bits(exp_lut[f2h_bits(-g)]);
                 M.out[0][gw + (i >> 1) * TW] = (g / (1.0f + nexp)) * r;
             }
             return;
@@ -171,7 +172,7 @@ __global__ void __launch_bounds__(MS_THREADS, MS_CTAS_PER_SM) matvec_stream_kern
         if (lane == 0) {
             int mat = 0, rr = gw + i * TW;
             if (M.n > 1 && rr >= M.m[0]) { rr -= M.m[0]; mat = 1; if (M.n > 2 && rr >= M.m[1]) { rr -= M.m[1]; mat = 2; } }
-            if (A.epilogue == 1) r = r + A.residual[rr];
+            if (A.epilogue == 1) r = r + (mat == 0 ? A.residual[0] : mat == 1 ? A.residual[1] : A.residual[2])[rr];
             float* o = mat == 0 ? M.out[0] : mat == 1 ? M.out[1] : M.out[2];
             o[rr] = r;
         }
@@ -215,10 +216,10 @@ int cc_launch_matvec_stream(cc_device* dev, int type, const StreamArgs& A) {
     cudaError_t e;
     if (type == CC_Q8_0) {
         if (smem > 48 * 1024) CC_CUDA(dev, cudaFuncSetAttribute(matvec_stream_kernel<CC_Q8_0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        e = cudaLaunchKernelEx(&cfg, matvec_stream_kernel<CC_Q8_0>, A);
+        e = cudaLaunchKernelEx(&cfg, matvec_stream_kernel<CC_Q8_0>, A, (const uint16_t*)dev->exp_lut);
     } else {
         if (smem > 48 * 1024) CC_CUDA(dev, cudaFuncSetAttribute(matvec_stream_kernel<CC_Q4_0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        e = cudaLaunchKernelEx(&cfg, matvec_stream_kernel<CC_Q4_0>, A);
+        e = cudaLaunchKernelEx(&cfg, matvec_stream_kernel<CC_Q4_0>, A, (const uint16_t*)dev->exp_lut);
     }
     if (e != cudaSuccess) return cc_fail(dev, CC_ERR_CUDA, "matvec_stream launch: %s", cudaGetErrorString(e));
     dev->launches++;
@@ -235,6 +236,5 @@ int cc_launch_matvec_stream_plain(cc_device* dev, const cc_buf* w, const void* a
     A.mats.m[0] = (int)m;
     A.act = act;
     A.k = (int)k;
-    A.exp_lut = dev->exp_lut;
     return cc_launch_matvec_stream(dev, w->dtype, A);
 }

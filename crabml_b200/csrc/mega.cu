@@ -88,8 +88,8 @@ __global__ void __launch_bounds__(MK_THREADS, MK_CTAS_PER_SM) mega_kernel(const 
             break;
         }
         case MK_ATTN:
-            if (s_ph.at.kv_f16) phase_attn<true>(s_ph, (float*)work, s_red, dyn, exp_lut, abar0, apar, AT_CH, bar, err_host, &s_abort, scores);
-            else phase_attn<false>(s_ph, (float*)work, s_red, dyn, exp_lut, abar0, apar, AT_CH, bar, err_host, &s_abort, scores);
+            if (s_ph.at.kv_f16) phase_attn<true, false>(s_ph, (float*)work, s_red, dyn, exp_lut, abar0, apar, AT_CH, bar, err_host, &s_abort, scores);
+            else phase_attn<false, false>(s_ph, (float*)work, s_red, dyn, exp_lut, abar0, apar, AT_CH, bar, err_host, &s_abort, scores);
             break;
         case MK_ROWS: phase_rows(s_ph, dyn); break;
         case MK_ARGMAX: phase_argmax(s_ph, dyn, s_red); break;

@@ -282,7 +282,7 @@ static __device__ MK_GENERIC_ATTR void phase_matvec_generic(const MkPhase& ph, u
             if (lane == 0) { pend_a = first; pend_b = v; pend_row = r; pend_lut = exp_lut[f2h_bits(-first)]; }
         } else if (A.epilogue == 1) {
             flush_pending();
-            if (lane == 0) { pend_a = v; pend_row = r; pend_res = ldcg_f(A.residual + r); }
+            if (lane == 0) { pend_a = v; pend_row = r; pend_res = ldcg_f(A.residual[0] + r); }      // one matrix: lazy.cu keeps per-matrix vectors out of this phase
         } else if (lane == 0) {
             float* o = mat == 0 ? M.out[0] : mat == 1 ? M.out[1] : M.out[2];
             o[r] = v;
@@ -343,7 +343,7 @@ __device__ __forceinline__ unsigned atom_add_release(unsigned* p, unsigned v) {
 // CTA c then accumulates PV for the dimensions [c hd / S, (c + 1) hd / S), sequentially over s, and quantises those hd / (32 S) Q8_0
 // blocks of the output.  Each score is an independent dot product and each output element's PV sum keeps its order, so the bits do not
 // depend on S.
-template <bool KV_F16, bool SPLIT>
+template <bool KV_F16, bool SPLIT, bool NEOX>
 static __device__ void phase_attn_heads(const MkPhase& ph, float* sm, float* s_red, const uint8_t* dyn, const uint16_t* exp_lut, unsigned abar0, unsigned& apar, const int at_ch,
                                         unsigned* bar, unsigned* err_host, int* s_abort, float* scores) {
     const AttnArgs& a = ph.at;
@@ -415,7 +415,21 @@ static __device__ void phase_attn_heads(const MkPhase& ph, float* sm, float* s_r
         if (issuer) for (int j = 0; j < min(AT_NBUF, NJ); j++) issue_job(j);
         for (int i = threadIdx.x; i < hd; i += MK_THREADS) {
             float qv, kvv;
-            if (i < rope_dim) {
+            if (NEOX) {                                              // pairs (j, j + hd/2), j < rope_dim/2 (fused.cu attn_decode_kernel)
+                const int half = hd >> 1;
+                const bool second = i >= half;
+                const int j = second ? i - half : i;
+                if (j < pairs) {
+                    const float c = rope_tab[j], s = rope_tab[pairs + j];
+                    const float q0 = ldcg_f(a.q + h * hd + j), q1 = ldcg_f(a.q + h * hd + j + half);
+                    const float k0 = ldcg_f(a.k + g * hd + j), k1 = ldcg_f(a.k + g * hd + j + half);
+                    qv = second ? q0 * s + q1 * c : q0 * c - q1 * s;
+                    kvv = second ? k0 * s + k1 * c : k0 * c - k1 * s;
+                } else {
+                    qv = ldcg_f(a.q + h * hd + i);
+                    kvv = ldcg_f(a.k + g * hd + i);
+                }
+            } else if (i < rope_dim) {
                 const int j = i >> 1;
                 const float c = rope_tab[j], s = rope_tab[pairs + j];
                 const float q0 = ldcg_f(a.q + h * hd + 2 * j), q1 = ldcg_f(a.q + h * hd + 2 * j + 1);
@@ -558,20 +572,21 @@ static __device__ void phase_attn_heads(const MkPhase& ph, float* sm, float* s_r
 #else
 #define MK_ATTN_SPLIT_ATTR
 #endif
-template <bool KV_F16>
+template <bool KV_F16, bool NEOX>
 static __device__ MK_ATTN_SPLIT_ATTR void phase_attn_split(const MkPhase& ph, float* sm, float* s_red, const uint8_t* dyn, const uint16_t* exp_lut, unsigned abar0, unsigned& apar, const int at_ch,
                                         unsigned* bar, unsigned* err_host, int* s_abort, float* scores) {
-    phase_attn_heads<KV_F16, true>(ph, sm, s_red, dyn, exp_lut, abar0, apar, at_ch, bar, err_host, s_abort, scores);
+    phase_attn_heads<KV_F16, true, NEOX>(ph, sm, s_red, dyn, exp_lut, abar0, apar, at_ch, bar, err_host, s_abort, scores);
 }
 
 // below AT_SPLIT_MIN_KV cached positions the score exchange costs more than the split saves (Llama-2-7B, per layer, split against one
 // CTA per head: 10.4 / 8.8 us at ~60 positions, 14.3 / 12.9 at ~190, 22.3 / 23.1 at ~440, 70 / 88 at ~2040; NVIDIA H100 80GB HBM3,
 // 700 W): one CTA per head
-template <bool KV_F16>
+// NEOX: the qwen2 instantiations of the ring kernel (mega_ring.cu QWEN2), whose attention phases pair RoPE elements (j, j + hd/2)
+template <bool KV_F16, bool NEOX>
 static __device__ __forceinline__ void phase_attn(const MkPhase& ph, float* sm, float* s_red, const uint8_t* dyn, const uint16_t* exp_lut, unsigned abar0, unsigned& apar,
                                                   const int at_ch, unsigned* bar, unsigned* err_host, int* s_abort, float* scores) {
-    if (ph.at.split > 1 && ((const int64_t*)(dyn + ph.dyn_off))[1] >= AT_SPLIT_MIN_KV) phase_attn_split<KV_F16>(ph, sm, s_red, dyn, exp_lut, abar0, apar, at_ch, bar, err_host, s_abort, scores);
-    else phase_attn_heads<KV_F16, false>(ph, sm, s_red, dyn, exp_lut, abar0, apar, at_ch, bar, err_host, s_abort, scores);
+    if (ph.at.split > 1 && ((const int64_t*)(dyn + ph.dyn_off))[1] >= AT_SPLIT_MIN_KV) phase_attn_split<KV_F16, NEOX>(ph, sm, s_red, dyn, exp_lut, abar0, apar, at_ch, bar, err_host, s_abort, scores);
+    else phase_attn_heads<KV_F16, false, NEOX>(ph, sm, s_red, dyn, exp_lut, abar0, apar, at_ch, bar, err_host, s_abort, scores);
 }
 
 // ---- ROWS phase: copy_rows_from with the row indices in dyn (embedding lookup / row pick) -----------------------------------

@@ -271,7 +271,8 @@ __device__ __forceinline__ void mr_dot2(const uint8_t* spA, const uint8_t* spB, 
 // smem: the phase's working area (mr_x_off); s_wn: the norm-weight stage, holding the weights `wst` once this thread's cp.async groups
 // are complete (requested here when they are not ph.norm_w); x_staged: the input row was requested into the working area as the
 // barrier opened
-template <int TYPE>
+// QW: epilogue 1 adds the vector of the row's matrix (qwen2's q/k/v biases); otherwise it has one matrix (the residual add)
+template <int TYPE, bool QW>
 __device__ void phase_matvec_ring(const MkPhase& ph, uint8_t* smem, float* s_wn, const float*& wst, bool x_staged, const uint16_t* exp_lut, MrCons& RC,
                                   const CommDev& comm, unsigned xseq, unsigned long long* stamp1) {
     const StreamArgs& A = ph.mv;
@@ -418,7 +419,11 @@ __device__ void phase_matvec_ring(const MkPhase& ph, uint8_t* smem, float* s_wn,
         for (int t = 0; t < 2; t++) {
             if (lane == 0 && pend_row[t] >= 0) {
                 if (pair) M.out[0][pend_row[t]] = (pend_a[t] / (1.0f + h2f_bits(pend_lut[t]))) * pend_b[t];
-                else M.out[0][pend_row[t]] = pend_a[t] + pend_res[t];
+                else if (QW) {
+                    int mat;
+                    const int rr = mr_locate(M, g, pend_row[t], 0, mat);
+                    (mat == 0 ? M.out[0] : mat == 1 ? M.out[1] : M.out[2])[rr] = pend_a[t] + pend_res[t];
+                } else M.out[0][pend_row[t]] = pend_a[t] + pend_res[t];
             }
             pend_row[t] = -1;
         }
@@ -475,7 +480,12 @@ __device__ void phase_matvec_ring(const MkPhase& ph, uint8_t* smem, float* s_wn,
                 const int u = u0 + t, rc = g.first + u * g.stride;
                 if (lane != 0) continue;
                 if (pair) { pend_a[t] = first[t]; pend_b[t] = r; pend_row[t] = rc; pend_lut[t] = exp_lut[f2h_bits(-first[t])]; }      // silu(gate) * up
-                else if (A.epilogue == 1) { pend_a[t] = r; pend_row[t] = rc; pend_res[t] = ldcg_f(A.residual + rc); }              // + residual (llama2.rs:266,636)
+                else if (A.epilogue == 1 && QW) {                                                                                   // + bias of the row's matrix
+                    int mat;
+                    const int rr = mr_locate(M, g, rc, 0, mat);
+                    pend_a[t] = r; pend_row[t] = rc; pend_res[t] = ldcg_f((mat == 0 ? A.residual[0] : mat == 1 ? A.residual[1] : A.residual[2]) + rr);
+                }
+                else if (A.epilogue == 1) { pend_a[t] = r; pend_row[t] = rc; pend_res[t] = ldcg_f(A.residual[0] + rc); }           // + residual (llama2.rs:266,636)
                 else if (A.epilogue == 3) s_part[u] = r;                                                                            // partial row -> this CTA's exchange stage
                 else {
                     int mat;
@@ -500,7 +510,9 @@ __device__ void phase_matvec_ring(const MkPhase& ph, uint8_t* smem, float* s_wn,
     }
 }
 
-template <bool GEN, bool SMP>      // SMP: the table ends with its only SAMPLE phase (see mega.cu)
+// SMP: the table ends with its only SAMPLE phase (see mega.cu).  QWEN2: the table has qwen2 layers -- Neox RoPE in its attention phases,
+// one bias per matrix in its q/k/v phases -- a separate instantiation, so that the llama ones compile exactly as without qwen2
+template <bool GEN, bool SMP, bool QWEN2>
 __global__ void __launch_bounds__(MR_THREADS, 1) mega_ring_kernel(const MkPhase* __restrict__ phases, int n_phases, const uint8_t* dyn, unsigned* bar,
                                                                   const uint16_t* exp_lut, unsigned long long* prof, bool test_stall, int wtop_off, unsigned* err_host,
                                                                   const CommDev comm, const MrRing R, float* scores) {
@@ -572,12 +584,12 @@ __global__ void __launch_bounds__(MR_THREADS, 1) mega_ring_kernel(const MkPhase*
                 if (s_ph.x && s_ph.norm_w) { wst = s_ph.next_norm_w; if (wst) mr_stage_f32(s_wn, wst, s_ph.next_norm_n); }
                 break;
             }
-            if (s_ph.wtype == CC_Q8_0) phase_matvec_ring<CC_Q8_0>(s_ph, work, s_wn, wst, xstaged == p, exp_lut, RC, comm, xseq, st1);
-            else phase_matvec_ring<CC_Q4_0>(s_ph, work, s_wn, wst, xstaged == p, exp_lut, RC, comm, xseq, st1);
+            if (s_ph.wtype == CC_Q8_0) phase_matvec_ring<CC_Q8_0, QWEN2>(s_ph, work, s_wn, wst, xstaged == p, exp_lut, RC, comm, xseq, st1);
+            else phase_matvec_ring<CC_Q4_0, QWEN2>(s_ph, work, s_wn, wst, xstaged == p, exp_lut, RC, comm, xseq, st1);
             break;
         case MK_ATTN:
-            if (s_ph.at.kv_f16) phase_attn<true>(s_ph, (float*)work, s_red, dyn, exp_lut, abar0, apar, R.at_ch, bar, err_host, &s_abort, scores);
-            else phase_attn<false>(s_ph, (float*)work, s_red, dyn, exp_lut, abar0, apar, R.at_ch, bar, err_host, &s_abort, scores);
+            if (s_ph.at.kv_f16) phase_attn<true, QWEN2>(s_ph, (float*)work, s_red, dyn, exp_lut, abar0, apar, R.at_ch, bar, err_host, &s_abort, scores);
+            else phase_attn<false, QWEN2>(s_ph, (float*)work, s_red, dyn, exp_lut, abar0, apar, R.at_ch, bar, err_host, &s_abort, scores);
             break;
         case MK_ROWS: phase_rows(s_ph, dyn); break;
         case MK_REDUCE: phase_reduce(s_ph, comm, xseq, false); break;
@@ -651,7 +663,8 @@ size_t cc_mega_ring_smem_for_phase(const MkPhase& ph) {
 #define MR_MIN_SLOTS 12
 static size_t mr_ring_off(const MegaLaunch& L) { return ((((L.smem + 15) & ~(size_t)15) + L.wstage) + 127) & ~(size_t)127; }
 static auto mr_kernel(const MegaLaunch& L) {
-    return L.generic ? (L.sample ? mega_ring_kernel<true, true> : mega_ring_kernel<true, false>) : (L.sample ? mega_ring_kernel<false, true> : mega_ring_kernel<false, false>);
+    if (L.qwen2) return L.generic ? (L.sample ? mega_ring_kernel<true, true, true> : mega_ring_kernel<true, false, true>) : (L.sample ? mega_ring_kernel<false, true, true> : mega_ring_kernel<false, false, true>);
+    return L.generic ? (L.sample ? mega_ring_kernel<true, true, false> : mega_ring_kernel<true, false, false>) : (L.sample ? mega_ring_kernel<false, true, false> : mega_ring_kernel<false, false, false>);
 }
 int cc_mega_ring_slots(const MegaLaunch& L) {
     cudaFuncAttributes fa;

@@ -155,14 +155,18 @@ def load_gguf(path: str, device: CudaTensorDevice, shard=None, f16_kv=False):
     def scalar(k):
         return f[k].parts[f[k].data[0]][0]
     arch = bytes(f["general.architecture"].parts[f["general.architecture"].data[0]]).decode()
-    if arch != "llama":
+    if arch not in ("llama", "qwen2"):                    # model.rs:285-351, 559
         raise TensorError(f"unsupported architecture {arch}")
+    if arch == "qwen2" and shard is not None and shard[1] > 1:
+        raise TensorError("sharding: only the llama forward is sharded")
     tokens = [bytes(f["tokenizer.ggml.tokens"].parts[i]).decode("utf-8") for i in f["tokenizer.ggml.tokens"].data]
     conf = LlamaConfig(int(scalar(f"{arch}.attention.head_count")), int(scalar(f"{arch}.attention.head_count_kv")),
                        int(scalar(f"{arch}.block_count")), int(scalar(f"{arch}.embedding_length")),
                        int(scalar(f"{arch}.feed_forward_length")), int(scalar(f"{arch}.context_length")), len(tokens),
                        float(np.float32(scalar(f"{arch}.attention.layer_norm_rms_epsilon"))),
-                       int(scalar(f"{arch}.rope.dimension_count")) if f"{arch}.rope.dimension_count" in f else 0)
+                       int(scalar(f"{arch}.rope.dimension_count")) if f"{arch}.rope.dimension_count" in f else 0, arch)
+    # RoPE runs at base 10000 for every architecture, as in the reference (rope.rs:48,69 hard-code it): `{arch}.rope.freq_base` is
+    # deliberately not read, so a qwen2 file decodes as the reference decodes it (DESIGN.md §7)
     tensors = {t.name: t for t in rd.tensors}
 
     plan = None
@@ -181,6 +185,9 @@ def load_gguf(path: str, device: CudaTensorDevice, shard=None, f16_kv=False):
     names = {"wq": "attn_q", "wk": "attn_k", "wv": "attn_v", "wo": "attn_output", "ffn_gate": "ffn_gate", "ffn_down": "ffn_down",
              "ffn_up": "ffn_up", "rms_att": "attn_norm", "rms_ffn": "ffn_norm"}
     w = {k: [load(f"blk.{l}.{v}.weight", k) for l in range(L)] for k, v in names.items()}
+    if arch == "qwen2":
+        for k, v in (("bq", "attn_q"), ("bk", "attn_k"), ("bv", "attn_v")):
+            w[k] = [load(f"blk.{l}.{v}.bias") for l in range(L)]
     w["token_embed"] = load("token_embd.weight")
     w["rms_final"] = load("output_norm.weight")
     if "output.weight" in tensors:
@@ -233,4 +240,7 @@ def synthetic_weights(device: CudaTensorDevice, conf: LlamaConfig, wtype: int, c
     w["token_embed"] = syn(conf.vocab_size, dim, wtype)
     w["output_weight"] = syn(conf.vocab_size, dim, ct, "output_weight")
     w["rms_final"] = norm()
+    if conf.arch == "qwen2":                # q/k/v biases (llama2.rs:315-317), of the size of a matvec output element
+        for k, n in (("bq", dim), ("bk", kv), ("bv", kv)):
+            w[k] = [CudaTensor.from_cpu((0.5 * rng.standard_normal(n)).astype(np.float32), [n], capi.F32, device) for _ in range(L)]
     return w
