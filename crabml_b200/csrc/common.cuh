@@ -306,8 +306,9 @@ struct MkPhase {
                                         // SAMPLE: as ARGMAX, with a SampleDyn at dyn_off and the sampler scratch at dst
     int norm_ahead, pad2;               // fused norm: no op of the table writes norm_w (model weights), so it may be staged before earlier phases end
 };
-#define MK_PROF_SLOTS 9      // developer profiling: u64 stamps per phase (CTA 0 / thread 0): 0 start, 1 activation ready, 2 rows done, 3 arrived, 4 x staged, 5 rms known,
-                             // 6-7 ring consumer counters, 8 norm weights available (mega_ring.cu); read by tools/mega_profile*.py
+#define MK_PROF_SLOTS 10     // developer profiling: u64 stamps per phase (CTA 0 / thread 0): 0 start, 1 activation ready, 2 rows done, 3 arrived, 4 x staged, 5 rms known,
+                             // 6-7 ring consumer counters, 8 norm weights available, 9 ring occupancy as the barrier in front of the phase opened
+                             // (mega_ring.cu); read by tools/mega_profile*.py
 size_t cc_mega_smem_for_phase(const MkPhase& ph);      // working area, without the norm-weight staging area on top of it
 const CommDev* cc_comm_dev(cc_device* dev);
 bool cc_comm_is_nccl(cc_device* dev);

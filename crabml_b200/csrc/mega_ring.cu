@@ -25,7 +25,7 @@
 #define MR_PRODUCER_WARPS 4        // 20 warps: five per SM sub-partition, still 96 registers per thread
 #define MR_THREADS (MK_THREADS + 32 * MR_PRODUCER_WARPS)
 #define MR_MAX_SLOTS 112
-#define MR_Q8_SLOTS 24             // ring depth for Q8_0 entries (cc_mega_ring_slots)
+#define MR_Q8_FLIGHT 10            // Q8_0 entries a producer lets be in flight at once (cc_launch_mega_ring)
 #define MR_DESC_WORDS ((int)(sizeof(MkPhase) / 4))
 #define MR_DESC_PER_LANE ((MR_DESC_WORDS + 31) / 32)
 
@@ -34,6 +34,7 @@ struct MrRing {
     int slot_bytes;        // bytes per slot (multiple of 128): quants of up to 4 groups, then their f16 scales
     int nslots;
     int at_ch;             // ATTN phase: cache rows per TMA chunk
+    int flight;            // entry e is issued only once entry e - flight has landed (flight = nslots: no such limit)
 };
 
 __device__ __forceinline__ void mr_expect_tx(unsigned bar, unsigned bytes) { asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory"); }
@@ -57,6 +58,24 @@ __device__ __forceinline__ bool mr_try_wait(unsigned bar, unsigned parity) {
     unsigned ok;
     asm volatile("{\n.reg .pred p;\nmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\nselp.u32 %0, 1, 0, p;\n}\n" : "=r"(ok) : "r"(bar), "r"(parity) : "memory");
     return ok != 0;
+}
+__device__ __forceinline__ bool mr_test_wait(unsigned bar, unsigned parity) {
+    unsigned ok;
+    asm volatile("{\n.reg .pred p;\nmbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\nselp.u32 %0, 1, 0, p;\n}\n" : "=r"(ok) : "r"(bar), "r"(parity) : "memory");
+    return ok != 0;
+}
+// Developer profiling (CTA 0, warp 0, all lanes), as the barrier in front of a phase opens: how many entries from `ent` on (the consumers'
+// next entry) the producers have issued into the ring and how many of those have landed, as (landed << 8) | issued -- one look at every
+// slot.  A called function: inlined, or taken at more points of a phase, it moves the kernel's spills.
+__device__ __noinline__ unsigned mr_ring_fill(const volatile unsigned* s_seq, unsigned full0, int nslots, unsigned ent) {
+    unsigned iss = 0, got = 0;
+    for (int sl = threadIdx.x & 31; sl < nslots; sl += 32) {
+        const unsigned q = s_seq[sl];
+        if (q && (int)(q - 1u - ent) >= 0) { iss++; got += mr_test_wait(full0 + 8u * sl, ((q - 1u) / (unsigned)nslots) & 1u) ? 1u : 0u; }
+    }
+    iss = __reduce_add_sync(0xffffffffu, iss);
+    got = __reduce_add_sync(0xffffffffu, got);
+    return (got << 8) | iss;
 }
 // Slot hand-back: the consumer stores (entry number + 1) into the slot's "done" word (release), the producer polls it (acquire) for
 // exactly the previous tenant's number -- an mbarrier parity could not tell one lap from two.  `dep` ties the store behind the
@@ -102,6 +121,13 @@ __device__ __forceinline__ int mr_locate(const StreamMats& M, const MrGeo& g, in
     return r;
 }
 
+// entry f has landed: it has been consumed (the slot's done word has reached it; a slot's tenants are consumed in order), or it is the
+// slot's tenant and its barrier phase has completed -- exact, since the tenant cannot change before it is consumed
+__device__ __forceinline__ bool mr_landed(unsigned f, int nslots, unsigned full0, unsigned done0, volatile unsigned* s_seq) {
+    const unsigned sl = f % (unsigned)nslots;
+    if ((int)(mr_ld_acquire_shared(done0 + 4u * sl) - 1u - f) >= 0) return true;
+    return s_seq[sl] == f + 1u && mr_test_wait(full0 + 8u * sl, (f / (unsigned)nslots) & 1u);
+}
 // ---- producer warp: runs ahead of everybody ---------------------------------------------------------------------------------------------
 // All 32 lanes issue (a single issuing thread manages only ~1 entry per few hundred cycles); lane l owns the entries l, l + 32, ...
 // of a phase: it decomposes the entry index into (unit, virtual row, segment), waits until the slot's previous tenant has been consumed, arms the
@@ -159,7 +185,8 @@ __device__ void mr_producer(const MkPhase* __restrict__ phases, int n_phases, co
                     e = ent + (unsigned)j; slot = e % (unsigned)R.nslots; use = e / (unsigned)R.nslots;
                     have = true;
                 }
-                if (!use || mr_ld_acquire_shared(done0 + 4u * slot) == e - (unsigned)R.nslots + 1u) {      // the slot's previous tenant has been consumed
+                if ((!use || mr_ld_acquire_shared(done0 + 4u * slot) == e - (unsigned)R.nslots + 1u)      // the slot's previous tenant has been consumed
+                    && (R.flight >= R.nslots || e < (unsigned)R.flight || mr_landed(e - (unsigned)R.flight, R.nslots, full0, done0, s_seq))) {
                     const unsigned fb = full0 + 8u * slot, dst = ring0 + slot * (unsigned)R.slot_bytes;
                     const unsigned dbytes = (nbe * 2u + 15u) & ~15u;        // the scale rows are padded to 16 bytes (CC_D_STRIDE): a short last segment copies its padding
                     mr_expect_tx(fb, nbe * BB + dbytes);
@@ -180,7 +207,7 @@ __device__ void mr_producer(const MkPhase* __restrict__ phases, int n_phases, co
         __syncwarp();
     }
     if (lane == 0) { __threadfence_block(); atomicAdd(s_prod_done, 1); }
-    if (pt == 0 && prof_tail && blockIdx.x == 0) { prof_tail[1] = p_trips; prof_tail[2] = p_cyc; prof_tail[3] = p_iss; }
+    if (pt == 0 && prof_tail && blockIdx.x == 0) { prof_tail[1] = p_trips; prof_tail[2] = p_cyc; prof_tail[3] = p_iss; prof_tail[4] = (unsigned)R.nslots; }
 }
 
 // ---- consumer side of a streaming MATVEC phase ------------------------------------------------------------------------------------------
@@ -561,7 +588,11 @@ __global__ void __launch_bounds__(MR_THREADS, 1) mega_ring_kernel(const MkPhase*
     const int n_loop = SMP ? n_phases - 1 : n_phases;      // SMP: the last phase, the sampler, runs after the loop
     for (int p = 0; p < n_loop; p++) {
         const bool stamp = prof && blockIdx.x == 0 && threadIdx.x == 0;
-        if (stamp) { prof[p * MK_PROF_SLOTS] = globaltimer_ns(); prof[p * MK_PROF_SLOTS + 1] = 0; prof[p * MK_PROF_SLOTS + 4] = 0; prof[p * MK_PROF_SLOTS + 5] = 0; prof[p * MK_PROF_SLOTS + 8] = 0; }
+        const bool stampw = prof && blockIdx.x == 0 && threadIdx.x < 32;        // warp 0: ring occupancy (mr_ring_fill)
+        if (stamp) {
+            prof[p * MK_PROF_SLOTS] = globaltimer_ns(); prof[p * MK_PROF_SLOTS + 1] = 0; prof[p * MK_PROF_SLOTS + 4] = 0; prof[p * MK_PROF_SLOTS + 5] = 0; prof[p * MK_PROF_SLOTS + 8] = 0;
+            if (p == 0) prof[9] = 0;            // later phases: stamped as the barrier in front of them opens
+        }
         MK_SYNC();                           // descriptor p is in shared memory (stored one phase ago)
         const MkPhase& s_ph = s_phs[p & 1];
         if (p == 0 && !(s_ph.type == MK_MATVEC && s_ph.x && s_ph.norm_w)) { wst = s_ph.next_norm_w; if (wst) mr_stage_f32(s_wn, wst, s_ph.next_norm_n); }
@@ -606,6 +637,8 @@ __global__ void __launch_bounds__(MR_THREADS, 1) mega_ring_kernel(const MkPhase*
         if (more) {
             grid_barrier_wait(bar, gridDim.x, gen, comm, xg ? xseq + 1u : 0u, &s_abort, err_host);
             gen++; if (xg) xseq++;
+            // the occupancy as the barrier opened, or as this CTA gave up on it
+            if (stampw) { const unsigned f = mr_ring_fill(s_seq, full0, R.nslots, RC.ent_base); if (stamp) prof[(p + 1) * MK_PROF_SLOTS + 9] = f; }
             if (s_abort) break;              // a barrier timed out: bail out, the host reports it
             // the barrier is open: the row the next fused prologue quantises is complete -- request it before the descriptor bookkeeping
             const MkPhase& nph = s_phs[(p + 1) & 1];
@@ -656,10 +689,15 @@ size_t cc_mega_ring_smem_for_phase(const MkPhase& ph) {
 // and the norm-weight stage, and takes what is left of the SM's shared memory.  Returns the slot count, or 0 when fewer than
 // MR_MIN_SLOTS fit -- e.g. a 32 K-token context, whose attention phase needs 128 KB for the score row alone -- and lazy.cu runs the
 // table in the CUDA-graph mode.
-// Ring depth: a Q8_0 ring (4352-byte slots) is faster SHALLOW -- 24 slots = 104 KB per SM decode a Llama-2-7B token in 3.88 ms
+// Ring depth, history: a Q8_0 ring (4352-byte slots) was faster SHALLOW -- 24 slots = 104 KB per SM decode a Llama-2-7B token in 3.88 ms
 // against 4.04 ms with the ~40 that fit, and 20 / 16 / 12 slots are slower again (NVIDIA H100 80GB HBM3, 400 W).  Retuned with the
 // prologue inputs staged early: 16-24 slots within the spread, 28 and 32 are 4-6 % slower (same card, 700 W).  The Q4_0 consumer is
 // ALU-bound and keeps every slot that fits: a 55 KB ring (24 of its slots) cost it 2-4 %, 46 KB 9 %.
+// Why: more than ~24 Q8_0 entries in flight per SM make the SMs' progress through a phase uneven, and the barrier waits for the
+// slowest; but a 24-slot ring is full, and its SM reads no weights, through every prologue and attention phase (tools/mega_profile.py).
+// So every ring now takes all the slots that fit, and a Q8_0 producer keeps at most MR_Q8_FLIGHT entries in flight: the in-phase queue
+// stays short, and the slots beyond it fill with landed weights while the SM has nothing else to read (DESIGN §10).  The Q4_0 consumer
+// is the bound of its phases and keeps no in-flight limit.
 #define MR_MIN_SLOTS 12
 static size_t mr_ring_off(const MegaLaunch& L) { return ((((L.smem + 15) & ~(size_t)15) + L.wstage) + 127) & ~(size_t)127; }
 static auto mr_kernel(const MegaLaunch& L) {
@@ -673,7 +711,7 @@ int cc_mega_ring_slots(const MegaLaunch& L) {
     if (L.slot_bytes <= 0 || off >= cap) return 0;
     const int fit = (int)std::min((cap - off) / (size_t)L.slot_bytes, (size_t)MR_MAX_SLOTS);
     if (fit < MR_MIN_SLOTS) return 0;
-    return L.slot_bytes >= 4352 ? std::min(fit, MR_Q8_SLOTS) : fit;
+    return fit;
 }
 
 int cc_launch_mega_ring(cc_device* dev, const MkPhase* phases_dev, int n_phases, const uint8_t* dyn_dev, unsigned* bar_dev, const MegaLaunch& L,
@@ -691,6 +729,7 @@ int cc_launch_mega_ring(cc_device* dev, const MkPhase* phases_dev, int n_phases,
     if (comm) cd = *comm;
     MrRing R;
     R.ring_off = (int)ring_off; R.slot_bytes = L.slot_bytes; R.nslots = L.nslots; R.at_ch = L.at_ch;
+    R.flight = L.slot_bytes >= 4352 ? std::min(L.nslots, MR_Q8_FLIGHT) : L.nslots;
     const uint16_t* lut = dev->exp_lut;
     return mk_launch(dev, kern, dev->sm_count, MR_THREADS, smem, phases_dev, n_phases, dyn_dev, bar_dev, lut, prof, cc_mega_test_stall(), (int)wtop,
                      dev->err_host, (const CommDev)cd, (const MrRing)R, L.scores);

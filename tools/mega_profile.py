@@ -27,7 +27,7 @@ for i in range(40):
     r.forward([100 + i], pos, export=False); pos += 1
 ms = dev.timer_end()
 print(f"40 tokens back to back: {ms / 40 * 1e3:.1f} us per token by CUDA events (kernel time below + inter-launch gap)")
-SL = 9                                      # stamps per phase (common.cuh MK_PROF_SLOTS)
+SL = 10                                     # stamps per phase (common.cuh MK_PROF_SLOTS)
 CAP = SL * 4097
 ts = (C.c_uint64 * CAP)(); ty = (C.c_int32 * CAP)(); n = C.c_int32(0)
 dev.check(dev.lib.cc_lazy_mega_profile(dev.handle, ts, ty, CAP, C.byref(n)))
@@ -66,7 +66,19 @@ for k, v in sorted(agg.items(), key=lambda kv: -sum(kv[1])):
     m = np.mean(np.array(sub[k]), axis=0)
     ringinfo = f" || ring w0: {m[9]:4.1f} entries, {m[8] / max(m[9], 1):6.0f} cyc/entry, waiting {100 * m[7] / max(m[8], 1):3.0f} %" if m[9] > 0 else ""
     print(f"  {k:16s} n={len(v):3d}  sum {sum(v):8.1f} us  avg {np.mean(v):6.2f}  min {min(v):6.2f}  max {max(v):6.2f}   | {m[0]:5.2f} | {m[1]:5.2f} | {m[2]:5.2f} | {m[3]:5.2f} || {m[10]:5.2f} | {m[4]:5.2f} || {m[5]:5.2f} | {m[6]:5.2f}{ringinfo}")
-tail = [int(ts[n * SL + i]) for i in range(1, 4)]
+tail = [int(ts[n * SL + i]) for i in range(1, 5)]      # producer trips, cycles, entries; ring slots
 if tail[0]:
     print(f"  ring producer (CTA 0, lane 0): {tail[0]} trips, {tail[2]} entries issued, {tail[1] / tail[0]:.0f} cycles per trip, {tail[1] / 1.965e3:.0f} us inside streaming phases")
+    # ring occupancy of CTA 0 (slot 9) as the barrier in front of a phase opened: entries beyond the consumers' position that the producers
+    # had issued / that had landed.  No slot is handed back before the phase's rows start, so a ring full here stays full, and this SM
+    # reads no weights, through the prologue (and, for an attention phase, the whole phase)
+    nslots = tail[3]
+    print(f"  ring occupancy as the barrier in front of the phase opened (CTA 0, entries landed / issued ahead of the consumers; {nslots} slots):")
+    occ = collections.defaultdict(list)
+    for i in range(1, n):
+        o = int(ts[i * SL + 9])
+        occ[name(ty[i])].append((o >> 8 & 0xFF, o & 0xFF))
+    for k, v in occ.items():
+        a = np.array(v, dtype=np.float64)
+        print(f"    {k:16s} {np.mean(a[:, 0]):5.1f} / {np.mean(a[:, 1]):5.1f}   full in {100 * np.mean(a[:, 0] >= nslots):3.0f} % of {len(a)}")
 dev.close()

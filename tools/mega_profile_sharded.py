@@ -38,7 +38,7 @@ dev.timer_begin()
 for i in range(40):
     r.forward([100 + i], pos, export=False); pos += 1
 ms = dev.timer_end()
-SL = 9                                      # stamps per phase (common.cuh MK_PROF_SLOTS)
+SL = 10                                     # stamps per phase (common.cuh MK_PROF_SLOTS)
 CAP = SL * 4097
 ts = (C.c_uint64 * CAP)(); ty = (C.c_int32 * CAP)(); n = C.c_int32(0)
 dev.check(dev.lib.cc_lazy_mega_profile(dev.handle, ts, ty, CAP, C.byref(n)))
