@@ -167,7 +167,7 @@ extern "C" CC_API int cc_copy_rows_from(cc_device* dev, const cc_view* dst, cons
     if (rc) return rc;
     // pinned staging slot may still be read by an earlier async copy: keep it simple and synchronous w.r.t. the stream
     CC_CUDA(dev, cudaMemcpyAsync(dev->dev_idx, rows, (size_t)n_rows * 8, cudaMemcpyHostToDevice, dev->stream));
-    return cc_launch_dequant_rows(dev, src->buf, (const int64_t*)dev->dev_idx, n_rows, cols, dst->buf->plane[0], dt);
+    return cc_launch_dequant_rows(dev, cc_deq_planes(src->buf, cols), src->buf->dtype, (const int64_t*)dev->dev_idx, n_rows, cols, dst->buf->plane[0], dt);
 }
 
 // ---- in-place ops -------------------------------------------------------------------------------------------------------
@@ -333,7 +333,7 @@ extern "C" CC_API int cc_copy_rows_from_slot(cc_device* dev, const cc_view* dst,
     if (rc) return rc;
     if (LAZY(dev)) return cc_lazy_record(dev, L_COPY_ROWS, dst, src, nullptr, 0, 0, 0, slot + 1, nullptr, 0);
     // NOTE: the id in the slot was produced by argmax over this model's logits, i.e. it is < vocab rows by construction
-    return cc_launch_dequant_rows(dev, src->buf, dev->slots + slot, 1, cols, dst->buf->plane[0], dt);
+    return cc_launch_dequant_rows(dev, cc_deq_planes(src->buf, cols), src->buf->dtype, dev->slots + slot, 1, cols, dst->buf->plane[0], dt);
 }
 extern "C" CC_API int cc_slot_set(cc_device* dev, int32_t slot, int64_t value) {
     if (!dev) return CC_ERR_ARG;

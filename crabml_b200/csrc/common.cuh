@@ -181,6 +181,22 @@ int cc_fail(cc_device* dev, int code, const char* fmt, ...);
                            cudaGetErrorString(_e), __FILE__, __LINE__);                     \
     } while (0)
 
+// launch with programmatic dependent launch (pdl: cc_device::pdl): the kernel may start while the previous one in the stream drains
+template <class... KArgs, class... Args>
+static cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, bool pdl, Args... args) {
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = grid;
+    cfg.blockDim = block;
+    cfg.dynamicSmemBytes = smem;
+    cfg.stream = stream;
+    cudaLaunchAttribute at[1];
+    at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    at[0].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = at;
+    cfg.numAttrs = pdl ? 1 : 0;
+    return cudaLaunchKernelEx(&cfg, kernel, KArgs(args)...);
+}
+
 // counter-based generator of the synthetic weights (repack.cu) and of the sampler's coin (sample_dev.cuh)
 __host__ __device__ inline uint64_t cc_splitmix64(uint64_t x) {
     x += 0x9E3779B97F4A7C15ull;
@@ -208,7 +224,15 @@ size_t cc_device_layout_bytes(int t, int64_t rows, int64_t cols);
 void cc_assign_planes(cc_buf* b);
 int cc_launch_repack(cc_device* dev, const uint8_t* gguf_dev, cc_buf* dst);           // GGUF AoS -> planes
 int cc_launch_unrepack(cc_device* dev, const cc_buf* src, uint8_t* gguf_dev);          // planes -> GGUF AoS
-int cc_launch_dequant_rows(cc_device* dev, const cc_buf* src, const int64_t* rows_dev, int n_rows,
+struct DeqPlanes { const uint8_t* p[CC_MAX_PLANES]; int64_t cols; };
+// the planes of b as the dequantising kernels read them; cols is the row length of an unquantised (f32 / f16) b
+inline DeqPlanes cc_deq_planes(const cc_buf* b, int64_t cols) {
+    DeqPlanes P;
+    for (int i = 0; i < CC_MAX_PLANES; i++) P.p[i] = b->plane[i];
+    P.cols = b->cols > 0 ? b->cols : cols;
+    return P;
+}
+int cc_launch_dequant_rows(cc_device* dev, const DeqPlanes& src, int src_dtype, const int64_t* rows_dev, int n_rows,
                            int64_t cols, void* dst, int dst_dtype);                    // copy_rows_from
 int cc_launch_synth(cc_device* dev, uint8_t* gguf_dev, int t, int64_t nblocks, uint64_t seed, uint64_t tid, float scale);
 
@@ -287,7 +311,6 @@ struct AttnArgs {            // fused decode attention (fused.cu)
 #define AT_ARRIVE_WORD 128
 #define AT_SPLIT_MAX_HEADS ((1024 - AT_ARRIVE_WORD) / 8)
 int cc_attn_split(const AttnArgs& a, int grid);
-struct DeqPlanes { const uint8_t* p[CC_MAX_PLANES]; int64_t cols; };
 // megakernel phase descriptor (mega.cu); built by lazy.cu
 enum { MK_NORMQ = 0, MK_MATVEC = 1, MK_ATTN = 2, MK_ROWS = 3, MK_REDUCE = 4, MK_GATHER = 5, MK_ARGMAX = 6, MK_SAMPLE = 7 };
 struct MkPhase {
@@ -338,7 +361,7 @@ int cc_mega_ring_slots(const MegaLaunch& L);
 int cc_launch_mega_ring(cc_device* dev, const MkPhase* phases_dev, int n_phases, const uint8_t* dyn_dev, unsigned* bar_dev, const MegaLaunch& L,
                         unsigned long long* prof, const CommDev* comm);
 int cc_check_async_error(cc_device* dev);     // after a stream synchronize: did a persistent kernel give up on a barrier?
-int cc_launch_normq(cc_device* dev, float* x, float* orig, const float* norm_w, float eps, int64_t n, void* act_scratch, bool write_back);
+int cc_launch_normq(cc_device* dev, float* x, float* orig, const float* norm_w, float eps, int64_t n, ActQ8_0 act, bool write_back);
 int cc_launch_attn_decode(cc_device* dev, const AttnArgs& a, const int64_t* dyn /* {pos, kv_len} */, const float* rope_tab /* cos[pairs], sin[pairs] */);
 bool cc_attn_decode_fits(int64_t hd, int64_t max_len);      // can the single-pass attention kernel hold the score row of this cache?
 struct LazyState;

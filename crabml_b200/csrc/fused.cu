@@ -200,30 +200,13 @@ __global__ void __launch_bounds__(AT_THREADS) attn_decode_kernel(const float* __
     }
 }
 
-// ---- launch helpers (PDL attribute) -----------------------------------------------------------------------------------
-template <class... KArgs, class... Args>
-static cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, bool pdl, Args... args) {
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = grid;
-    cfg.blockDim = block;
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = stream;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    at[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = at;
-    cfg.numAttrs = pdl ? 1 : 0;
-    return cudaLaunchKernelEx(&cfg, kernel, KArgs(args)...);
-}
-
-int cc_launch_normq(cc_device* dev, float* x, float* orig, const float* norm_w, float eps, int64_t n, void* act_scratch, bool write_back) {
+int cc_launch_normq(cc_device* dev, float* x, float* orig, const float* norm_w, float eps, int64_t n, ActQ8_0 act, bool write_back) {
     CC_REQUIRE(dev, n % 32 == 0, "normq: length %lld %% 32 != 0", (long long)n);
     CC_REQUIRE(dev, n % 4 == 0, "normq: length %lld %% 4 != 0", (long long)n);
     int ctas = (int)((n / 32 + NQ_THREADS / 32 - 1) / (NQ_THREADS / 32));
     if (ctas > NQ_MAX_CTAS) ctas = NQ_MAX_CTAS;
     if (ctas < 1 || (norm_w && write_back)) ctas = 1;
-    cudaError_t e = launch_pdl(normq_kernel, dim3(ctas), dim3(NQ_THREADS), 0, dev->stream, dev->pdl, x, orig, norm_w, eps, (int)n, cc_act_q8_0(act_scratch, n),
-                               write_back ? 1 : 0);
+    cudaError_t e = launch_pdl(normq_kernel, dim3(ctas), dim3(NQ_THREADS), 0, dev->stream, dev->pdl, x, orig, norm_w, eps, (int)n, act, write_back ? 1 : 0);
     if (e != cudaSuccess) return cc_fail(dev, CC_ERR_CUDA, "normq launch: %s", cudaGetErrorString(e));
     dev->launches++;
     return CC_OK;

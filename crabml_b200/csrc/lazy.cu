@@ -4,9 +4,10 @@
 // eager mode.  Per-launch overhead, not kernel bodies, is what caps decode.  In lazy mode the
 // SAME C-ABI calls only append to a queue (after the same argument checks); the queue is executed at the first call that
 // needs a result on the host (export / debug tap / synchronize -- the reference synchronises only there too, llama2.rs:209):
-//   1. fuse: runs of ops that match the Llama decode layer (llama2.rs:226-269, 527-638) are replaced by the kernels of
-//      fused.cu / matvec_stream.cu; anything unrecognised falls back to its eager kernel, in order;
-//   2. the resulting launch list is hashed (kernel ids, pointers, static sizes).  Values that change every token
+//   1. fuse: runs of ops that match the Llama decode layer (llama2.rs:226-269, 527-638) are replaced by fused steps, each described by
+//      one phase descriptor (MkPhase) that the persistent kernels run and the CUDA-graph mode launches as a kernel of fused.cu /
+//      matvec_stream.cu; anything unrecognised falls back to its eager kernel, in order;
+//   2. the plan is hashed: each eager op's words and each fused step's descriptor bytes.  Values that change every token
 //      (position, KV length, token ids, RoPE table) live in a small device buffer `dyn` that the kernels read;
 //   3. first time a hash is seen the launches are stream-captured into a CUDA graph (programmatic-dependent-launch edges
 //      included); afterwards a token = one 1-2 KB H2D copy of `dyn` + one cudaGraphLaunch.
@@ -17,7 +18,6 @@
 #include <string.h>
 
 #include <chrono>
-#include <functional>
 
 #include "sample_dev.cuh"
 
@@ -146,15 +146,39 @@ int cc_lazy_record(cc_device* dev, int kind, const cc_view* a, const cc_view* b,
 }
 
 // ---- plan building ---------------------------------------------------------------------------------------------------
+// A zero-filled descriptor of one fused step: its bytes, padding included (AttnArgs has 4 at its end), become signature words.
+// Fill its fields in place: a struct assigned into it need not carry its own padding over.
+static MkPhase new_phase(int type) {
+    MkPhase ph;
+    memset(&ph, 0, sizeof(ph));
+    ph.type = type;
+    return ph;
+}
+
 struct Plan {
     std::vector<uint64_t> sig;
     std::vector<uint8_t> dyn;
-    std::vector<std::function<int(uint8_t* dyn_dev)>> steps;
+    // the CUDA-graph mode's launches, in order: a fused step (index into `emitted`) or an eager op (index into the queue)
+    struct Step { bool eager; uint32_t at; };
+    std::vector<Step> steps;
     bool cacheable = true;
+    std::vector<MkPhase> emitted;    // the fused steps' descriptors as emitted, before merge_prologue folds any of `phases` together
     std::vector<MkPhase> phases;     // megakernel form of the same plan (valid while mega_ok)
     bool mega_ok = true;
     void S(uint64_t v) { sig.push_back(v); }
     void SP(const void* p) { sig.push_back((uint64_t)(uintptr_t)p); }
+    // One fused step.  A captured graph bakes in all of its descriptor: the persistent kernels read the uploaded table, the CUDA-graph
+    // mode launches from it (launch_phase).  So the descriptor's bytes are its signature words.  graph_step = false: a phase whose
+    // CUDA-graph form is the eager ops the caller emits after it (Fuser::eager).
+    void phase(const MkPhase& ph, bool graph_step = true) {
+        static_assert(sizeof(MkPhase) % 8 == 0, "a descriptor is whole signature words");
+        S(0x2000);
+        const size_t at = sig.size();
+        sig.resize(at + sizeof(MkPhase) / 8);
+        memcpy(&sig[at], &ph, sizeof(MkPhase));
+        phases.push_back(ph);
+        if (graph_step) { steps.push_back({false, (uint32_t)emitted.size()}); emitted.push_back(ph); }
+    }
     size_t dyn_put(const void* p, size_t n) {
         size_t off = (dyn.size() + 15) & ~(size_t)15;
         dyn.resize(off + n);
@@ -163,10 +187,82 @@ struct Plan {
     }
 };
 
+// Four interleaved lanes, so that the ~15 000 words of a Llama-2-7B token are not one chain of dependent multiplies.  The key only
+// has to spread plans apart: a hit compares the whole signature.
 static uint64_t hash_sig(const std::vector<uint64_t>& s) {
-    uint64_t h = 1469598103934665603ull;
-    for (uint64_t v : s) { h ^= v; h *= 1099511628211ull; h ^= h >> 29; }
-    return h;
+    const uint64_t prime = 1099511628211ull;
+    uint64_t h[4] = {1469598103934665603ull, 1469598103934665603ull ^ 1, 1469598103934665603ull ^ 2, 1469598103934665603ull ^ 3};
+    for (size_t i = 0; i < s.size(); i += 4)
+        for (size_t l = 0; l < 4 && i + l < s.size(); l++) { h[l] ^= s[i + l]; h[l] *= prime; h[l] ^= h[l] >> 29; }
+    return ((h[0] * prime ^ h[1]) * prime ^ h[2]) * prime ^ h[3];
+}
+
+// ---- the CUDA-graph mode's launches ---------------------------------------------------------------------------------------------
+// one recorded op as its eager kernel
+static int run_op(cc_device* d, const LOp& op) {
+    const LView &a = op.a, &b = op.b;
+    switch (op.kind) {
+    case L_DUP: {
+        int64_t n = vlen(a);
+        if (n && cudaMemcpyAsync(op.out->base, a.buf->plane[0], (size_t)n * 4, cudaMemcpyDeviceToDevice, d->stream) != cudaSuccess) return cc_fail(d, CC_ERR_CUDA, "dup copy failed");
+        return CC_OK;
+    }
+    case L_RMS_NORM: return cc_launch_rms_norm(d, (float*)a.buf->plane[0], a.ndim == 1 ? 1 : a.shape[0], a.shape[a.ndim - 1], op.f);
+    case L_MUL: return cc_launch_binary(d, (float*)a.buf->plane[0], op.i0, (const float*)b.buf->plane[0], op.i1, 1);
+    case L_ADD: return cc_launch_binary(d, (float*)a.buf->plane[0], op.i0, (const float*)b.buf->plane[0], op.i1, 0);
+    case L_SCALE: return cc_launch_scale(d, (float*)a.buf->plane[0], vlen(a), op.f);
+    case L_SILU: return cc_launch_silu(d, (float*)a.buf->plane[0], vlen(a));
+    case L_GELU: return cc_launch_gelu(d, (float*)a.buf->plane[0], vlen(a));
+    case L_ALLREDUCE: return cc_launch_all_reduce(d, (float*)a.buf->plane[0], op.i0, nullptr);
+    case L_ALLGATHER: return cc_launch_all_gather(d, (const float*)b.buf->plane[0], op.i0, (float*)a.buf->plane[0]);
+    case L_ARGMAX: return cc_launch_argmax(d, (const float*)a.buf->plane[0], vlen(a), d->slots + op.i0, d->history, nullptr, op.i1);
+    case L_SOFTMAX: { int64_t cols = a.shape[a.ndim - 1]; return cc_launch_softmax(d, (float*)a.buf->plane[0], cols ? vlen(a) / cols : 0, cols); }
+    case L_ROPE: return cc_launch_rope_exact(d, (float*)a.buf->plane[0], op.i1, op.i2, a.shape[a.ndim - 1], (int)op.f, op.i0, op.rows[0]);
+    case L_CONCAT:
+        return cc_launch_strided_copy(d, b.buf->plane[0], b.buf->dtype, b.shape, b.strides, a.buf->plane[0], a.buf->dtype, a.strides,
+                                      a.shape[op.i0] * a.strides[op.i0], a.ndim);
+    case L_CONTIGUOUS: {
+        int64_t dstr[CC_MAX_DIMS]; int64_t s = 1;
+        for (int k = a.ndim - 1; k >= 0; k--) { dstr[k] = s; s *= a.shape[k]; }
+        return cc_launch_strided_copy(d, a.buf->plane[0], a.buf->dtype, a.shape, a.strides, op.out->base, a.buf->dtype, dstr, 0, a.ndim);
+    }
+    case L_BMM:
+        return cc_launch_batch_matmul(d, (const float*)a.buf->plane[0], b.buf->plane[0], b.buf->dtype, (float*)op.out->base, a.shape[0], b.shape[0],
+                                      a.shape[1], a.shape[2], b.shape[2], b.strides[0], b.strides[1], b.strides[2]);
+    case L_COPY_ROWS: {
+        int n = (int)op.rows.size();
+        int rc = cc_ensure_dev_idx(d, (size_t)n * 8);
+        if (rc) return rc;
+        if (cudaMemcpyAsync(d->dev_idx, op.rows.data(), (size_t)n * 8, cudaMemcpyHostToDevice, d->stream) != cudaSuccess) return cc_fail(d, CC_ERR_CUDA, "row index upload failed");
+        return cc_launch_dequant_rows(d, cc_deq_planes(b.buf, a.shape[a.ndim - 1]), b.buf->dtype, (const int64_t*)d->dev_idx, n, a.shape[a.ndim - 1],
+                                      a.buf->plane[0], a.buf->dtype);
+    }
+    case L_MATVEC:
+        return cc_launch_matmul_vec(d, a.buf, (const float*)b.buf->plane[0], (float*)op.out->base, a.shape[0], a.shape[1], b.ndim == 1 ? 1 : b.shape[0]);
+    }
+    return cc_fail(d, CC_ERR_UNSUPPORTED, "lazy: unknown op kind %d", op.kind);
+}
+
+// one fused step, by its descriptor, as the kernel of fused.cu / matvec_stream.cu / comm.cu that does what its phase does in the
+// persistent kernels (a generic K-quant MATVEC phase has none: its graph form is eager ops)
+static int launch_phase(cc_device* d, const MkPhase& ph, const uint8_t* dyn_dev) {
+    switch (ph.type) {
+    case MK_NORMQ: return cc_launch_normq(d, ph.x, ph.orig, ph.norm_w, ph.eps, ph.n, ph.act, ph.write_back);
+    case MK_MATVEC: {
+        StreamArgs A = ph.mv;
+        if (A.epilogue == 3) A.epilogue = 0;      // the exchange's stores into every rank's slot: here the REDUCE / GATHER step's kernel
+        return cc_launch_matvec_stream(d, ph.wtype, A);
+    }
+    case MK_ATTN: return cc_launch_attn_decode(d, ph.at, (const int64_t*)(dyn_dev + ph.dyn_off), (const float*)(dyn_dev + ph.rope_off));
+    case MK_ROWS:
+        return cc_launch_dequant_rows(d, ph.planes, ph.src_dtype, ph.rows_dev ? (const int64_t*)ph.rows_dev : (const int64_t*)(dyn_dev + ph.dyn_off),
+                                      ph.n_rows, ph.cols, ph.dst, ph.dst_dtype);
+    case MK_REDUCE: return cc_launch_all_reduce(d, ph.red_dst, ph.red_n, ph.red_res);
+    case MK_GATHER: return cc_launch_all_gather(d, ph.x, ph.red_n, ph.red_dst);
+    case MK_ARGMAX: return cc_launch_argmax(d, ph.x, ph.n, (int64_t*)ph.slot_dev, (int64_t*)ph.hist_dev, (const int64_t*)(dyn_dev + ph.dyn_off), -1);
+    case MK_SAMPLE: return cc_launch_sample(d, ph.x, ph.n, nullptr, (const SampleDyn*)(dyn_dev + ph.dyn_off), (int64_t*)ph.slot_dev, (int64_t*)ph.hist_dev);
+    }
+    return cc_fail(d, CC_ERR_UNSUPPORTED, "lazy: unknown phase type %d", ph.type);
 }
 
 struct Fuser {
@@ -204,12 +300,10 @@ struct Fuser {
     // skips the tail of an rhs longer than 1 (arithmetic.rs:5-68) -- a fused epilogue or norm would apply it to every element
     bool covers(const LOp& op, int64_t n) const { return op.i0 == n && op.i1 == n; }
 
-    // ---- eager fallback for one op -----------------------------------------------------------------------------
-    bool covered_by_phase = false;     // set while try_generic emits the eager steps of ops its megakernel phase covers
-    void fallback(size_t i) {
-        if (!covered_by_phase) P.mega_ok = false;
-        LOp op = q[i];       // copy: lambdas outlive the queue only until flush ends, but keep them self-contained
-        cc_device* d = dev;
+    // ---- eager steps ----------------------------------------------------------------------------------------------------------
+    // op i runs as its eager kernel in the CUDA-graph mode
+    void eager(size_t i) {
+        const LOp& op = q[i];
         P.S(0x1000 + op.kind); P.SP(op.a.buf ? op.a.buf->plane[0] : nullptr); P.SP(op.b.buf ? op.b.buf->plane[0] : nullptr);
         P.SP(op.out ? op.out->plane[0] : nullptr);
         // the pool hands an f32 and an f16 buffer of one size class the same address, and a weight re-created at a freed address may
@@ -224,49 +318,13 @@ struct Fuser {
         default: break;
         }
         for (int64_t r : op.rows) P.S((uint64_t)r);
-        P.steps.push_back([d, op](uint8_t*) -> int {
-            const LView &a = op.a, &b = op.b;
-            switch (op.kind) {
-            case L_DUP: {
-                int64_t n = vlen(a);
-                if (n && cudaMemcpyAsync(op.out->base, a.buf->plane[0], (size_t)n * 4, cudaMemcpyDeviceToDevice, d->stream) != cudaSuccess) return cc_fail(d, CC_ERR_CUDA, "dup copy failed");
-                return CC_OK;
-            }
-            case L_RMS_NORM: return cc_launch_rms_norm(d, (float*)a.buf->plane[0], a.ndim == 1 ? 1 : a.shape[0], a.shape[a.ndim - 1], op.f);
-            case L_MUL: return cc_launch_binary(d, (float*)a.buf->plane[0], op.i0, (const float*)b.buf->plane[0], op.i1, 1);
-            case L_ADD: return cc_launch_binary(d, (float*)a.buf->plane[0], op.i0, (const float*)b.buf->plane[0], op.i1, 0);
-            case L_SCALE: return cc_launch_scale(d, (float*)a.buf->plane[0], vlen(a), op.f);
-            case L_SILU: return cc_launch_silu(d, (float*)a.buf->plane[0], vlen(a));
-            case L_GELU: return cc_launch_gelu(d, (float*)a.buf->plane[0], vlen(a));
-            case L_ALLREDUCE: return cc_launch_all_reduce(d, (float*)a.buf->plane[0], op.i0, nullptr);
-            case L_ALLGATHER: return cc_launch_all_gather(d, (const float*)b.buf->plane[0], op.i0, (float*)a.buf->plane[0]);
-            case L_ARGMAX: return cc_launch_argmax(d, (const float*)a.buf->plane[0], vlen(a), d->slots + op.i0, d->history, nullptr, op.i1);
-            case L_SOFTMAX: { int64_t cols = a.shape[a.ndim - 1]; return cc_launch_softmax(d, (float*)a.buf->plane[0], cols ? vlen(a) / cols : 0, cols); }
-            case L_ROPE: return cc_launch_rope_exact(d, (float*)a.buf->plane[0], op.i1, op.i2, a.shape[a.ndim - 1], (int)op.f, op.i0, op.rows[0]);
-            case L_CONCAT:
-                return cc_launch_strided_copy(d, b.buf->plane[0], b.buf->dtype, b.shape, b.strides, a.buf->plane[0], a.buf->dtype, a.strides,
-                                              a.shape[op.i0] * a.strides[op.i0], a.ndim);
-            case L_CONTIGUOUS: {
-                int64_t dstr[CC_MAX_DIMS]; int64_t s = 1;
-                for (int k = a.ndim - 1; k >= 0; k--) { dstr[k] = s; s *= a.shape[k]; }
-                return cc_launch_strided_copy(d, a.buf->plane[0], a.buf->dtype, a.shape, a.strides, op.out->base, a.buf->dtype, dstr, 0, a.ndim);
-            }
-            case L_BMM:
-                return cc_launch_batch_matmul(d, (const float*)a.buf->plane[0], b.buf->plane[0], b.buf->dtype, (float*)op.out->base, a.shape[0], b.shape[0],
-                                              a.shape[1], a.shape[2], b.shape[2], b.strides[0], b.strides[1], b.strides[2]);
-            case L_COPY_ROWS: {
-                int n = (int)op.rows.size();
-                int rc = cc_ensure_dev_idx(d, (size_t)n * 8);
-                if (rc) return rc;
-                if (cudaMemcpyAsync(d->dev_idx, op.rows.data(), (size_t)n * 8, cudaMemcpyHostToDevice, d->stream) != cudaSuccess) return cc_fail(d, CC_ERR_CUDA, "row index upload failed");
-                return cc_launch_dequant_rows(d, b.buf, (const int64_t*)d->dev_idx, n, a.shape[a.ndim - 1], a.buf->plane[0], a.buf->dtype);
-            }
-            case L_MATVEC:
-                return cc_launch_matmul_vec(d, a.buf, (const float*)b.buf->plane[0], (float*)op.out->base, a.shape[0], a.shape[1], b.ndim == 1 ? 1 : b.shape[0]);
-            }
-            return cc_fail(d, CC_ERR_UNSUPPORTED, "lazy: unknown op kind %d", op.kind);
-        });
+        P.steps.push_back({true, (uint32_t)i});
         q[i].done = true;
+    }
+    // op i runs as its eager kernel, and no phase of the persistent kernels covers it: the plan runs in the CUDA-graph mode
+    void fallback(size_t i) {
+        P.mega_ok = false;
+        eager(i);
     }
 
     // ---- matchers shared by the patterns below -------------------------------------------------------------------------------
@@ -326,22 +384,16 @@ struct Fuser {
     size_t try_normq(size_t i, int act_sel, cc_buf** xbuf) {
         const NormMatch nm = match_norm(i);
         if (!nm.len || nm.n % 32 || nm.n > 65536) return 0;
-        const int64_t n = nm.n; const float eps = nm.eps;
-        float* x = (float*)nm.x->plane[0];
-        float* og = nm.orig ? (float*)nm.orig->base : nullptr;
-        const float* w = (const float*)nm.w->plane[0];
-        void* act = lz->act[act_sel];
-        cc_device* d = dev;
         // the normalised f32 row only has to be materialised if something other than the following matvecs reads it
         // (only matvecs the streaming kernel will take consume the quantised scratch; any other reader -- a K-quant or batched
         // matvec falling back to its eager kernel -- needs the f32 row)
         size_t end = i + nm.len;
         while (streams(end, nm.x)) end++;
-        const bool write_back = !dead_after(nm.x, end);
-        P.S(0x2001); P.SP(x); P.SP(og); P.SP(w); P.SP(act); P.S((uint64_t)n); uint32_t eb; memcpy(&eb, &eps, 4); P.S(eb); P.S(write_back);
-        P.steps.push_back([=](uint8_t*) { return cc_launch_normq(d, x, og, w, eps, n, act, write_back); });
-        { MkPhase ph = {}; ph.type = MK_NORMQ; ph.write_back = write_back; ph.x = x; ph.orig = og; ph.norm_w = w; ph.eps = eps; ph.n = (int)n; ph.act = cc_act_q8_0(act, n);
-          ph.norm_ahead = !written(nm.w); P.phases.push_back(ph); }
+        MkPhase ph = new_phase(MK_NORMQ);
+        ph.write_back = !dead_after(nm.x, end);
+        ph.x = (float*)nm.x->plane[0]; ph.orig = nm.orig ? (float*)nm.orig->base : nullptr; ph.norm_w = (const float*)nm.w->plane[0];
+        ph.eps = nm.eps; ph.n = (int)nm.n; ph.act = cc_act_q8_0(lz->act[act_sel], nm.n); ph.norm_ahead = !written(nm.w);
+        P.phase(ph);
         *xbuf = nm.x;
         for (size_t t = i; t < i + nm.len; t++) q[t].done = true;
         return nm.len;
@@ -355,21 +407,30 @@ struct Fuser {
         const int wt = m0.a.buf->dtype; const int64_t k = m0.a.shape[1];
         const GroupMatch g = match_group(i, xbuf, wt, k);
         size_t n = g.n, used = g.used;
-        StreamArgs A = {};
-        A.k = (int)k; A.epilogue = g.epilogue;
-        for (int t = 0; t < 3; t++) A.residual[t] = g.residual[t] ? (const float*)g.residual[t]->plane[0] : nullptr;
         // sharded path: column-split matvec -> allreduce [-> + residual]  /  row-split classifier -> allgather (comm.cu)
         int xchg = 0; float* xdst = nullptr; const float* xres = nullptr;
-        if (A.epilogue == 0 && is(i + 1, L_ALLREDUCE) && q[i + 1].a.buf == m0.out && q[i + 1].i0 == m0.a.shape[0]) {
+        if (g.epilogue == 0 && is(i + 1, L_ALLREDUCE) && q[i + 1].a.buf == m0.out && q[i + 1].i0 == m0.a.shape[0]) {
             n = 1; xchg = 1; used = 2; xdst = (float*)m0.out->base;
             if (is(i + 2, L_ADD) && q[i + 2].a.buf == m0.out && vlen(q[i + 2].b) == m0.a.shape[0] && covers(q[i + 2], m0.a.shape[0]) &&
                 q[i + 2].b.buf->dtype == CC_F32 && vcontig(q[i + 2].b)) {
                 xres = (const float*)q[i + 2].b.buf->plane[0];
                 used = 3;
             }
-        } else if (A.epilogue == 0 && is(i + 1, L_ALLGATHER) && q[i + 1].b.buf == m0.out && q[i + 1].i0 == m0.a.shape[0]) {
+        } else if (g.epilogue == 0 && is(i + 1, L_ALLGATHER) && q[i + 1].b.buf == m0.out && q[i + 1].i0 == m0.a.shape[0]) {
             n = 1; xchg = 2; used = 2; xdst = (float*)q[i + 1].a.buf->plane[0];
         }
+        void* act = lz->act[act_sel >= 0 ? act_sel : 1];
+        if (act_sel < 0) {                     // plain quantise of x (matmul_vec.rs:37-40)
+            MkPhase qz = new_phase(MK_NORMQ);
+            qz.x = (float*)m0.b.buf->plane[0]; qz.n = (int)k; qz.act = cc_act_q8_0(act, k);
+            P.phase(qz);
+        }
+        MkPhase ph = new_phase(MK_MATVEC);
+        ph.wtype = wt;
+        StreamArgs& A = ph.mv;
+        A.k = (int)k; A.epilogue = xchg ? 3 : g.epilogue; A.act = act;
+        ph.xgpu = xchg != 0;
+        for (int t = 0; t < 3; t++) A.residual[t] = g.residual[t] ? (const float*)g.residual[t]->plane[0] : nullptr;
         A.mats.n = (int)n;
         for (size_t t = 0; t < n; t++) {
             A.mats.qs[t] = q[i + t].a.buf->plane[0];
@@ -377,27 +438,13 @@ struct Fuser {
             A.mats.out[t] = (float*)q[i + t].out->base;
             A.mats.m[t] = (int)q[i + t].a.shape[0];
         }
-        cc_device* d = dev;
-        void* act = lz->act[act_sel >= 0 ? act_sel : 1];
-        A.act = act;
-        if (act_sel < 0) {                     // plain quantise of x (matmul_vec.rs:37-40)
-            float* x = (float*)m0.b.buf->plane[0];
-            P.S(0x2002); P.SP(x); P.SP(act); P.S((uint64_t)k);
-            P.steps.push_back([=](uint8_t*) { return cc_launch_normq(d, x, nullptr, nullptr, 0.0f, k, act, false); });
-            { MkPhase ph = {}; ph.type = MK_NORMQ; ph.x = x; ph.n = (int)k; ph.act = cc_act_q8_0(act, k); P.phases.push_back(ph); }
-        }
-        P.S(0x2003); P.S(wt); P.S(k); P.S(A.epilogue); P.SP(A.residual[0]); P.SP(A.residual[1]); P.SP(A.residual[2]); P.SP(act);
-        for (size_t t = 0; t < n; t++) { P.SP(A.mats.qs[t]); P.SP(A.mats.out[t]); P.S(A.mats.m[t]); }
-        P.steps.push_back([=](uint8_t*) { return cc_launch_matvec_stream(d, wt, A); });
-        { MkPhase ph = {}; ph.type = MK_MATVEC; ph.wtype = wt; ph.mv = A; if (xchg) { ph.mv.epilogue = 3; ph.xgpu = 1; }
-          P.phases.push_back(ph); }
+        P.phase(ph);
         if (xchg) {
             const int64_t mrows = m0.a.shape[0];
-            float* part = A.mats.out[0];
-            P.S(0x2006); P.S(xchg); P.SP(xdst); P.SP(xres); P.S(mrows);
-            if (xchg == 1) P.steps.push_back([=](uint8_t*) { return cc_launch_all_reduce(d, part, mrows, xres); });
-            else P.steps.push_back([=](uint8_t*) { return cc_launch_all_gather(d, part, mrows, xdst); });
-            MkPhase ph = {}; ph.type = xchg == 1 ? MK_REDUCE : MK_GATHER; ph.red_n = (int)mrows; ph.red_dst = xdst; ph.red_res = xres; P.phases.push_back(ph);
+            MkPhase ex = new_phase(xchg == 1 ? MK_REDUCE : MK_GATHER);
+            ex.red_n = (int)mrows; ex.red_dst = xdst; ex.red_res = xres;
+            if (xchg == 2) ex.x = A.mats.out[0];      // the row to gather, for launch_phase (the persistent kernels read the exchange slots)
+            P.phase(ex);
             if (!cc_comm_dev(dev) || cc_comm_is_nccl(dev)) P.mega_ok = false;      // NCCL baseline: graph of kernels + NCCL nodes (lazy mode 1)
             if ((((mrows + dev->sm_count - 1) / dev->sm_count + 3) & ~(int64_t)3) > 512) P.mega_ok = false;   // one CTA's row block must fit the exchange stage (mega_phases.cuh MK_XSTAGE_ROWS)
         }
@@ -443,9 +490,9 @@ struct Fuser {
             rope_off = P.dyn_put(tab.data(), tab.size() * 4);
             rope_pos = pos; rope_hd = (int)hd; this->rope_dim = (int)rope_dim; rope_mode = mode;
         }
-        int64_t dynv[2] = {pos, kv_len};
-        size_t dyn_off = P.dyn_put(dynv, sizeof(dynv));
-        AttnArgs A = {};
+        const int64_t dynv[2] = {pos, kv_len};
+        MkPhase ph = new_phase(MK_ATTN);
+        AttnArgs& A = ph.at;
         A.q = (const float*)qb->plane[0]; A.k = (const float*)kb->plane[0]; A.v = (const float*)vb->plane[0];
         A.kcache = kc->plane[0]; A.vcache = vc->plane[0];
         A.out = (float*)b2.out->base;
@@ -457,15 +504,8 @@ struct Fuser {
         A.seq_stride = seq_stride; A.scale = sc.f;
         // the most CTAs per head the score scratch allows; the persistent kernel's split is chosen with its grid (choose_mega)
         A.split = (size_t)n_heads * (size_t)(A.max_len + 1) * 4 <= lz->scores_cap ? AT_SPLIT_MAX : 1;
-        cc_device* d = dev;
-        size_t roff = rope_off;
-        P.S(0x2004); P.SP(A.q); P.SP(A.k); P.SP(A.v); P.SP(A.kcache); P.SP(A.vcache); P.SP(A.out); P.SP(A.act_scratch); P.S(A.split); P.SP(lz->scores);
-        P.S(n_heads); P.S(n_kv); P.S(hd); P.S(rope_dim); P.S(A.rope_neox); P.S(seq_stride); P.S(A.kv_f16); uint32_t sb; memcpy(&sb, &A.scale, 4); P.S(sb); P.S(dyn_off); P.S(roff);
-        P.steps.push_back([=](uint8_t* dyn_dev) {
-            return cc_launch_attn_decode(d, A, (const int64_t*)(dyn_dev + dyn_off), (const float*)(dyn_dev + roff));
-        });
-        { MkPhase ph = {}; ph.type = MK_ATTN; ph.at = A; ph.dyn_off = dyn_off; ph.rope_off = roff; ph.act = cc_act_q8_0(lz->act[1], n_heads * hd);
-          P.phases.push_back(ph); }
+        ph.dyn_off = P.dyn_put(dynv, sizeof(dynv)); ph.rope_off = rope_off; ph.act = cc_act_q8_0(lz->act[1], n_heads * hd);
+        P.phase(ph);
         *obuf = b2.out;
         for (size_t t = i; t < i + 9; t++) q[t].done = true;
         return 9;
@@ -475,20 +515,14 @@ struct Fuser {
     size_t try_copy_rows(size_t i) {
         if (!is(i, L_COPY_ROWS)) return 0;
         const LOp& op = q[i];
-        cc_device* d = dev;
-        const cc_buf* src = op.b.buf;
-        void* dst = op.a.buf->plane[0];
-        int dt = op.a.buf->dtype;
-        int64_t cols = op.a.shape[op.a.ndim - 1];
+        const int64_t cols = op.a.shape[op.a.ndim - 1];
         const int slot = (int)op.i2 - 1;                     // >= 0: the single row index lives in a device slot (cc_copy_rows_from_slot)
-        int n = slot >= 0 ? 1 : (int)op.rows.size();
-        size_t off = slot >= 0 ? 0 : P.dyn_put(op.rows.data(), op.rows.size() * 8);
-        const int64_t* rows_dev = slot >= 0 ? dev->slots + slot : nullptr;
-        P.S(0x2005); P.SP(src->plane[0]); P.SP(dst); P.S(dt); P.S(n); P.S(cols); P.S(off); P.SP(rows_dev); P.S(src->dtype); P.S(src->cols);   // (types: fallback())
-        P.steps.push_back([=](uint8_t* dyn_dev) { return cc_launch_dequant_rows(d, src, rows_dev ? rows_dev : (const int64_t*)(dyn_dev + off), n, cols, dst, dt); });
-        { MkPhase ph = {}; ph.type = MK_ROWS; ph.dyn_off = off; for (int t = 0; t < CC_MAX_PLANES; t++) ph.planes.p[t] = src->plane[t];
-          ph.planes.cols = src->cols > 0 ? src->cols : cols; ph.src_dtype = src->dtype; ph.dst_dtype = dt; ph.n_rows = n; ph.cols = cols; ph.dst = dst;
-          ph.rows_dev = (const long long*)rows_dev; P.phases.push_back(ph); }
+        MkPhase ph = new_phase(MK_ROWS);
+        ph.planes = cc_deq_planes(op.b.buf, cols); ph.src_dtype = op.b.buf->dtype;
+        ph.dst = op.a.buf->plane[0]; ph.dst_dtype = op.a.buf->dtype; ph.n_rows = slot >= 0 ? 1 : (int)op.rows.size(); ph.cols = cols;
+        if (slot >= 0) ph.rows_dev = (const long long*)(dev->slots + slot);
+        else ph.dyn_off = P.dyn_put(op.rows.data(), op.rows.size() * 8);
+        P.phase(ph);
         q[i].done = true;
         return 1;
     }
@@ -497,16 +531,11 @@ struct Fuser {
     size_t try_argmax(size_t i) {
         if (!is(i, L_ARGMAX)) return 0;
         const LOp& op = q[i];
-        cc_device* d = dev;
-        const float* x = (const float*)op.a.buf->plane[0];
-        const int64_t n = vlen(op.a);
-        int64_t* slot = dev->slots + op.i0;
-        int64_t* hist = dev->history;
         const int64_t hidx = op.i1;
-        size_t off = P.dyn_put(&hidx, 8);
-        P.S(0x2007); P.SP(x); P.S((uint64_t)n); P.SP(slot); P.S(off);
-        P.steps.push_back([=](uint8_t* dyn_dev) { return cc_launch_argmax(d, x, n, slot, hist, (const int64_t*)(dyn_dev + off), -1); });
-        { MkPhase ph = {}; ph.type = MK_ARGMAX; ph.x = (float*)x; ph.n = (int)n; ph.dyn_off = off; ph.slot_dev = (long long*)slot; ph.hist_dev = (long long*)hist; P.phases.push_back(ph); }
+        MkPhase ph = new_phase(MK_ARGMAX);
+        ph.x = (float*)op.a.buf->plane[0]; ph.n = (int)vlen(op.a); ph.dyn_off = P.dyn_put(&hidx, 8);
+        ph.slot_dev = (long long*)(dev->slots + op.i0); ph.hist_dev = (long long*)dev->history;
+        P.phase(ph);
         q[i].done = true;
         return 1;
     }
@@ -516,27 +545,21 @@ struct Fuser {
     size_t try_sample(size_t i) {
         if (!is(i, L_SAMPLE)) return 0;
         const LOp& op = q[i];
-        cc_device* d = dev;
-        const float* x = (const float*)op.a.buf->plane[0];
-        const int64_t n = vlen(op.a);
-        int64_t* slot = dev->slots + op.i0;
-        int64_t* hist = dev->history;
-        void* scratch = dev->sample_scratch;            // sized for this queue before fusing (cc_lazy_flush)
         SampleDyn a;
         a.seed = (unsigned long long)op.rows[0]; a.coin_index = op.i2; a.hist_index = op.i1; a.temperature = op.f;
         const uint32_t pb = (uint32_t)op.rows[1]; memcpy(&a.topp, &pb, 4);
-        const size_t off = P.dyn_put(&a, sizeof(a));
-        P.S(0x2008); P.SP(x); P.S((uint64_t)n); P.SP(slot); P.S(off); P.SP(scratch);
-        P.steps.push_back([=](uint8_t* dyn_dev) { return cc_launch_sample(d, x, n, nullptr, (const SampleDyn*)(dyn_dev + off), slot, hist); });
-        { MkPhase ph = {}; ph.type = MK_SAMPLE; ph.x = (float*)x; ph.n = (int)n; ph.dyn_off = off; ph.slot_dev = (long long*)slot; ph.hist_dev = (long long*)hist;
-          ph.dst = scratch; P.phases.push_back(ph); }
+        MkPhase ph = new_phase(MK_SAMPLE);
+        ph.x = (float*)op.a.buf->plane[0]; ph.n = (int)vlen(op.a); ph.dyn_off = P.dyn_put(&a, sizeof(a));
+        ph.slot_dev = (long long*)(dev->slots + op.i0); ph.hist_dev = (long long*)dev->history;
+        ph.dst = dev->sample_scratch;                    // sized for this queue before fusing (cc_lazy_flush)
+        P.phase(ph);
         q[i].done = true;
         return 1;
     }
 
     // ---- pattern: K-quant matvecs (generic MATVEC phase of the megakernel) ----------------------------------------------------------------
     //   [[DUP] RMS_NORM MUL]  MATVEC{1..3, same K-quant type, same f32 row x, b = 1}  [SILU MUL | ADD]
-    // In the CUDA-graph mode (lazy = 1) these ops keep running as their eager kernels, in order (fallback steps); for the megakernel
+    // In the CUDA-graph mode (lazy = 1) these ops keep running as their eager kernels, in order (eager steps); for the megakernel
     // the whole group is ONE phase: fused prologue (norm + Q8_K quantisation of x) + T::row_dot rows + epilogue -- the same
     // arithmetic as the eager kernels, so the two modes agree bit for bit.
     size_t try_generic(size_t i) {
@@ -557,26 +580,24 @@ struct Fuser {
         const size_t end = j + g.used;
         // the normalised row is overwritten in place by the eager ops; the fused prologue never materialises it: nobody else may read it
         if (nm.len && !dead_after(xb, end)) return 0;
-        StreamArgs A = {};
+        for (size_t t = 0; t < g.n; t++) if (q[j + t].a.buf->cols != k) return 0;
+        MkPhase ph = new_phase(MK_MATVEC);
+        ph.wtype = wt; ph.act_type = CC_Q8_K;
+        StreamArgs& A = ph.mv;
         A.k = (int)k; A.epilogue = g.epilogue; A.residual[0] = g.residual[0] ? (const float*)g.residual[0]->plane[0] : nullptr;
         A.mats.n = (int)g.n;
         for (size_t t = 0; t < g.n; t++) {
             const cc_buf* w = q[j + t].a.buf;
-            if (w->cols != k) return 0;
             A.mats.qs[t] = w->plane[0]; A.mats.d[t] = (const uint16_t*)w->plane[1]; A.mats.p2[t] = w->plane[2]; A.mats.p3[t] = w->plane[3];
             A.mats.out[t] = (float*)q[j + t].out->base;
             A.mats.m[t] = (int)q[j + t].a.shape[0];
         }
-        MkPhase ph = {};
-        ph.type = MK_MATVEC; ph.wtype = wt; ph.act_type = CC_Q8_K; ph.mv = A;
         ph.x = (float*)xb->plane[0]; ph.orig = nm.orig ? (float*)nm.orig->base : nullptr; ph.eps = nm.eps; ph.n = (int)k;
         ph.norm_w = nm.len ? (const float*)nm.w->plane[0] : nullptr;
         ph.norm_ahead = nm.len && !written(nm.w);
-        // eager steps for the CUDA-graph mode, op by op, without disqualifying the megakernel form
-        covered_by_phase = true;
-        for (size_t t = i; t < end; t++) fallback(t);
-        covered_by_phase = false;
-        P.phases.push_back(ph);
+        // the CUDA-graph mode runs the group's ops as their eager kernels, in order; the phase covers them in the persistent kernel
+        P.phase(ph, false);
+        for (size_t t = i; t < end; t++) eager(t);
         return end - i;
     }
 
@@ -705,7 +726,7 @@ static int size_scratch(cc_device* dev, LazyState* lz) {
             score_need = std::max(score_need, (size_t)op.a.shape[0] * (size_t)(op.b.strides[0] / op.b.strides[2] + 1) * 4);
     if (score_need > lz->scores_cap) {
         cudaStreamSynchronize(dev->stream);
-        graph_cache_clear(lz);
+        graph_cache_clear(lz);                       // cached persistent-kernel graphs hold the old score rows
         cudaFree(lz->scores); lz->scores = nullptr; lz->scores_cap = 0;
         size_t cap = (size_t)1 << 20; while (cap < score_need) cap <<= 1;
         if (cudaMalloc(&lz->scores, cap) != cudaSuccess) return cc_fail(dev, CC_ERR_CUDA, "lazy: score scratch alloc failed");
@@ -734,8 +755,9 @@ static int upload_dyn(cc_device* dev, LazyState* lz, const Plan& P) {
     return rc;
 }
 
-static int run_steps(const Plan& P, uint8_t* dyn_dev) {
-    for (auto& st : P.steps) if (int r = st(dyn_dev)) return r;
+static int run_steps(cc_device* dev, const Plan& P, const std::vector<LOp>& q, const uint8_t* dyn_dev) {
+    for (const Plan::Step& st : P.steps)
+        if (int r = st.eager ? run_op(dev, q[st.at]) : launch_phase(dev, P.emitted[st.at], dyn_dev)) return r;
     return CC_OK;
 }
 
@@ -776,7 +798,7 @@ static int capture(cc_device* dev, LazyState* lz, Plan& P, uint64_t key, GraphCa
     if (!rc) {
         if (L.variant != MEGA_NONE && lz->prof_dev && P.phases.size() < 4000) { lz->prof_types.clear(); for (auto& ph : P.phases) lz->prof_types.push_back(ph.type * 16 + (ph.type == MK_MATVEC ? ph.mv.mats.n + 4 * ph.mv.epilogue + 1024 * (ph.mv.k >> 10) : 0)); }
         unsigned long long* prof = P.phases.size() < 4000 ? lz->prof_dev : nullptr;
-        if (L.variant == MEGA_NONE) rc = run_steps(P, lz->dyn_dev);
+        if (L.variant == MEGA_NONE) rc = run_steps(dev, P, lz->q, lz->dyn_dev);
         else if (L.variant == MEGA_RING) rc = cc_launch_mega_ring(dev, ge.phases_dev, (int)P.phases.size(), lz->dyn_dev, lz->bar_dev, L, prof, cc_comm_dev(dev));
         else rc = cc_launch_mega(dev, ge.phases_dev, (int)P.phases.size(), lz->dyn_dev, lz->bar_dev, L, prof);
         e = cudaStreamEndCapture(dev->stream, &graph);
@@ -814,7 +836,7 @@ int cc_lazy_flush(cc_device* dev) {
     if (rc) {
     } else if (!P.cacheable) {
         lz->uncached++;
-        rc = run_steps(P, lz->dyn_dev);
+        rc = run_steps(dev, P, lz->q, lz->dyn_dev);
     } else {
         P.S(P.dyn.size());
         uint64_t key = hash_sig(P.sig);

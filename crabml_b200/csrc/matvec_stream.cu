@@ -203,24 +203,9 @@ int cc_launch_matvec_stream(cc_device* dev, int type, const StreamArgs& A) {
     int64_t m_cat = A.epilogue == 2 ? A.mats.m[0] : (int64_t)A.mats.m[0] + (A.mats.n > 1 ? A.mats.m[1] : 0) + (A.mats.n > 2 ? A.mats.m[2] : 0);
     int64_t need = (m_cat + MS_WARPS - 1) / MS_WARPS;
     if (need < grid) grid = (int)(need > 0 ? need : 1);
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(grid);
-    cfg.blockDim = dim3(MS_THREADS);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = dev->stream;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    at[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = at;
-    cfg.numAttrs = dev->pdl ? 1 : 0;
-    cudaError_t e;
-    if (type == CC_Q8_0) {
-        if (smem > 48 * 1024) CC_CUDA(dev, cudaFuncSetAttribute(matvec_stream_kernel<CC_Q8_0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        e = cudaLaunchKernelEx(&cfg, matvec_stream_kernel<CC_Q8_0>, A, (const uint16_t*)dev->exp_lut);
-    } else {
-        if (smem > 48 * 1024) CC_CUDA(dev, cudaFuncSetAttribute(matvec_stream_kernel<CC_Q4_0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        e = cudaLaunchKernelEx(&cfg, matvec_stream_kernel<CC_Q4_0>, A, (const uint16_t*)dev->exp_lut);
-    }
+    auto kernel = type == CC_Q8_0 ? matvec_stream_kernel<CC_Q8_0> : matvec_stream_kernel<CC_Q4_0>;
+    if (smem > 48 * 1024) CC_CUDA(dev, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    cudaError_t e = launch_pdl(kernel, dim3(grid), dim3(MS_THREADS), smem, dev->stream, dev->pdl, A, (const uint16_t*)dev->exp_lut);
     if (e != cudaSuccess) return cc_fail(dev, CC_ERR_CUDA, "matvec_stream launch: %s", cudaGetErrorString(e));
     dev->launches++;
     return CC_OK;

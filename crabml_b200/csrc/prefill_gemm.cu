@@ -328,9 +328,7 @@ static int pg_weight_f16(cc_device* dev, const cc_buf* w, int64_t m, int64_t k, 
     void* dst = nullptr;
     if (cacheable) { CC_CUDA(dev, cudaMalloc(&dst, (size_t)m * k * 2)); }
     else { int rc = pg_ensure(dev, &s->w, &s->w_bytes, (size_t)m * k * 2); if (rc) return rc; dst = s->w; }
-    DeqPlanes pl;
-    for (int i = 0; i < CC_MAX_PLANES; i++) pl.p[i] = w->plane[i];
-    pl.cols = w->cols > 0 ? w->cols : k;
+    const DeqPlanes pl = cc_deq_planes(w, k);
     const int64_t n = m * k;
     dequant_w_f16_kernel<<<(unsigned)((n / 2 + 255) / 256), 256, 0, dev->stream>>>(w->dtype, pl, n, (__half*)dst);
     CC_LAUNCH_CHECK(dev);

@@ -130,15 +130,12 @@ __global__ void dequant_rows_kernel(int t, DeqPlanes P, const int64_t* rows, int
     if (dst_f32) dst_f32[i] = v; else dst_f16[i] = __float2half_rn(v);
 }
 
-int cc_launch_dequant_rows(cc_device* dev, const cc_buf* src, const int64_t* rows_dev, int n_rows, int64_t cols,
+int cc_launch_dequant_rows(cc_device* dev, const DeqPlanes& src, int src_dtype, const int64_t* rows_dev, int n_rows, int64_t cols,
                            void* dst, int dst_dtype) {
-    DeqPlanes P;
-    for (int i = 0; i < CC_MAX_PLANES; i++) P.p[i] = src->plane[i];
-    P.cols = src->cols > 0 ? src->cols : cols;
     int64_t total = (int64_t)n_rows * cols;
     if (total == 0) return CC_OK;
     dequant_rows_kernel<<<(unsigned)((total + 255) / 256), 256, 0, dev->stream>>>(
-        src->dtype, P, rows_dev, n_rows, cols, dst_dtype == CC_F32 ? (float*)dst : nullptr,
+        src_dtype, src, rows_dev, n_rows, cols, dst_dtype == CC_F32 ? (float*)dst : nullptr,
         dst_dtype == CC_F16 ? (__half*)dst : nullptr);
     CC_LAUNCH_CHECK(dev);
     return CC_OK;
