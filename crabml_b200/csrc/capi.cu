@@ -1,24 +1,7 @@
-// capi.cu -- extern "C" entry points: argument checks mirroring CpuTensor (cpu_tensor.rs:126-446) + launches.
-#include <string.h>
+// capi.cu -- extern "C" entry points: argument checks mirroring CpuTensor (cpu_tensor.rs:126-446), then one op record (op_record.cuh)
+// that eager mode runs at once and lazy mode queues.
+#include "op_record.cuh"
 
-#include "sample_dev.cuh"
-
-// ---- strider helpers (tensor/strider.rs) ------------------------------------------------------------------
-static int64_t view_len(const cc_view* v) {
-    int64_t n = 1;
-    for (int i = 0; i < v->ndim; i++) n *= v->shape[i];
-    return n;
-}
-static bool view_contiguous(const cc_view* v) {                      // strider.rs:182-206
-    if (v->ndim == 0) return true;
-    if (v->strides[v->ndim - 1] != 1) return false;
-    int64_t last = 1;
-    for (int i = v->ndim - 1; i >= 0; i--) {
-        if (last != v->strides[i]) return false;
-        last *= v->shape[i];
-    }
-    return true;
-}
 static bool view_ok(const cc_view* v) { return v && v->buf && v->ndim >= 1 && v->ndim <= CC_MAX_DIMS; }
 // highest element offset the view addresses (-1 for an empty view); negative strides / shapes are rejected by the caller
 static int64_t view_max_offset(const cc_view* v) {
@@ -49,10 +32,6 @@ static bool view_in_bounds(const cc_view* v) {
         CC_REQUIRE(dev, (v)->ndim == 2 && (v)->shape[1] == (v)->buf->cols && (v)->shape[0] <= (v)->buf->rows,                  \
                    "%s: view [%lld, %lld] does not match the quantized matrix [%lld, %lld]", what, (long long)(v)->shape[0],   \
                    (long long)((v)->ndim == 2 ? (v)->shape[1] : 0), (long long)(v)->buf->rows, (long long)(v)->buf->cols)
-// lazy mode (lazy.cu): after the same argument checks as eager mode the op is queued instead of launched
-enum { L_COPY_ROWS, L_DUP, L_RMS_NORM, L_MUL, L_ADD, L_SCALE, L_MATVEC, L_ROPE, L_CONCAT, L_CONTIGUOUS, L_BMM, L_SOFTMAX, L_SILU, L_GELU, L_ALLREDUCE, L_ALLGATHER, L_ARGMAX, L_SAMPLE };
-int cc_lazy_record(cc_device* dev, int kind, const cc_view* a, const cc_view* b, cc_buf* out, float f, int64_t i0, int64_t i1, int64_t i2,
-                   const int64_t* rows, int n_rows);
 #define LAZY(dev) ((dev)->lz != nullptr && !(dev)->exact)
 #define FLUSH(dev)                                  \
     do {                                            \
@@ -60,6 +39,134 @@ int cc_lazy_record(cc_device* dev, int kind, const cc_view* a, const cc_view* b,
     } while (0)
 
 #define REQUIRE_F32(dev, v, what) CC_REQUIRE(dev, (v)->buf->dtype == CC_F32, "%s: not f32, but got type %d", what, (v)->buf->dtype)
+
+// ---- one op's launch ----------------------------------------------------------------------------------------------------
+// fast-order matmul_vec of b rows of x: x quantised to the weight's partner type, then the streaming kernel (decode), the dense
+// tensor-core GEMM (prefill_gemm.cu) or the warp-per-row kernel.  The activation scratch only grows here when it is too small; lazy.cu
+// sizes it before any capture.
+static int launch_matmul_vec(cc_device* dev, const cc_buf* w, const float* xf, float* out, int64_t m, int64_t k, int64_t b) {
+    const int wt = w->dtype, at = cc_partner_type(wt);
+    const bool stream = b == 1 && cc_stream_supported(wt, k);
+    const bool dense = !stream && cc_prefill_supported(wt, m, k, b);
+    int rc = CC_OK;
+    if (at != CC_F32 && !(dense && at == CC_Q8_0)) {         // (the dense path quantises Q8_0 partners itself, fused with the f16 conversion)
+        rc = cc_ensure_act_scratch(dev, cc_act_bytes(at, b * k));
+        if (!rc) rc = cc_launch_quantize(dev, xf, b * k, at, dev->act_scratch);     // matmul_vec.rs:37-40
+    }
+    if (rc) return rc;
+    if (stream) return cc_launch_matvec_stream_plain(dev, w, dev->act_scratch, out, m, k);     // decode hot path
+    if (dense) return cc_launch_prefill_matmul(dev, w, dev->act_scratch, at == CC_Q8_0 ? xf : nullptr, out, m, k, b);
+    return cc_launch_matvec(dev, w, dev->act_scratch, xf, out, m, k, b);
+}
+
+// exact_order: reference-layout activation blocks + scalar-order dot on the GGUF-layout weights
+static int launch_matmul_vec_exact(cc_device* dev, const cc_buf* w, const float* xf, float* out, int64_t m, int64_t k, int64_t b) {
+    const int wt = w->dtype, at = cc_partner_type(wt);
+    int rc = CC_OK;
+    if (at != CC_F32) {
+        rc = cc_ensure_act_scratch(dev, cc_act_bytes(at, b * k));
+        if (!rc) rc = cc_launch_quantize(dev, xf, b * k, at, dev->act_scratch);     // matmul_vec.rs:37-40
+    }
+    const uint8_t* wraw = cc_is_quant(wt) ? w->raw : w->plane[0];
+    if (!rc && !wraw) rc = cc_fail(dev, CC_ERR_TENSOR, "matmul_vec(exact): weight has no GGUF-layout copy");
+    void* blocks = nullptr; size_t cls = 0;
+    if (!rc && (at == CC_Q8_0 || at == CC_Q8_1 || at == CC_Q8_K)) {
+        rc = cc_pool_alloc(dev, (size_t)(b * k / cc_block_elems(at)) * cc_block_bytes(at), &blocks, &cls);
+        if (!rc) rc = cc_launch_act_to_blocks(dev, dev->act_scratch, b * k, at, (uint8_t*)blocks);
+    }
+    const uint8_t* act = blocks ? (const uint8_t*)blocks : at == CC_F32 ? (const uint8_t*)xf : (const uint8_t*)dev->act_scratch;
+    if (!rc) rc = cc_launch_matvec_exact(dev, wt, wraw, act, out, m, k, b);
+    if (blocks) cc_pool_free(dev, blocks, cls);
+    return rc;
+}
+
+// The kernels of one checked op: every op of eager mode, and every op of lazy mode that no fused step takes.  An exact_order device
+// runs the reference's summation order where it differs from the fast one (exact.cu); lazy mode never runs on such a device.
+int cc_run_op(cc_device* d, const LOp& op) {
+    const cc_view &a = op.a, &b = op.b;
+    float* x = (float*)a.buf->plane[0];
+    switch (op.kind) {
+    case L_DUP: {
+        const int64_t n = view_len(&a);
+        if (n) CC_CUDA(d, cudaMemcpyAsync(op.out->base, a.buf->plane[0], (size_t)n * 4, cudaMemcpyDeviceToDevice, d->stream));
+        return CC_OK;
+    }
+    case L_CONTIGUOUS: {
+        int64_t dstr[CC_MAX_DIMS];
+        int64_t s = 1;
+        for (int i = a.ndim - 1; i >= 0; i--) { dstr[i] = s; s *= a.shape[i]; }
+        return cc_launch_strided_copy(d, a.buf->plane[0], a.buf->dtype, a.shape, a.strides, op.out->base, a.buf->dtype, dstr, 0, a.ndim);
+    }
+    case L_CONCAT:
+        return cc_launch_strided_copy(d, b.buf->plane[0], b.buf->dtype, b.shape, b.strides, a.buf->plane[0], a.buf->dtype, a.strides,
+                                      a.shape[op.i0] * a.strides[op.i0], a.ndim);
+    case L_COPY_ROWS: {
+        const int64_t cols = a.shape[a.ndim - 1];
+        if (op.i2 > 0)      // NOTE: the id in the slot was produced by argmax over this model's logits, i.e. it is < vocab rows by construction
+            return cc_launch_dequant_rows(d, cc_deq_planes(b.buf, cols), b.buf->dtype, d->slots + (op.i2 - 1), 1, cols, a.buf->plane[0], a.buf->dtype);
+        const size_t n = op.rows.size();
+        int rc = cc_ensure_dev_idx(d, n * 8);
+        if (rc) return rc;
+        CC_CUDA(d, cudaMemcpyAsync(d->dev_idx, op.rows.data(), n * 8, cudaMemcpyHostToDevice, d->stream));
+        return cc_launch_dequant_rows(d, cc_deq_planes(b.buf, cols), b.buf->dtype, (const int64_t*)d->dev_idx, (int)n, cols, a.buf->plane[0], a.buf->dtype);
+    }
+    case L_ROPE:
+        // cos/sin are evaluated on the host with the same libm calls as the reference (rope.rs:52-53,74-75) in both
+        // modes: bit-exact, and no slow large-argument device sinf/cosf
+        return cc_launch_rope_exact(d, x, op.i1, op.i2, a.shape[a.ndim - 1], (int)op.f, op.i0, op.rows[0]);
+    case L_RMS_NORM: {
+        const int64_t rows = a.ndim == 1 ? 1 : a.shape[0], cols = a.shape[a.ndim - 1];
+        return d->exact ? cc_launch_rms_norm_exact(d, x, rows, cols, op.f) : cc_launch_rms_norm(d, x, rows, cols, op.f);
+    }
+    case L_SOFTMAX: {
+        const int64_t cols = a.shape[a.ndim - 1], rows = cols ? view_len(&a) / cols : 0;
+        return d->exact ? cc_launch_softmax_exact(d, x, rows, cols) : cc_launch_softmax(d, x, rows, cols);
+    }
+    case L_SILU: return cc_launch_silu(d, x, view_len(&a));
+    case L_GELU: return cc_launch_gelu(d, x, view_len(&a));
+    case L_MUL: return cc_launch_binary(d, x, op.i0, (const float*)b.buf->plane[0], op.i1, 1);
+    case L_ADD: return cc_launch_binary(d, x, op.i0, (const float*)b.buf->plane[0], op.i1, 0);
+    case L_SCALE: return cc_launch_scale(d, x, view_len(&a), op.f);
+    case L_ALLREDUCE: return cc_launch_all_reduce(d, x, op.i0, nullptr);
+    case L_ALLGATHER: return cc_launch_all_gather(d, (const float*)b.buf->plane[0], op.i0, x);
+    case L_ARGMAX: return cc_launch_argmax(d, x, view_len(&a), d->slots + op.i0, d->history, nullptr, op.i1);
+    case L_SAMPLE: {
+        int rc = cc_ensure_sample_scratch(d, view_len(&a));
+        if (rc) return rc;
+        const SampleDyn s = cc_sample_dyn(op);
+        return cc_launch_sample(d, x, view_len(&a), &s, nullptr, d->slots + op.i0, d->history);
+    }
+    case L_MATVEC: {
+        const float* xf = (const float*)b.buf->plane[0];
+        const int64_t rows = b.ndim == 1 ? 1 : b.shape[0];
+        if (d->exact) return launch_matmul_vec_exact(d, a.buf, xf, (float*)op.out->base, a.shape[0], a.shape[1], rows);
+        return launch_matmul_vec(d, a.buf, xf, (float*)op.out->base, a.shape[0], a.shape[1], rows);
+    }
+    case L_BMM:
+        if (d->exact && b.strides[1] == 1)
+            return cc_launch_bmm_kcontig_exact(d, x, b.buf->plane[0], b.buf->dtype, (float*)op.out->base, a.shape[0], b.shape[0], a.shape[1],
+                                               a.shape[2], b.shape[2], b.strides[0], b.strides[2]);
+        return cc_launch_batch_matmul(d, x, b.buf->plane[0], b.buf->dtype, (float*)op.out->base, a.shape[0], b.shape[0], a.shape[1], a.shape[2],
+                                      b.shape[2], b.strides[0], b.strides[1], b.strides[2]);
+    }
+    return cc_fail(d, CC_ERR_UNSUPPORTED, "unknown op kind %d", op.kind);
+}
+
+// lazy mode queues a checked op (lazy.cu), eager mode runs it now.  An op with a result (out != NULL) gets a new activation of out_elems
+// elements as op.out: *out receives it on success, and it is released on failure.
+static int submit(cc_device* dev, LOp op, cc_buf** out = nullptr, int64_t out_elems = 0, int out_type = CC_F32) {
+    if (out) {
+        int rc = cc_new_activation(dev, out_elems, out_type, false, &op.out);
+        if (rc) return rc;
+    }
+    cc_buf* result = op.out;
+    const int rc = LAZY(dev) ? cc_lazy_record(dev, std::move(op)) : cc_run_op(dev, op);
+    if (out) {
+        if (rc) cc_tensor_release(result);
+        else *out = result;
+    }
+    return rc;
+}
 
 // ---- dup / export / contiguous ----------------------------------------------------------------------------------
 extern "C" CC_API int cc_tensor_dup(cc_device* dev, const cc_view* src, cc_buf** out) {     // cpu_tensor.rs:333-337
@@ -69,13 +176,7 @@ extern "C" CC_API int cc_tensor_dup(cc_device* dev, const cc_view* src, cc_buf**
     // the reference copies the WHOLE buffer (iter_f32) and gives it the view's shape
     int64_t n = view_len(src);
     CC_REQUIRE(dev, n == src->buf->nelems || view_contiguous(src), "dup: shape does not cover the buffer");
-    cc_buf* b = nullptr;
-    int rc = cc_new_activation(dev, n, CC_F32, false, &b);
-    if (rc) return rc;
-    *out = b;
-    if (LAZY(dev)) return cc_lazy_record(dev, L_DUP, src, nullptr, b, 0, 0, 0, 0, nullptr, 0);
-    if (n) CC_CUDA(dev, cudaMemcpyAsync(b->base, src->buf->plane[0], (size_t)n * 4, cudaMemcpyDeviceToDevice, dev->stream));
-    return CC_OK;
+    return submit(dev, LOp{.kind = L_DUP, .a = *src}, out, n);
 }
 
 extern "C" CC_API int cc_tensor_export_f32(cc_device* dev, const cc_view* src, float* dst, size_t n) {   // cpu_tensor.rs:339-349
@@ -102,18 +203,7 @@ extern "C" CC_API int cc_contiguous(cc_device* dev, const cc_view* src, cc_buf**
     int t = src->buf->dtype;
     CC_REQUIRE(dev, t == CC_F32 || t == CC_F16, "contiguous: only f32/f16");
     CC_REQUIRE(dev, src->ndim == 2 || src->ndim == 3, "contiguous: only 2d/3d tensors");
-    int64_t n = view_len(src);
-    cc_buf* b = nullptr;
-    int rc = cc_new_activation(dev, n, t, false, &b);
-    if (rc) return rc;
-    int64_t dstr[CC_MAX_DIMS];
-    int64_t s = 1;
-    for (int i = src->ndim - 1; i >= 0; i--) { dstr[i] = s; s *= src->shape[i]; }
-    if (LAZY(dev)) { *out = b; return cc_lazy_record(dev, L_CONTIGUOUS, src, nullptr, b, 0, 0, 0, 0, nullptr, 0); }
-    rc = cc_launch_strided_copy(dev, src->buf->plane[0], t, src->shape, src->strides, b->base, t, dstr, 0, src->ndim);
-    if (rc) { cc_tensor_release(b); return rc; }
-    *out = b;
-    return CC_OK;
+    return submit(dev, LOp{.kind = L_CONTIGUOUS, .a = *src}, out, view_len(src), t);
 }
 
 // ---- concatenate: cpu_tensor.rs:251-292 ------------------------------------------------------------------------------
@@ -135,9 +225,7 @@ extern "C" CC_API int cc_concatenate(cc_device* dev, const cc_view* self, const 
         if (top >= 0) hi += top * self->strides[i];
     }
     CC_REQUIRE(dev, view_len(rhs) == 0 || hi < self->buf->nelems, "concatenate: exceeds the pre-allocated storage");
-    if (LAZY(dev)) return cc_lazy_record(dev, L_CONCAT, self, rhs, nullptr, 0, axis, 0, 0, nullptr, 0);
-    return cc_launch_strided_copy(dev, rhs->buf->plane[0], t2, rhs->shape, rhs->strides, self->buf->plane[0], t1,
-                                  self->strides, self->shape[axis] * self->strides[axis], self->ndim);
+    return submit(dev, LOp{.kind = L_CONCAT, .a = *self, .b = *rhs, .i0 = axis});
 }
 
 // ---- copy_rows_from: cpu_tensor.rs:306-331 ----------------------------------------------------------------------------
@@ -160,14 +248,7 @@ extern "C" CC_API int cc_copy_rows_from(cc_device* dev, const cc_view* dst, cons
     for (int i = 0; i < n_rows; i++)
         CC_REQUIRE(dev, rows[i] >= 0 && (rows[i] + 1) * cols <= src_len, "copy_rows_from: row %lld out of range", (long long)rows[i]);
     if (n_rows == 0) return CC_OK;
-    if (LAZY(dev)) return cc_lazy_record(dev, L_COPY_ROWS, dst, src, nullptr, 0, 0, 0, 0, rows, n_rows);
-    int rc = cc_ensure_dev_idx(dev, (size_t)n_rows * 8);
-    if (rc) return rc;
-    rc = cc_ensure_pinned(dev, (size_t)n_rows * 8);
-    if (rc) return rc;
-    // pinned staging slot may still be read by an earlier async copy: keep it simple and synchronous w.r.t. the stream
-    CC_CUDA(dev, cudaMemcpyAsync(dev->dev_idx, rows, (size_t)n_rows * 8, cudaMemcpyHostToDevice, dev->stream));
-    return cc_launch_dequant_rows(dev, cc_deq_planes(src->buf, cols), src->buf->dtype, (const int64_t*)dev->dev_idx, n_rows, cols, dst->buf->plane[0], dt);
+    return submit(dev, LOp{.kind = L_COPY_ROWS, .a = *dst, .b = *src, .rows = std::vector<int64_t>(rows, rows + n_rows)});
 }
 
 // ---- in-place ops -------------------------------------------------------------------------------------------------------
@@ -181,10 +262,7 @@ extern "C" CC_API int cc_rope_inplace(cc_device* dev, const cc_view* x, int32_t 
     if (x->ndim == 2) { n_batch = 1; stride = view_len(x); hd = x->shape[1]; }
     else { n_batch = x->shape[0]; stride = x->strides[0]; hd = x->shape[2]; }
     CC_REQUIRE(dev, rope_dims >= 0 && rope_dims <= hd && rope_dims % 2 == 0, "rope_inplace: bad rope_dims %lld", (long long)rope_dims);
-    if (LAZY(dev)) return cc_lazy_record(dev, L_ROPE, x, nullptr, nullptr, (float)mode, pos, n_batch, stride, &rope_dims, 1);
-    // cos/sin are evaluated on the host with the same libm calls as the reference (rope.rs:52-53,74-75) in both
-    // modes: bit-exact, and no slow large-argument device sinf/cosf
-    return cc_launch_rope_exact(dev, (float*)x->buf->plane[0], n_batch, stride, hd, mode, pos, rope_dims);
+    return submit(dev, LOp{.kind = L_ROPE, .a = *x, .f = (float)mode, .i0 = pos, .i1 = n_batch, .i2 = stride, .rows = {rope_dims}});
 }
 
 extern "C" CC_API int cc_rms_norm_inplace(cc_device* dev, const cc_view* x, float eps) {    // rms_norm.rs:9-30
@@ -192,11 +270,9 @@ extern "C" CC_API int cc_rms_norm_inplace(cc_device* dev, const cc_view* x, floa
     CC_REQUIRE(dev, view_contiguous(x), "rms_norm_inplace: not contiguous");
     CC_REQUIRE(dev, x->ndim == 1 || x->ndim == 2, "rms_norm_inplace: only 1d/2d tensors");
     REQUIRE_F32(dev, x, "rms_norm_inplace");
-    int64_t rows = x->ndim == 1 ? 1 : x->shape[0], cols = x->ndim == 1 ? x->shape[0] : x->shape[1];
+    int64_t cols = x->shape[x->ndim - 1];
     CC_REQUIRE(dev, cols % 32 == 0, "rms_norm_inplace: length %lld %% 32 != 0", (long long)cols);   // rms_norm.rs:34
-    if (LAZY(dev)) return cc_lazy_record(dev, L_RMS_NORM, x, nullptr, nullptr, eps, 0, 0, 0, nullptr, 0);
-    if (dev->exact) return cc_launch_rms_norm_exact(dev, (float*)x->buf->plane[0], rows, cols, eps);
-    return cc_launch_rms_norm(dev, (float*)x->buf->plane[0], rows, cols, eps);
+    return submit(dev, LOp{.kind = L_RMS_NORM, .a = *x, .f = eps});
 }
 
 extern "C" CC_API int cc_softmax_inplace(cc_device* dev, const cc_view* x, int32_t axis) {  // softmax.rs:11-37
@@ -205,26 +281,21 @@ extern "C" CC_API int cc_softmax_inplace(cc_device* dev, const cc_view* x, int32
     CC_REQUIRE(dev, view_contiguous(x), "softmax_inplace: not contiguous");
     REQUIRE_F32(dev, x, "softmax_inplace");
     CC_REQUIRE(dev, axis == x->ndim - 1, "only axis=%d is supported on a %d dimensions tensor", x->ndim - 1, x->ndim);
-    int64_t cols = x->shape[x->ndim - 1];
-    if (LAZY(dev)) return cc_lazy_record(dev, L_SOFTMAX, x, nullptr, nullptr, 0, 0, 0, 0, nullptr, 0);
-    if (dev->exact) return cc_launch_softmax_exact(dev, (float*)x->buf->plane[0], cols ? view_len(x) / cols : 0, cols);
-    return cc_launch_softmax(dev, (float*)x->buf->plane[0], cols ? view_len(x) / cols : 0, cols);
+    return submit(dev, LOp{.kind = L_SOFTMAX, .a = *x});
 }
 
 extern "C" CC_API int cc_silu_inplace(cc_device* dev, const cc_view* x) {                   // silu.rs:6-13: whole buffer
     CHECK_VIEW(dev, x, "silu_inplace");
     REQUIRE_F32(dev, x, "silu_inplace");
-    if (LAZY(dev)) return cc_lazy_record(dev, L_SILU, x, nullptr, nullptr, 0, 0, 0, 0, nullptr, 0);
-    return cc_launch_silu(dev, (float*)x->buf->plane[0], view_len(x));
+    return submit(dev, LOp{.kind = L_SILU, .a = *x});
 }
 extern "C" CC_API int cc_gelu_inplace(cc_device* dev, const cc_view* x) {                   // gelu.rs:10-15
     CHECK_VIEW(dev, x, "gelu_inplace");
     REQUIRE_F32(dev, x, "gelu_inplace");
-    if (LAZY(dev)) return cc_lazy_record(dev, L_GELU, x, nullptr, nullptr, 0, 0, 0, 0, nullptr, 0);
-    return cc_launch_gelu(dev, (float*)x->buf->plane[0], view_len(x));
+    return submit(dev, LOp{.kind = L_GELU, .a = *x});
 }
 
-static int binary(cc_device* dev, const cc_view* x, const cc_view* rhs, int op, const char* what) {   // arithmetic.rs:5-68
+static int binary(cc_device* dev, const cc_view* x, const cc_view* rhs, int kind, const char* what) {   // arithmetic.rs:5-68
     CHECK_VIEW(dev, x, what);
     CHECK_VIEW(dev, rhs, what);
     REQUIRE_F32(dev, x, what);
@@ -238,17 +309,15 @@ static int binary(cc_device* dev, const cc_view* x, const cc_view* rhs, int op, 
         ny -= ny % 4;
         if (ny == 0) return CC_OK;
     }
-    if (LAZY(dev)) return cc_lazy_record(dev, op == 1 ? L_MUL : L_ADD, x, rhs, nullptr, 0, n, ny, 0, nullptr, 0);
-    return cc_launch_binary(dev, (float*)x->buf->plane[0], n, (const float*)rhs->buf->plane[0], ny, op);
+    return submit(dev, LOp{.kind = kind, .a = *x, .b = *rhs, .i0 = n, .i1 = ny});
 }
-extern "C" CC_API int cc_mul_inplace(cc_device* dev, const cc_view* x, const cc_view* rhs) { return binary(dev, x, rhs, 1, "mul_inplace"); }
-extern "C" CC_API int cc_add_inplace(cc_device* dev, const cc_view* x, const cc_view* rhs) { return binary(dev, x, rhs, 0, "add_inplace"); }
+extern "C" CC_API int cc_mul_inplace(cc_device* dev, const cc_view* x, const cc_view* rhs) { return binary(dev, x, rhs, L_MUL, "mul_inplace"); }
+extern "C" CC_API int cc_add_inplace(cc_device* dev, const cc_view* x, const cc_view* rhs) { return binary(dev, x, rhs, L_ADD, "add_inplace"); }
 extern "C" CC_API int cc_scale_inplace(cc_device* dev, const cc_view* x, float rhs) {
     CHECK_VIEW(dev, x, "scale_inplace");
     REQUIRE_F32(dev, x, "scale_inplace");
     CC_REQUIRE(dev, view_contiguous(x), "scale_inplace: not contiguous");
-    if (LAZY(dev)) return cc_lazy_record(dev, L_SCALE, x, nullptr, nullptr, rhs, 0, 0, 0, nullptr, 0);
-    return cc_launch_scale(dev, (float*)x->buf->plane[0], view_len(x), rhs);
+    return submit(dev, LOp{.kind = L_SCALE, .a = *x, .f = rhs});
 }
 
 // ---- exchange step of the sharded path (comm.cu) ------------------------------------------------------------------------
@@ -259,8 +328,7 @@ extern "C" CC_API int cc_all_reduce_sum_inplace(cc_device* dev, const cc_view* x
     CC_REQUIRE(dev, dev->comm, "all_reduce_sum_inplace: no communicator on this device");
     const int64_t n = view_len(x);
     CC_REQUIRE(dev, n % 4 == 0 && n <= CC_COMM_MAX_ELEMS, "all_reduce_sum_inplace: %lld elements unsupported", (long long)n);
-    if (LAZY(dev)) return cc_lazy_record(dev, L_ALLREDUCE, x, nullptr, nullptr, 0, n, 0, 0, nullptr, 0);
-    return cc_launch_all_reduce(dev, (float*)x->buf->plane[0], n, nullptr);
+    return submit(dev, LOp{.kind = L_ALLREDUCE, .a = *x, .i0 = n});
 }
 extern "C" CC_API int cc_all_gather(cc_device* dev, const cc_view* dst, const cc_view* src) {
     CHECK_VIEW(dev, dst, "all_gather dst");
@@ -272,8 +340,7 @@ extern "C" CC_API int cc_all_gather(cc_device* dev, const cc_view* dst, const cc
     const int64_t n = view_len(src);
     CC_REQUIRE(dev, view_len(dst) == n * cc_comm_world(dev), "all_gather: dst has %lld elements, want %lld x %d", (long long)view_len(dst), (long long)n, cc_comm_world(dev));
     CC_REQUIRE(dev, n % 4 == 0 && n <= CC_COMM_MAX_ELEMS, "all_gather: %lld elements per rank unsupported", (long long)n);
-    if (LAZY(dev)) return cc_lazy_record(dev, L_ALLGATHER, dst, src, nullptr, 0, n, 0, 0, nullptr, 0);
-    return cc_launch_all_gather(dev, (const float*)src->buf->plane[0], n, (float*)dst->buf->plane[0]);
+    return submit(dev, LOp{.kind = L_ALLGATHER, .a = *dst, .b = *src, .i0 = n});
 }
 
 // ---- greedy decoding without a host round trip per token (extension: not part of the reference's trait) ---------------------------------
@@ -287,8 +354,7 @@ extern "C" CC_API int cc_argmax_to_slot(cc_device* dev, const cc_view* x, int32_
     CC_REQUIRE(dev, slot >= 0 && slot < CC_N_SLOTS && hist_index < CC_HISTORY_CAP, "argmax_to_slot: slot %d / history index %lld out of range", slot, (long long)hist_index);
     int rc = cc_ensure_slots(dev);
     if (rc) return rc;
-    if (LAZY(dev)) return cc_lazy_record(dev, L_ARGMAX, x, nullptr, nullptr, 0, slot, hist_index, 0, nullptr, 0);
-    return cc_launch_argmax(dev, (const float*)x->buf->plane[0], view_len(x), dev->slots + slot, dev->history, nullptr, hist_index);
+    return submit(dev, LOp{.kind = L_ARGMAX, .a = *x, .i0 = slot, .i1 = hist_index});
 }
 // Temperature + top-p sampling into a slot (sampler.rs:27-107; sample_dev.cuh).  coin = 24 bits of splitmix64(seed ^
 // splitmix64(coin_index)) / 2^24, so one seed reproduces one run in every mode.  temperature 0 is cc_argmax_to_slot (same op, same bits).
@@ -305,16 +371,9 @@ extern "C" CC_API int cc_sample_to_slot(cc_device* dev, const cc_view* x, float 
     if (temperature == 0.0f) return cc_argmax_to_slot(dev, x, slot, hist_index);        // sampler.rs:28-30
     int rc = cc_ensure_slots(dev);
     if (rc) return rc;
-    if (LAZY(dev)) {
-        uint32_t pb; memcpy(&pb, &topp, 4);
-        const int64_t extra[2] = {(int64_t)seed, (int64_t)pb};
-        return cc_lazy_record(dev, L_SAMPLE, x, nullptr, nullptr, temperature, slot, hist_index, coin_index, extra, 2);
-    }
-    rc = cc_ensure_sample_scratch(dev, view_len(x));
-    if (rc) return rc;
-    SampleDyn a;
-    a.seed = seed; a.coin_index = coin_index; a.hist_index = hist_index; a.temperature = temperature; a.topp = topp;
-    return cc_launch_sample(dev, (const float*)x->buf->plane[0], view_len(x), &a, nullptr, dev->slots + slot, dev->history);
+    uint32_t pb;
+    memcpy(&pb, &topp, 4);
+    return submit(dev, LOp{.kind = L_SAMPLE, .a = *x, .f = temperature, .i0 = slot, .i1 = hist_index, .i2 = coin_index, .rows = {(int64_t)seed, (int64_t)pb}});
 }
 // copy_rows_from with ONE row whose index is the content of a device slot
 extern "C" CC_API int cc_copy_rows_from_slot(cc_device* dev, const cc_view* dst, const cc_view* src, int32_t slot) {
@@ -331,9 +390,7 @@ extern "C" CC_API int cc_copy_rows_from_slot(cc_device* dev, const cc_view* dst,
     CC_REQUIRE(dev, !cc_is_quant(src->buf->dtype) || cols == src->buf->cols, "copy_rows_from_slot: row length does not match the quantized matrix");
     int rc = cc_ensure_slots(dev);
     if (rc) return rc;
-    if (LAZY(dev)) return cc_lazy_record(dev, L_COPY_ROWS, dst, src, nullptr, 0, 0, 0, slot + 1, nullptr, 0);
-    // NOTE: the id in the slot was produced by argmax over this model's logits, i.e. it is < vocab rows by construction
-    return cc_launch_dequant_rows(dev, cc_deq_planes(src->buf, cols), src->buf->dtype, dev->slots + slot, 1, cols, dst->buf->plane[0], dt);
+    return submit(dev, LOp{.kind = L_COPY_ROWS, .a = *dst, .b = *src, .i2 = slot + 1});
 }
 extern "C" CC_API int cc_slot_set(cc_device* dev, int32_t slot, int64_t value) {
     if (!dev) return CC_ERR_ARG;
@@ -384,24 +441,6 @@ extern "C" CC_API void cc_host_free(cc_device* dev, void* p) {
     cudaFreeHost(p);
 }
 
-// fast-order matmul_vec of b rows of x (eager calls, and the lazy fallback step in lazy.cu): x quantised to the weight's partner type,
-// then the streaming kernel (decode), the dense tensor-core GEMM (prefill_gemm.cu) or the warp-per-row kernel.  The activation scratch
-// only grows here when it is too small; lazy.cu sizes it before any capture.
-int cc_launch_matmul_vec(cc_device* dev, const cc_buf* w, const float* xf, float* out, int64_t m, int64_t k, int64_t b) {
-    const int wt = w->dtype, at = cc_partner_type(wt);
-    const bool stream = b == 1 && cc_stream_supported(wt, k);
-    const bool dense = !stream && cc_prefill_supported(wt, m, k, b);
-    int rc = CC_OK;
-    if (at != CC_F32 && !(dense && at == CC_Q8_0)) {         // (the dense path quantises Q8_0 partners itself, fused with the f16 conversion)
-        rc = cc_ensure_act_scratch(dev, cc_act_bytes(at, b * k));
-        if (!rc) rc = cc_launch_quantize(dev, xf, b * k, at, dev->act_scratch);     // matmul_vec.rs:37-40
-    }
-    if (rc) return rc;
-    if (stream) return cc_launch_matvec_stream_plain(dev, w, dev->act_scratch, out, m, k);     // decode hot path
-    if (dense) return cc_launch_prefill_matmul(dev, w, dev->act_scratch, at == CC_Q8_0 ? xf : nullptr, out, m, k, b);
-    return cc_launch_matvec(dev, w, dev->act_scratch, xf, out, m, k, b);
-}
-
 // ---- matmul_vec: cpu_tensor.rs:371-386 + primitives/matmul_vec.rs:9-78 -------------------------------------------------
 extern "C" CC_API int cc_matmul_vec(cc_device* dev, const cc_view* w, const cc_view* x, cc_buf** out) {
     CHECK_VIEW(dev, w, "matmul_vec");
@@ -419,31 +458,7 @@ extern "C" CC_API int cc_matmul_vec(cc_device* dev, const cc_view* w, const cc_v
     CC_REQUIRE(dev, at >= 0, "matmul_vec: unsupported weight type %d", wt);
     CC_REQUIRE(dev, k % cc_block_elems(at) == 0, "matmul_vec: k=%lld is not a multiple of the %d-element activation block",
                (long long)k, cc_block_elems(at));
-    cc_buf* c = nullptr;
-    int rc = cc_new_activation(dev, b * m, CC_F32, false, &c);
-    if (rc) return rc;
-    if (LAZY(dev)) { *out = c; return cc_lazy_record(dev, L_MATVEC, w, x, c, 0, 0, 0, 0, nullptr, 0); }
-    const float* xf = (const float*)x->buf->plane[0];
-    if (dev->exact) {
-        // exact_order: reference-layout activation blocks + scalar-order dot on the GGUF-layout weights
-        if (at != CC_F32) {
-            rc = cc_ensure_act_scratch(dev, cc_act_bytes(at, b * k));
-            if (!rc) rc = cc_launch_quantize(dev, xf, b * k, at, dev->act_scratch);     // matmul_vec.rs:37-40
-        }
-        const uint8_t* wraw = cc_is_quant(wt) ? w->buf->raw : w->buf->plane[0];
-        if (!rc && !wraw) rc = cc_fail(dev, CC_ERR_TENSOR, "matmul_vec(exact): weight has no GGUF-layout copy");
-        void* blocks = nullptr; size_t cls = 0;
-        if (!rc && (at == CC_Q8_0 || at == CC_Q8_1 || at == CC_Q8_K)) {
-            rc = cc_pool_alloc(dev, (size_t)(b * k / cc_block_elems(at)) * cc_block_bytes(at), &blocks, &cls);
-            if (!rc) rc = cc_launch_act_to_blocks(dev, dev->act_scratch, b * k, at, (uint8_t*)blocks);
-        }
-        const uint8_t* act = blocks ? (const uint8_t*)blocks : at == CC_F32 ? (const uint8_t*)xf : (const uint8_t*)dev->act_scratch;
-        if (!rc) rc = cc_launch_matvec_exact(dev, wt, wraw, act, (float*)c->base, m, k, b);
-        if (blocks) cc_pool_free(dev, blocks, cls);
-    } else rc = cc_launch_matmul_vec(dev, w->buf, xf, (float*)c->base, m, k, b);
-    if (rc) { cc_tensor_release(c); return rc; }
-    *out = c;
-    return CC_OK;
+    return submit(dev, LOp{.kind = L_MATVEC, .a = *w, .b = *x}, out, b * m);
 }
 
 // ---- batch_matmul: cpu_tensor.rs:352-366 + primitives/batch_matmul.rs:15-45 --------------------------------------------
@@ -461,19 +476,7 @@ extern "C" CC_API int cc_batch_matmul(cc_device* dev, const cc_view* a, const cc
     CC_REQUIRE(dev, b->shape[1] == k, "batch_matmul: inner dims differ");
     CC_REQUIRE(dev, bb > 0 && ab >= bb && ab % bb == 0, "batch_matmul: lhs batch %lld is not a multiple of rhs batch %lld",
                (long long)ab, (long long)bb);
-    cc_buf* c = nullptr;
-    int rc = cc_new_activation(dev, ab * m * n, CC_F32, false, &c);
-    if (rc) return rc;
-    if (LAZY(dev)) { *out = c; return cc_lazy_record(dev, L_BMM, a, b, c, 0, 0, 0, 0, nullptr, 0); }
-    if (dev->exact && b->strides[1] == 1)
-        rc = cc_launch_bmm_kcontig_exact(dev, (const float*)a->buf->plane[0], b->buf->plane[0], bt, (float*)c->base, ab, bb, m, k, n,
-                                         b->strides[0], b->strides[2]);
-    else
-        rc = cc_launch_batch_matmul(dev, (const float*)a->buf->plane[0], b->buf->plane[0], bt, (float*)c->base, ab, bb, m, k, n,
-                                    b->strides[0], b->strides[1], b->strides[2]);
-    if (rc) { cc_tensor_release(c); return rc; }
-    *out = c;
-    return CC_OK;
+    return submit(dev, LOp{.kind = L_BMM, .a = *a, .b = *b}, out, ab * m * n);
 }
 
 // ---- debug tap: cpu_tensor.rs:232-241 -------------------------------------------------------------------------------------

@@ -117,9 +117,6 @@ struct cc_device {
     std::unordered_map<size_t, std::set<uintptr_t>> free_lists;   // per size class, ordered: allocation takes the LOWEST free address
     size_t pool_live_bytes = 0;
 
-    // pinned staging for export / row indices
-    void* pinned = nullptr;
-    size_t pinned_bytes = 0;
     void* dev_idx = nullptr;      // device copy of row indices
     size_t dev_idx_bytes = 0;
 
@@ -216,7 +213,6 @@ int cc_pool_alloc(cc_device* dev, size_t bytes, void** out, size_t* cls);
 void cc_pool_free(cc_device* dev, void* p, size_t cls);
 int cc_new_activation(cc_device* dev, int64_t nelems, int dtype, bool zero, cc_buf** out);
 int cc_ensure_act_scratch(cc_device* dev, size_t bytes);
-int cc_ensure_pinned(cc_device* dev, size_t bytes);
 int cc_ensure_dev_idx(cc_device* dev, size_t bytes);
 
 // ---- repack.cu -----------------------------------------------------------------------------------
@@ -373,7 +369,6 @@ bool cc_stream_supported(int type, int64_t k);
 bool cc_mega_generic_supported(int type, int64_t k);      // K-quant weights: generic MATVEC phase of the megakernel (mega.cu)
 int cc_launch_matvec_stream(cc_device* dev, int type, const StreamArgs& A);
 int cc_launch_matvec_stream_plain(cc_device* dev, const cc_buf* w, const void* act, float* out, int64_t m, int64_t k);
-int cc_launch_matmul_vec(cc_device* dev, const cc_buf* w, const float* x, float* out, int64_t m, int64_t k, int64_t b);     // capi.cu
 
 // ---- exact.cu (exact_order verification mode) -------------------------------------------------------
 int cc_launch_matvec_exact(cc_device* dev, int t, const uint8_t* w_gguf, const uint8_t* act_blocks, float* out,

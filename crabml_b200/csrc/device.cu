@@ -95,7 +95,7 @@ extern "C" CC_API int cc_device_create(const cc_device_options* opts, cc_device*
     // scratch buffers are sized once for every realistic row (k up to 1M elements): growing them later means cudaFree, which waits
     // for EVERY kernel of the context -- with several devices of one process on one GPU (in-process ranks) a peer may be spinning
     // on this rank's exchange at that moment
-    if (cc_ensure_act_scratch(dev, (size_t)4 << 20) != CC_OK || cc_ensure_pinned(dev, (size_t)64 << 10) != CC_OK || cc_ensure_dev_idx(dev, (size_t)64 << 10) != CC_OK) {
+    if (cc_ensure_act_scratch(dev, (size_t)4 << 20) != CC_OK || cc_ensure_dev_idx(dev, (size_t)64 << 10) != CC_OK) {
         delete dev;
         return CC_ERR_CUDA;
     }
@@ -117,7 +117,6 @@ extern "C" CC_API void cc_device_destroy(cc_device* dev) {
     for (auto& kv : dev->free_lists)
         for (uintptr_t p : kv.second) cudaFree((void*)p);
     if (dev->act_scratch) cudaFree(dev->act_scratch);
-    if (dev->pinned) cudaFreeHost(dev->pinned);
     for (int i = 0; i < 2; i++) { if (dev->up_pinned[i]) cudaFreeHost(dev->up_pinned[i]); if (dev->up_ev[i]) cudaEventDestroy(dev->up_ev[i]); }
     if (dev->err_host) cudaFreeHost(dev->err_host);
     if (dev->err_dev) cudaFree(dev->err_dev);
@@ -243,14 +242,6 @@ int cc_ensure_act_scratch(cc_device* dev, size_t bytes) {
     size_t nb = size_class(bytes);
     CC_CUDA(dev, cudaMalloc(&dev->act_scratch, nb));
     dev->act_scratch_bytes = nb;
-    return CC_OK;
-}
-int cc_ensure_pinned(cc_device* dev, size_t bytes) {
-    if (bytes <= dev->pinned_bytes) return CC_OK;
-    if (dev->pinned) { CC_CUDA(dev, cudaStreamSynchronize(dev->stream)); CC_CUDA(dev, cudaFreeHost(dev->pinned)); }
-    size_t nb = size_class(bytes);
-    CC_CUDA(dev, cudaMallocHost(&dev->pinned, nb));
-    dev->pinned_bytes = nb;
     return CC_OK;
 }
 int cc_ensure_dev_idx(cc_device* dev, size_t bytes) {

@@ -6,7 +6,7 @@
 // needs a result on the host (export / debug tap / synchronize -- the reference synchronises only there too, llama2.rs:209):
 //   1. fuse: runs of ops that match the Llama decode layer (llama2.rs:226-269, 527-638) are replaced by fused steps, each described by
 //      one phase descriptor (MkPhase) that the persistent kernels run and the CUDA-graph mode launches as a kernel of fused.cu /
-//      matvec_stream.cu; anything unrecognised falls back to its eager kernel, in order;
+//      matvec_stream.cu; anything unrecognised runs in order through cc_run_op (capi.cu), as in eager mode;
 //   2. the plan is hashed: each eager op's words and each fused step's descriptor bytes.  Values that change every token
 //      (position, KV length, token ids, RoPE table) live in a small device buffer `dyn` that the kernels read;
 //   3. first time a hash is seen the launches are stream-captured into a CUDA graph (programmatic-dependent-launch edges
@@ -19,21 +19,7 @@
 
 #include <chrono>
 
-#include "sample_dev.cuh"
-
-enum LKind { L_COPY_ROWS, L_DUP, L_RMS_NORM, L_MUL, L_ADD, L_SCALE, L_MATVEC, L_ROPE, L_CONCAT, L_CONTIGUOUS, L_BMM, L_SOFTMAX, L_SILU, L_GELU, L_ALLREDUCE, L_ALLGATHER, L_ARGMAX, L_SAMPLE };
-
-struct LView { cc_buf* buf = nullptr; int ndim = 0; int64_t shape[CC_MAX_DIMS] = {0, 0, 0, 0}, strides[CC_MAX_DIMS] = {0, 0, 0, 0}; };
-
-struct LOp {
-    int kind;
-    LView a, b;              // a: self / lhs / dst ; b: rhs / src
-    cc_buf* out = nullptr;   // freshly allocated result (MATVEC, BMM, DUP, CONTIGUOUS)
-    float f = 0.0f;
-    int64_t i0 = 0, i1 = 0, i2 = 0;
-    std::vector<int64_t> rows;
-    bool done = false;
-};
+#include "op_record.cuh"
 
 // one captured token graph.  The cache key is a 64-bit fold of the launch signature; `sig` is the signature itself and is compared
 // on every hit (a colliding key must re-capture, never replay another plan's baked pointers); `last_use` drives the LRU bound.
@@ -62,22 +48,6 @@ struct LazyState {
     uint64_t ns_record = 0, ns_fuse = 0, ns_submit = 0, n_ops = 0;      // host-side cost accounting
     MegaVariant mega_variant = MEGA_NONE;     // persistent kernel of the last megakernel flush
 };
-
-static LView mkview(const cc_view* v) {
-    LView l;
-    if (!v) return l;
-    l.buf = v->buf; l.ndim = v->ndim;
-    for (int i = 0; i < v->ndim; i++) { l.shape[i] = v->shape[i]; l.strides[i] = v->strides[i]; }
-    return l;
-}
-static int64_t vlen(const LView& v) { int64_t n = 1; for (int i = 0; i < v.ndim; i++) n *= v.shape[i]; return n; }
-static bool vcontig(const LView& v) {
-    if (v.ndim == 0) return true;
-    if (v.strides[v.ndim - 1] != 1) return false;
-    int64_t last = 1;
-    for (int i = v.ndim - 1; i >= 0; i--) { if (last != v.strides[i]) return false; last *= v.shape[i]; }
-    return true;
-}
 
 static void graph_entry_free(GraphEntry& ge) {
     if (ge.exec) cudaGraphExecDestroy(ge.exec);
@@ -131,13 +101,11 @@ void cc_lazy_destroy(cc_device* dev) {
 // ---- recording ---------------------------------------------------------------------------------------------------
 static void hold(LazyState* lz, cc_buf* b) { if (b) { cc_tensor_retain(b); lz->qrefs[b]++; } }
 
-int cc_lazy_record(cc_device* dev, int kind, const cc_view* a, const cc_view* b, cc_buf* out, float f, int64_t i0, int64_t i1, int64_t i2,
-                   const int64_t* rows, int n_rows) {
+int cc_lazy_record(cc_device* dev, LOp op) {
     LazyState* lz = dev->lz;
     auto t0 = std::chrono::steady_clock::now();
-    LOp op;
-    op.kind = kind; op.a = mkview(a); op.b = mkview(b); op.out = out; op.f = f; op.i0 = i0; op.i1 = i1; op.i2 = i2;
-    if (rows) op.rows.assign(rows, rows + n_rows);
+    for (cc_view* v : {&op.a, &op.b})      // a caller's view may leave the dims past ndim undefined; the plan signature hashes them all
+        for (int k = v->ndim; k < CC_MAX_DIMS; k++) v->shape[k] = v->strides[k] = 0;
     hold(lz, op.a.buf); hold(lz, op.b.buf); hold(lz, op.out);
     lz->q.push_back(std::move(op));
     lz->n_ops++;
@@ -198,51 +166,6 @@ static uint64_t hash_sig(const std::vector<uint64_t>& s) {
 }
 
 // ---- the CUDA-graph mode's launches ---------------------------------------------------------------------------------------------
-// one recorded op as its eager kernel
-static int run_op(cc_device* d, const LOp& op) {
-    const LView &a = op.a, &b = op.b;
-    switch (op.kind) {
-    case L_DUP: {
-        int64_t n = vlen(a);
-        if (n && cudaMemcpyAsync(op.out->base, a.buf->plane[0], (size_t)n * 4, cudaMemcpyDeviceToDevice, d->stream) != cudaSuccess) return cc_fail(d, CC_ERR_CUDA, "dup copy failed");
-        return CC_OK;
-    }
-    case L_RMS_NORM: return cc_launch_rms_norm(d, (float*)a.buf->plane[0], a.ndim == 1 ? 1 : a.shape[0], a.shape[a.ndim - 1], op.f);
-    case L_MUL: return cc_launch_binary(d, (float*)a.buf->plane[0], op.i0, (const float*)b.buf->plane[0], op.i1, 1);
-    case L_ADD: return cc_launch_binary(d, (float*)a.buf->plane[0], op.i0, (const float*)b.buf->plane[0], op.i1, 0);
-    case L_SCALE: return cc_launch_scale(d, (float*)a.buf->plane[0], vlen(a), op.f);
-    case L_SILU: return cc_launch_silu(d, (float*)a.buf->plane[0], vlen(a));
-    case L_GELU: return cc_launch_gelu(d, (float*)a.buf->plane[0], vlen(a));
-    case L_ALLREDUCE: return cc_launch_all_reduce(d, (float*)a.buf->plane[0], op.i0, nullptr);
-    case L_ALLGATHER: return cc_launch_all_gather(d, (const float*)b.buf->plane[0], op.i0, (float*)a.buf->plane[0]);
-    case L_ARGMAX: return cc_launch_argmax(d, (const float*)a.buf->plane[0], vlen(a), d->slots + op.i0, d->history, nullptr, op.i1);
-    case L_SOFTMAX: { int64_t cols = a.shape[a.ndim - 1]; return cc_launch_softmax(d, (float*)a.buf->plane[0], cols ? vlen(a) / cols : 0, cols); }
-    case L_ROPE: return cc_launch_rope_exact(d, (float*)a.buf->plane[0], op.i1, op.i2, a.shape[a.ndim - 1], (int)op.f, op.i0, op.rows[0]);
-    case L_CONCAT:
-        return cc_launch_strided_copy(d, b.buf->plane[0], b.buf->dtype, b.shape, b.strides, a.buf->plane[0], a.buf->dtype, a.strides,
-                                      a.shape[op.i0] * a.strides[op.i0], a.ndim);
-    case L_CONTIGUOUS: {
-        int64_t dstr[CC_MAX_DIMS]; int64_t s = 1;
-        for (int k = a.ndim - 1; k >= 0; k--) { dstr[k] = s; s *= a.shape[k]; }
-        return cc_launch_strided_copy(d, a.buf->plane[0], a.buf->dtype, a.shape, a.strides, op.out->base, a.buf->dtype, dstr, 0, a.ndim);
-    }
-    case L_BMM:
-        return cc_launch_batch_matmul(d, (const float*)a.buf->plane[0], b.buf->plane[0], b.buf->dtype, (float*)op.out->base, a.shape[0], b.shape[0],
-                                      a.shape[1], a.shape[2], b.shape[2], b.strides[0], b.strides[1], b.strides[2]);
-    case L_COPY_ROWS: {
-        int n = (int)op.rows.size();
-        int rc = cc_ensure_dev_idx(d, (size_t)n * 8);
-        if (rc) return rc;
-        if (cudaMemcpyAsync(d->dev_idx, op.rows.data(), (size_t)n * 8, cudaMemcpyHostToDevice, d->stream) != cudaSuccess) return cc_fail(d, CC_ERR_CUDA, "row index upload failed");
-        return cc_launch_dequant_rows(d, cc_deq_planes(b.buf, a.shape[a.ndim - 1]), b.buf->dtype, (const int64_t*)d->dev_idx, n, a.shape[a.ndim - 1],
-                                      a.buf->plane[0], a.buf->dtype);
-    }
-    case L_MATVEC:
-        return cc_launch_matmul_vec(d, a.buf, (const float*)b.buf->plane[0], (float*)op.out->base, a.shape[0], a.shape[1], b.ndim == 1 ? 1 : b.shape[0]);
-    }
-    return cc_fail(d, CC_ERR_UNSUPPORTED, "lazy: unknown op kind %d", op.kind);
-}
-
 // one fused step, by its descriptor, as the kernel of fused.cu / matvec_stream.cu / comm.cu that does what its phase does in the
 // persistent kernels (a generic K-quant MATVEC phase has none: its graph form is eager ops)
 static int launch_phase(cc_device* d, const MkPhase& ph, const uint8_t* dyn_dev) {
@@ -295,7 +218,6 @@ struct Fuser {
         int held = it == lz->qrefs.end() ? 0 : it->second;
         return b->refs.load() == held;
     }
-    static bool same_dense_1xN(const LView& v, int64_t n) { return vcontig(v) && vlen(v) == n; }
     // an ADD / MUL that covers all n elements: the recorded counts are those capi.cu's binary() kept after chunks_exact(4), which
     // skips the tail of an rhs longer than 1 (arithmetic.rs:5-68) -- a fused epilogue or norm would apply it to every element
     bool covers(const LOp& op, int64_t n) const { return op.i0 == n && op.i1 == n; }
@@ -337,9 +259,9 @@ struct Fuser {
         if (!(is(j, L_RMS_NORM) && is(j + 1, L_MUL))) return NormMatch();
         const LOp &rn = q[j], &mu = q[j + 1];
         if (mu.a.buf != rn.a.buf) return NormMatch();
-        const int64_t n = vlen(rn.a);
-        if (rn.a.ndim > 2 || (rn.a.ndim == 2 && rn.a.shape[0] != 1) || !vcontig(rn.a)) return NormMatch();
-        if (vlen(mu.b) != n || mu.b.buf->dtype != CC_F32 || !vcontig(mu.b) || !covers(mu, n)) return NormMatch();
+        const int64_t n = view_len(&rn.a);
+        if (rn.a.ndim > 2 || (rn.a.ndim == 2 && rn.a.shape[0] != 1) || !view_contiguous(&rn.a)) return NormMatch();
+        if (view_len(&mu.b) != n || mu.b.buf->dtype != CC_F32 || !view_contiguous(&mu.b) || !covers(mu, n)) return NormMatch();
         m.len = j + 2 - i; m.x = rn.a.buf; m.w = mu.b.buf; m.n = n; m.eps = rn.f;
         return m;
     }
@@ -347,7 +269,7 @@ struct Fuser {
     bool streams(size_t t, const cc_buf* x) const {
         if (!is(t, L_MATVEC)) return false;
         const LOp& mv = q[t];
-        return mv.b.buf == x && cc_stream_supported(mv.a.buf->dtype, mv.a.shape[1]) && vlen(mv.b) == mv.a.shape[1] && vcontig(mv.b);
+        return mv.b.buf == x && cc_stream_supported(mv.a.buf->dtype, mv.a.shape[1]) && view_len(&mv.b) == mv.a.shape[1] && view_contiguous(&mv.b);
     }
     // the MATVEC at j (weight type wt, k columns) and up to two more of the same type and k on row x, with the epilogue that follows:
     // gate/up + silu + mul (llama2.rs:620-630), or one ADD of an f32 vector per matrix, in matrix order: x = matvec + residual
@@ -357,18 +279,18 @@ struct Fuser {
     bool adds_vector(size_t at, size_t t) const {
         if (!is(at, L_ADD)) return false;
         const LOp &mv = q[t], &ad = q[at];
-        return ad.a.buf == mv.out && vlen(ad.b) == mv.a.shape[0] && covers(ad, mv.a.shape[0]) && ad.b.buf->dtype == CC_F32 && vcontig(ad.b);
+        return ad.a.buf == mv.out && view_len(&ad.b) == mv.a.shape[0] && covers(ad, mv.a.shape[0]) && ad.b.buf->dtype == CC_F32 && view_contiguous(&ad.b);
     }
     GroupMatch match_group(size_t j, const cc_buf* x, int wt, int64_t k) const {
         GroupMatch g;
         while (g.n < 3 && is(j + g.n, L_MATVEC) && q[j + g.n].b.buf == x && q[j + g.n].a.buf->dtype == wt && q[j + g.n].a.shape[1] == k &&
-               vlen(q[j + g.n].b) == k) g.n++;
+               view_len(&q[j + g.n].b) == k) g.n++;
         g.used = g.n;
         const LOp& m0 = q[j];
         bool adds = true;
         for (size_t t = 0; t < g.n; t++) adds = adds && adds_vector(j + g.n + t, j + t);
         if (g.n >= 2 && is(j + 2, L_SILU) && is(j + 3, L_MUL) && q[j + 2].a.buf == m0.out && q[j + 3].a.buf == m0.out && q[j + 3].b.buf == q[j + 1].out &&
-            m0.a.shape[0] == q[j + 1].a.shape[0] && vlen(q[j + 3].b) == m0.a.shape[0] && covers(q[j + 3], m0.a.shape[0]) && dead_after(q[j + 1].out, j + 4)) {
+            m0.a.shape[0] == q[j + 1].a.shape[0] && view_len(&q[j + 3].b) == m0.a.shape[0] && covers(q[j + 3], m0.a.shape[0]) && dead_after(q[j + 1].out, j + 4)) {
             g.n = 2; g.epilogue = 2; g.used = 4;
         } else if (adds) {
             g.epilogue = 1; g.used = 2 * g.n;
@@ -411,8 +333,8 @@ struct Fuser {
         int xchg = 0; float* xdst = nullptr; const float* xres = nullptr;
         if (g.epilogue == 0 && is(i + 1, L_ALLREDUCE) && q[i + 1].a.buf == m0.out && q[i + 1].i0 == m0.a.shape[0]) {
             n = 1; xchg = 1; used = 2; xdst = (float*)m0.out->base;
-            if (is(i + 2, L_ADD) && q[i + 2].a.buf == m0.out && vlen(q[i + 2].b) == m0.a.shape[0] && covers(q[i + 2], m0.a.shape[0]) &&
-                q[i + 2].b.buf->dtype == CC_F32 && vcontig(q[i + 2].b)) {
+            if (is(i + 2, L_ADD) && q[i + 2].a.buf == m0.out && view_len(&q[i + 2].b) == m0.a.shape[0] && covers(q[i + 2], m0.a.shape[0]) &&
+                q[i + 2].b.buf->dtype == CC_F32 && view_contiguous(&q[i + 2].b)) {
                 xres = (const float*)q[i + 2].b.buf->plane[0];
                 used = 3;
             }
@@ -533,7 +455,7 @@ struct Fuser {
         const LOp& op = q[i];
         const int64_t hidx = op.i1;
         MkPhase ph = new_phase(MK_ARGMAX);
-        ph.x = (float*)op.a.buf->plane[0]; ph.n = (int)vlen(op.a); ph.dyn_off = P.dyn_put(&hidx, 8);
+        ph.x = (float*)op.a.buf->plane[0]; ph.n = (int)view_len(&op.a); ph.dyn_off = P.dyn_put(&hidx, 8);
         ph.slot_dev = (long long*)(dev->slots + op.i0); ph.hist_dev = (long long*)dev->history;
         P.phase(ph);
         q[i].done = true;
@@ -545,11 +467,9 @@ struct Fuser {
     size_t try_sample(size_t i) {
         if (!is(i, L_SAMPLE)) return 0;
         const LOp& op = q[i];
-        SampleDyn a;
-        a.seed = (unsigned long long)op.rows[0]; a.coin_index = op.i2; a.hist_index = op.i1; a.temperature = op.f;
-        const uint32_t pb = (uint32_t)op.rows[1]; memcpy(&a.topp, &pb, 4);
+        const SampleDyn a = cc_sample_dyn(op);
         MkPhase ph = new_phase(MK_SAMPLE);
-        ph.x = (float*)op.a.buf->plane[0]; ph.n = (int)vlen(op.a); ph.dyn_off = P.dyn_put(&a, sizeof(a));
+        ph.x = (float*)op.a.buf->plane[0]; ph.n = (int)view_len(&op.a); ph.dyn_off = P.dyn_put(&a, sizeof(a));
         ph.slot_dev = (long long*)(dev->slots + op.i0); ph.hist_dev = (long long*)dev->history;
         ph.dst = dev->sample_scratch;                    // sized for this queue before fusing (cc_lazy_flush)
         P.phase(ph);
@@ -570,7 +490,7 @@ struct Fuser {
         const int wt = m0.a.buf->dtype; const int64_t k = m0.a.shape[1];
         if (!cc_mega_generic_supported(wt, k)) return 0;
         cc_buf* xb = nm.len ? nm.x : m0.b.buf;
-        if (m0.b.buf != xb || xb->dtype != CC_F32 || vlen(m0.b) != k || !vcontig(m0.b) || (m0.b.ndim == 2 && m0.b.shape[0] != 1) || m0.b.ndim > 2) return 0;
+        if (m0.b.buf != xb || xb->dtype != CC_F32 || view_len(&m0.b) != k || !view_contiguous(&m0.b) || (m0.b.ndim == 2 && m0.b.shape[0] != 1) || m0.b.ndim > 2) return 0;
         GroupMatch g = match_group(j, xb, wt, k);
         // the generic phase never writes a normalised row back (below), so a residual that is x itself would read the wrong row;
         // the residual add then runs as its own op, with or without a norm.  Its epilogue adds one vector to one matrix: the bias adds
@@ -732,13 +652,13 @@ static int size_scratch(cc_device* dev, LazyState* lz) {
         if (cudaMalloc(&lz->scores, cap) != cudaSuccess) return cc_fail(dev, CC_ERR_CUDA, "lazy: score scratch alloc failed");
         lz->scores_cap = cap;
     }
-    // eager matvec fallbacks (cc_launch_matmul_vec) use dev->act_scratch; growing it drops the cached graphs (cc_ensure_act_scratch)
+    // eager matvec steps (cc_run_op) use dev->act_scratch; growing it drops the cached graphs (cc_ensure_act_scratch)
     for (auto& op : lz->q) if (op.kind == L_MATVEC) {
         int at = cc_partner_type(op.a.buf->dtype);
         int64_t bb = op.b.ndim == 1 ? 1 : op.b.shape[0];
         if (at != CC_F32 && (rc = cc_ensure_act_scratch(dev, cc_act_bytes(at, bb * op.a.shape[1])))) return rc;
     }
-    for (auto& op : lz->q) if (op.kind == L_SAMPLE && (rc = cc_ensure_sample_scratch(dev, vlen(op.a)))) return rc;
+    for (auto& op : lz->q) if (op.kind == L_SAMPLE && (rc = cc_ensure_sample_scratch(dev, view_len(&op.a)))) return rc;
     return CC_OK;
 }
 
@@ -757,7 +677,7 @@ static int upload_dyn(cc_device* dev, LazyState* lz, const Plan& P) {
 
 static int run_steps(cc_device* dev, const Plan& P, const std::vector<LOp>& q, const uint8_t* dyn_dev) {
     for (const Plan::Step& st : P.steps)
-        if (int r = st.eager ? run_op(dev, q[st.at]) : launch_phase(dev, P.emitted[st.at], dyn_dev)) return r;
+        if (int r = st.eager ? cc_run_op(dev, q[st.at]) : launch_phase(dev, P.emitted[st.at], dyn_dev)) return r;
     return CC_OK;
 }
 
