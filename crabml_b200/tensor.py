@@ -66,6 +66,10 @@ class TensorStrider:
         return True
 
 
+MEGA_NONE, MEGA_REGISTER, MEGA_RING = 0, 1, 2      # CudaTensorDevice.mega_variant(): MegaVariant (common.cuh)
+MK_PROF_SLOTS = 10                                  # u64 stamps per phase of CudaTensorDevice.mega_profile() (common.cuh)
+
+
 class CudaTensorDevice:
     """T::DeviceRef.  Options mirror CpuTensorDeviceOptions (cpu_device.rs:13-48)."""
 
@@ -77,7 +81,7 @@ class CudaTensorDevice:
         if rc != capi.CC_OK:
             raise CudaError(self.lib.cc_last_error(None).decode())
         self.handle = h
-        self.debug_named_tensors = debug_named_tensors
+        self.debug_named_tensors, self.lazy = debug_named_tensors, int(lazy)
 
     def check(self, rc):
         if rc == capi.CC_OK:
@@ -139,8 +143,28 @@ class CudaTensorDevice:
                 "host_us_record": a[4] / 1e3, "host_us_fuse": a[5] / 1e3, "host_us_submit": a[6] / 1e3, "ops": a[7]}
 
     def mega_variant(self) -> int:
-        """0 none yet, 1 mega_kernel (tables without a Q8_0 / Q4_0 matvec), 2 mega_ring_kernel (TMA-fed shared-memory ring)."""
+        """MEGA_NONE none yet, MEGA_REGISTER mega_kernel (tables without a Q8_0 / Q4_0 matvec), MEGA_RING mega_ring_kernel (TMA-fed
+        shared-memory ring)."""
         return int(self.lib.cc_lazy_mega_variant(self.handle))
+
+    def mega_profile(self, max_phases=4096):
+        """(stamps [phases + 1, MK_PROF_SLOTS] uint64, phase type codes) of the last captured persistent kernel; needs a lazy device
+        created with CRABML_MEGA_PROF=1.  A type code is 16 * type (0 NORMQ, 1 MATVEC, 2 ATTN, 3 ROWS, 4 REDUCE, 5 GATHER, 6 ARGMAX,
+        7 SAMPLE), plus for a MATVEC phase its matrix count + 4 * epilogue + 1024 * (k >> 10)."""
+        cap = MK_PROF_SLOTS * (max_phases + 1)
+        ts, ty, n = np.zeros(cap, np.uint64), (C.c_int32 * cap)(), C.c_int32(0)
+        self.check(self.lib.cc_lazy_mega_profile(self.handle, ts.ctypes.data_as(C.POINTER(C.c_uint64)), ty, cap, C.byref(n)))
+        return ts[:(n.value + 1) * MK_PROF_SLOTS].reshape(n.value + 1, MK_PROF_SLOTS), tuple(ty[:n.value])
+
+    def mega_phase_types(self):
+        """the phase type codes of the last captured persistent kernel (mega_profile)"""
+        return self.mega_profile()[1]
+
+    def read_history(self, first, count):
+        """ids [first, first + count) of the device's history (sample_to_slot / cc_argmax_to_slot with hist_index >= 0)"""
+        out = np.empty(count, np.int64)
+        self.check(self.lib.cc_read_history(self.handle, first, count, out.ctypes.data_as(C.POINTER(C.c_int64))))
+        return out
 
     def dump_debug_tensor(self, name):                              # cpu_device.rs:96-98
         n = C.c_size_t(0)

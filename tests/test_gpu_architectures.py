@@ -9,7 +9,7 @@ from oracle import oracle as oc
 from oracle.llama_replay import Llama2Runner, LlamaConfig as OConf, LlamaWeights
 from oracle.tensor_ref import OracleDevice, OracleTensor
 from tests.blockgen import random_weight
-from tests.gpu_common import make_device
+from tests.gpu_common import assert_same_bits, fresh_device, run_modes
 
 pytestmark = pytest.mark.gpu
 
@@ -49,19 +49,19 @@ def oracle_logits(arch, wt, tokens, f16_kv):
     return np.stack([r.forward([t], p).copy() for p, t in enumerate(tokens)])
 
 
-def gpu_logits(arch, wt, tokens, f16_kv, **devkw):
+def gpu_logits(arch, wt, tokens, f16_kv):
+    """-> body(dev): the logits of every token"""
     from crabml_b200 import CudaTensor
     from crabml_b200 import runner as R
-    dev = make_device(**devkw)
-    try:
+
+    def body(dev):
         w = make_model(arch, CudaTensor, dev, wt, lambda raw, shape, t: CudaTensor.from_cpu(raw, shape, t, dev))
         conf = R.LlamaConfig(HEADS, KV, NL, DIM, HID, 64, VOCAB, 1e-6, HD, arch)
         r = R.LlamaRunner(dev, conf, w, 32, f16_kv=f16_kv)
         out = np.stack([r.forward([t], p).copy() for p, t in enumerate(tokens)])
         r.close()
         return out
-    finally:
-        dev.close()
+    return body
 
 
 @pytest.mark.parametrize("arch", ["qwen2", "gemma"])
@@ -71,10 +71,11 @@ def test_other_architectures_exact_and_fast(arch, wt):
     f16_kv = True                              # grouped-query attention (8 heads on 4 kv heads) with the f16 cache, the CLI default (main.rs:250)
     want = oracle_logits(arch, wt, tokens, f16_kv)
     assert np.isfinite(want).all() and np.abs(want).max() > 1e-3
-    exact = gpu_logits(arch, wt, tokens, f16_kv, exact_order=True)
-    np.testing.assert_array_equal(exact.view(np.uint32), want.view(np.uint32), err_msg=f"{arch}: exact_order vs the oracle replay")
-    fast = {m: gpu_logits(arch, wt, tokens, f16_kv, lazy=m) for m in (0, 1, 2)}
+    with fresh_device(exact_order=True) as dev:
+        exact = gpu_logits(arch, wt, tokens, f16_kv)(dev)
+    assert_same_bits(exact, want, f"{arch}: exact_order vs the oracle replay")
+    fast = run_modes(gpu_logits(arch, wt, tokens, f16_kv))
     for m in (1, 2):
-        np.testing.assert_array_equal(fast[m].view(np.uint32), fast[0].view(np.uint32), err_msg=f"{arch}: lazy={m} vs eager")
+        assert_same_bits(fast[m], fast[0], f"{arch}: lazy={m} vs eager")
     rel = float(np.abs(fast[0] - want).max() / np.abs(want).max())
     assert rel < 3e-2, (arch, rel)

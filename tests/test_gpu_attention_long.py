@@ -23,6 +23,8 @@ import pytest
 
 from oracle import oracle as oc
 from oracle.tensor_ref import OracleDevice, OracleTensor
+from crabml_b200.tensor import MEGA_NONE, MEGA_REGISTER, MEGA_RING
+from tests.gpu_common import MODE_DEVICE, assert_same_bits, fresh_device
 
 CURRENT = -1                                        # target: this token's own k / v row
 SCORE = 32.0                                        # the target's scaled score
@@ -32,9 +34,9 @@ KV_LENS = [1, 31, 32, 33, 63, 64, 65, 95, 96, 97, 127, 128, 129, 191, 192, 193, 
 HEADS = [(48, 6, 6), (64, 8, 8), (128, 32, 32), (128, 32, 8), (256, 8, 2)]      # (head_dim, n_heads, n_kv)
 # rows 0, at_ch - 1, at_ch, 2 at_ch - 1 and 3 at_ch for at_ch = 32 and 64
 BOUNDARY_ROWS = sorted({r for ch in (32, 64) for r in (0, ch - 1, ch, 2 * ch - 1, 3 * ch)})
-# (lazy, exact_order, ring matvec in the flush, expected mega_variant)
-MODES = {"eager": (0, False, False, 0), "graph": (1, False, False, 0), "register": (2, False, False, 1), "ring": (2, False, True, 2),
-         "exact": (0, True, False, 0)}
+# execution mode (its device: MODE_DEVICE) -> (ring matvec in the flush, expected mega_variant)
+MODES = {"eager": (False, MEGA_NONE), "graph": (False, MEGA_NONE), "register": (False, MEGA_REGISTER), "ring": (True, MEGA_RING),
+         "exact": (False, MEGA_NONE)}
 
 
 def group_of(h, n_heads, n_kv, f16):
@@ -184,19 +186,15 @@ _EAGER_MV = {}
 
 def eager_matvec():
     if "y" not in _EAGER_MV:
-        from tests.gpu_common import make_device
-        dev = make_device(lazy=0)
-        try:
+        with fresh_device(lazy=0) as dev:
             _EAGER_MV["y"] = ring_matvec(dev).export()
-        finally:
-            dev.close()
     return _EAGER_MV["y"]
 
 
 def run_retrieval(dev, mode, f16, hd, n_heads, n_kv, max_len, kv_lens, second_step=True):
     """every kv_len on one device (one max_len, one flush shape: the same kernel variant throughout)"""
     from crabml_b200 import CudaTensor
-    lazy, _, with_mv, variant = MODES[mode]
+    with_mv, variant = MODES[mode]
     dt = oc.F16 if f16 else oc.F32
     kc_full = CudaTensor.alloc([n_kv, max_len, hd], dt, dev)
     vc_full = CudaTensor.alloc([n_kv, max_len, hd], dt, dev)
@@ -209,11 +207,11 @@ def run_retrieval(dev, mode, f16, hd, n_heads, n_kv, max_len, kv_lens, second_st
             y = ring_matvec(dev) if with_mv else None
             out = attention(CudaTensor, dev, kc, vc, q, k, v, n_heads, n_kv, hd).export()
             what = f"{mode} {'f16' if f16 else 'f32'} hd {hd} heads {n_heads}/{n_kv} max_len {max_len}"
-            if lazy == 2:
+            if dev.lazy == 2:
                 assert dev.mega_variant() == variant, (what, kv_len, dev.mega_variant())
             R.check(out, step, f16, what)
             if y is not None:
-                np.testing.assert_array_equal(y.export().view(np.uint32), eager_matvec().view(np.uint32), err_msg=f"{what}: matvec vs eager")
+                assert_same_bits(y.export(), eager_matvec(), f"{what}: matvec vs eager")
             outs.append(out)
     return outs
 
@@ -225,13 +223,8 @@ def run_retrieval(dev, mode, f16, hd, n_heads, n_kv, max_len, kv_lens, second_st
 def test_retrieval_across_chunk_and_buffer_boundaries(mode, f16, hd, n_heads, n_kv):
     """Part 1: every kv_len in KV_LENS (crossing the first, second and third chunk of both chunk sizes, the first reuse of a buffer,
     and up to max_len - 1), two steps each, bit-exact against the analytic answer in every mode."""
-    from tests.gpu_common import make_device
-    lazy, exact, _, _ = MODES[mode]
-    dev = make_device(lazy=lazy, exact_order=exact)
-    try:
+    with fresh_device(**MODE_DEVICE[mode]) as dev:
         run_retrieval(dev, mode, f16, hd, n_heads, n_kv, MAX_LEN, KV_LENS)
-    finally:
-        dev.close()
 
 
 # ---- part 2: random data -----------------------------------------------------------------------------------------------------------
@@ -309,29 +302,25 @@ def test_random_attention_step_modes_oracle_and_f64(kv_len, f16, hd, n_heads, n_
     bit; exact_order mode equals the CPU oracle bit for bit; for f32 caches the megakernel is within the f64 budget above (skipped for
     f16 caches, where the reference's own f16 accumulation dominates)."""
     from crabml_b200 import CudaTensor
-    from tests.gpu_common import make_device
     K, V, q, k, v = random_case(hd, n_heads, n_kv, kv_len)
     dt = oc.F16 if f16 else oc.F32
     max_len = kv_len + 4
     got = {}
-    for mode, (lazy, exact, with_mv, variant) in MODES.items():
-        dev = make_device(lazy=lazy, exact_order=exact)
-        try:
+    for mode, (with_mv, variant) in MODES.items():
+        with fresh_device(**MODE_DEVICE[mode]) as dev:
             kc, vc = fill(CudaTensor, dev, CudaTensor.alloc([n_kv, max_len, hd], dt, dev), CudaTensor.alloc([n_kv, max_len, hd], dt, dev), K, V)
             y = ring_matvec(dev) if with_mv else None
             got[mode] = attention(CudaTensor, dev, kc, vc, q, k, v, n_heads, n_kv, hd, pos=kv_len).export()
-            if lazy == 2:
+            if dev.lazy == 2:
                 assert dev.mega_variant() == variant, (mode, dev.mega_variant())
             del y
-        finally:
-            dev.close()
     odev = OracleDevice()
     okc, ovc = fill(OracleTensor, odev, OracleTensor.alloc([n_kv, max_len, hd], dt, odev), OracleTensor.alloc([n_kv, max_len, hd], dt, odev), K, V)
     want = attention(OracleTensor, odev, okc, ovc, q, k, v, n_heads, n_kv, hd, pos=kv_len).export()
     assert np.isfinite(got["eager"]).all() and np.abs(got["eager"]).max() > 1e-3
     for mode in ("graph", "register", "ring"):
-        np.testing.assert_array_equal(got[mode].view(np.uint32), got["eager"].view(np.uint32), err_msg=f"{mode} vs eager, kv_len {kv_len}")
-    np.testing.assert_array_equal(got["exact"].view(np.uint32), want.view(np.uint32), err_msg=f"exact_order vs oracle, kv_len {kv_len}")
+        assert_same_bits(got[mode], got["eager"], f"{mode} vs eager, kv_len {kv_len}")
+    assert_same_bits(got["exact"], want, f"exact_order vs oracle, kv_len {kv_len}")
     if not f16:
         ref, budget = f64_attention_with_budget(q, k, v, K, V, kv_len, n_heads, n_kv, hd)
         ratio = float((np.abs(got["ring"].astype(np.float64) - ref) / budget).max())
@@ -346,7 +335,7 @@ def test_random_attention_step_modes_oracle_and_f64(kv_len, f16, hd, n_heads, n_
 # shared memory beside the working area, as in the real layer); and the 8-head attention alone, which runs the register kernel.  The
 # decision depends on head_dim and max_len, not on n_kv.  (head_dim, n_heads, n_kv, other phase: None = the ring matvec, 0 = none,
 # else the qkv phase of that dim; the persistent kernel below the switch)
-SWITCH_SHAPES = {"small": (128, 8, 2, None, 2), "7b": (128, 32, 8, 4096, 2), "attn": (128, 8, 2, 0, 1)}
+SWITCH_SHAPES = {"small": (128, 8, 2, None, MEGA_RING), "7b": (128, 32, 8, 4096, MEGA_RING), "attn": (128, 8, 2, 0, MEGA_REGISTER)}
 
 
 def qkv_phase(dev, dim):
@@ -364,18 +353,14 @@ def qkv_phase(dev, dim):
 def switch_step(shape, lazy, f16, max_len, kv_len, R=None):
     """fresh device; one step of the shape's flush at this max_len -> (variant, attention output, outputs of the other phase)"""
     from crabml_b200 import CudaTensor
-    from tests.gpu_common import make_device
     hd, n_heads, n_kv, dim, _ = SWITCH_SHAPES[shape]
     dt = oc.F16 if f16 else oc.F32
     R = R or Retrieval(hd, n_heads, n_kv, kv_len)
-    dev = make_device(lazy=lazy)
-    try:
+    with fresh_device(lazy=lazy) as dev:
         kc, vc = fill(CudaTensor, dev, CudaTensor.alloc([n_kv, max_len, hd], dt, dev), CudaTensor.alloc([n_kv, max_len, hd], dt, dev), R.K, R.V)
         ys = qkv_phase(dev, dim) if dim else [] if dim == 0 else [ring_matvec(dev)]
         out = attention(CudaTensor, dev, kc, vc, R.q1, R.k1, R.v1, n_heads, n_kv, hd).export()
         return dev.mega_variant(), out, [y.export() for y in ys]
-    finally:
-        dev.close()
 
 
 def first_max_len(shape, pred, lo, hi):
@@ -396,8 +381,8 @@ def switches(shape):
     """-> first max_len that leaves the persistent kernel for the CUDA graph"""
     if shape not in _SWITCHES:
         lo, hi = 256, 50808
-        assert switch_step(shape, 2, False, lo, 1)[0] == SWITCH_SHAPES[shape][4] and switch_step(shape, 2, False, hi, 1)[0] == 0
-        _SWITCHES[shape] = first_max_len(shape, lambda v: v == 0, lo, hi)
+        assert switch_step(shape, 2, False, lo, 1)[0] == SWITCH_SHAPES[shape][4] and switch_step(shape, 2, False, hi, 1)[0] == MEGA_NONE
+        _SWITCHES[shape] = first_max_len(shape, lambda v: v == MEGA_NONE, lo, hi)
     return _SWITCHES[shape]
 
 
@@ -410,18 +395,16 @@ def test_each_side_of_the_context_length_switches(shape, capsys):
     graph = switches(shape)
     hd, n_heads, n_kv, _, kernel = SWITCH_SHAPES[shape]
     with capsys.disabled():
-        print(f"\n{shape}: lazy=2 runs the {'ring' if kernel == 2 else 'register'} kernel up to max_len {graph - 1}, "
+        print(f"\n{shape}: lazy=2 runs the {'ring' if kernel == MEGA_RING else 'register'} kernel up to max_len {graph - 1}, "
               f"the CUDA graph of fused kernels from {graph}")
     for max_len in (graph - 1, graph):
         for f16 in (False, True):
             R = Retrieval(hd, n_heads, n_kv, max_len - 1)
             variant, out, ys = switch_step(shape, 2, f16, max_len, max_len - 1, R)
-            assert variant == (kernel if max_len < graph else 0), (max_len, variant)
+            assert variant == (kernel if max_len < graph else MEGA_NONE), (max_len, variant)
             R.check(out, 1, f16, f"{shape} lazy=2 max_len {max_len} variant {variant}")
             _, out0, ys0 = switch_step(shape, 0, f16, max_len, max_len - 1, R)
-            np.testing.assert_array_equal(out.view(np.uint32), out0.view(np.uint32))
-            for y, y0 in zip(ys, ys0):
-                np.testing.assert_array_equal(y.view(np.uint32), y0.view(np.uint32))
+            assert_same_bits((out, ys), (out0, ys0), f"{shape} lazy=2 vs eager, max_len {max_len} f16={f16}")
 
 
 @pytest.mark.gpu
@@ -432,8 +415,7 @@ def test_context_past_the_single_pass_kernel(lazy, max_len):
     must leave attention to the per-op kernels, as in eager mode, instead of failing the token; same bits as eager."""
     R = Retrieval(128, 8, 2, max_len - 1)
     variant, out, ys = switch_step("small", lazy, False, max_len, max_len - 1, R)
-    assert variant == 0
+    assert variant == MEGA_NONE
     R.check(out, 1, False, f"lazy={lazy} max_len {max_len}")
     _, out0, ys0 = switch_step("small", 0, False, max_len, max_len - 1, R)
-    np.testing.assert_array_equal(out.view(np.uint32), out0.view(np.uint32))
-    np.testing.assert_array_equal(ys[0].view(np.uint32), ys0[0].view(np.uint32))
+    assert_same_bits((out, ys[0]), (out0, ys0[0]), f"lazy={lazy} vs eager, max_len {max_len}")

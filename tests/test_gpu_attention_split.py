@@ -14,6 +14,8 @@ import numpy as np
 import pytest
 
 from oracle import oracle as oc
+from crabml_b200.tensor import MEGA_NONE, MEGA_REGISTER, MEGA_RING
+from tests.gpu_common import MODE_DEVICE, assert_same_bits, fresh_device
 from tests.test_gpu_attention_long import attention, fill
 
 WO_SEED = 0x5A17
@@ -22,8 +24,8 @@ MAX_LEN = 1100
 SHAPES = {"split4": (128, 32, 8, None), "split2": (64, 8, 2, None), "split1": (48, 6, 6, None),
           "split4-grid64": (128, 32, 8, 64), "split4-grid20": (128, 32, 8, 20)}
 KV_LENS = [0, 1, 2, 3, 4, 33, 129, 319, 320, 321, 322, 323, 351, 352, 353, 383, 384, 385, 447, 448, 449, 511, 512, 513, 600, 1000]
-# mode -> (lazy, wo matvec in the flush, expected mega_variant)
-MODES = {"eager": (0, True, 0), "graph": (1, True, 0), "ring": (2, True, 2), "register": (2, False, 1)}
+# execution mode (its device: MODE_DEVICE) -> (wo matvec in the flush, expected mega_variant)
+MODES = {"eager": (True, MEGA_NONE), "graph": (True, MEGA_NONE), "ring": (True, MEGA_RING), "register": (False, MEGA_REGISTER)}
 
 
 def case(hd, n_heads, n_kv, kv_len, step=0):
@@ -53,12 +55,10 @@ def step(dev, kc, vc, q, k, v, n_heads, n_kv, hd, pos, W):
 
 def run_mode(mode, f16, shape):
     from crabml_b200 import CudaTensor
-    from tests.gpu_common import make_device
     hd, n_heads, n_kv, limit = SHAPES[shape]
-    lazy, with_wo, variant = MODES[mode]
+    with_wo, variant = MODES[mode]
     dt = oc.F16 if f16 else oc.F32
-    dev = make_device(lazy=lazy)
-    try:
+    with fresh_device(**MODE_DEVICE[mode]) as dev:
         if limit:
             dev.set_sm_limit(limit)
         W = wo_weight(dev, n_heads * hd) if with_wo else None
@@ -68,15 +68,9 @@ def run_mode(mode, f16, shape):
             K, V, q, k, v = case(hd, n_heads, n_kv, kv_len)
             kc, vc = fill(CudaTensor, dev, kc_full, vc_full, K, V)
             res.append(step(dev, kc, vc, q, k, v, n_heads, n_kv, hd, kv_len, W))
-            if lazy == 2:
+            if dev.lazy == 2:
                 assert dev.mega_variant() == variant, (mode, shape, kv_len, dev.mega_variant())
         return res
-    finally:
-        dev.close()
-
-
-def same(a, b, what):
-    np.testing.assert_array_equal(a.view(np.uint32), b.view(np.uint32), err_msg=what)
 
 
 @pytest.mark.gpu
@@ -87,9 +81,9 @@ def test_split_attention_and_wo_quants_equal_eager(shape, f16):
     assert np.isfinite(got["eager"][-1][0]).all() and np.abs(got["eager"][-1][0]).max() > 1e-3
     for mode in ("graph", "ring", "register"):
         for kv_len, (o, y), (o0, y0) in zip(KV_LENS, got[mode], got["eager"]):
-            same(o, o0, f"{mode} {shape} f16={f16} kv_len {kv_len}: attention output vs eager")
+            assert_same_bits(o, o0, f"{mode} {shape} f16={f16} kv_len {kv_len}: attention output vs eager")
             if y is not None:
-                same(y, y0, f"{mode} {shape} f16={f16} kv_len {kv_len}: wo output vs eager")
+                assert_same_bits(y, y0, f"{mode} {shape} f16={f16} kv_len {kv_len}: wo output vs eager")
 
 
 @pytest.mark.gpu
@@ -97,11 +91,10 @@ def test_split_attention_and_wo_quants_equal_eager(shape, f16):
 def test_120_replayed_steps_equal_eager(f16):
     """One growing cache, 120 decode steps: lazy mode 2 replays one graph of the ring kernel (S = 4) every step."""
     from crabml_b200 import CudaTensor
-    from tests.gpu_common import make_device
     hd, n_heads, n_kv, _ = SHAPES["split4"]
     dt = oc.F16 if f16 else oc.F32
-    devs = {"eager": make_device(lazy=0), "ring": make_device(lazy=2)}
-    try:
+    with fresh_device(lazy=0) as eager, fresh_device(lazy=2) as ring:
+        devs = {"eager": eager, "ring": ring}
         st = {}
         for name, dev in devs.items():
             kc_full, vc_full = CudaTensor.alloc([n_kv, 440, hd], dt, dev), CudaTensor.alloc([n_kv, 440, hd], dt, dev)
@@ -112,12 +105,8 @@ def test_120_replayed_steps_equal_eager(f16):
         for t in range(120):
             _, _, q, k, v = case(hd, n_heads, n_kv, 0, step=t + 1)
             r = {name: step(dev, st[name][0], st[name][1], q, k, v, n_heads, n_kv, hd, 310 + t, st[name][2]) for name, dev in devs.items()}
-            assert devs["ring"].mega_variant() == 2
-            same(r["ring"][0], r["eager"][0], f"step {t}: attention output vs eager")
-            same(r["ring"][1], r["eager"][1], f"step {t}: wo output vs eager")
+            assert devs["ring"].mega_variant() == MEGA_RING
+            assert_same_bits(r["ring"], r["eager"], f"step {t}: (attention output, wo output) vs eager")
         s1 = devs["ring"].lazy_stats()
         delta = {k: s1[k] - s0[k] for k in ("flushes", "graph_captures", "graph_replays", "uncached")}
         assert delta["graph_replays"] >= 100 and delta["uncached"] == 0, delta
-    finally:
-        for dev in devs.values():
-            dev.close()

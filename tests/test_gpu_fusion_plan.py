@@ -1,33 +1,19 @@
 """Which ops the lazy fuser (lazy.cu) fuses, and which persistent kernel runs them.  Bit-identity alone cannot see a fusion that
 silently stops happening, since an unfused op gives the same bits through its eager kernel.  So each case pins, besides eager logits:
 lazy mode 1's kernel launches per token and its uncached flushes, and lazy mode 2's kernel variant and phase table fingerprint.  A
-fingerprint lists the type codes of cc_lazy_mega_profile: 16 * type (0 NORMQ, 1 MATVEC, 2 ATTN, 3 ROWS, 4 REDUCE, 5 GATHER,
+fingerprint lists the phase type codes of CudaTensorDevice.mega_phase_types(): 16 * type (0 NORMQ, 1 MATVEC, 2 ATTN, 3 ROWS, 4 REDUCE, 5 GATHER,
 6 ARGMAX, 7 SAMPLE), plus for a MATVEC phase its matrix count + 4 * epilogue + 1024 * (k >> 10)."""
-import ctypes as C
-
 import numpy as np
 import pytest
 
 from oracle import oracle as oc
-from tests.gpu_common import make_device
+from crabml_b200.tensor import MEGA_NONE, MEGA_REGISTER, MEGA_RING
+from tests.gpu_common import assert_same_bits, run_modes
 
 pytestmark = pytest.mark.gpu
 
 PROMPT = [1, 365, 2354]
 L7B = (32, 32, 1, 4096, 11008, 64, 32000, 1e-5, 128)
-
-
-def _fingerprint(dev):
-    cap = 9 * 4097
-    ts, ty, n = (C.c_uint64 * cap)(), (C.c_int32 * cap)(), C.c_int32(0)
-    dev.check(dev.lib.cc_lazy_mega_profile(dev.handle, ts, ty, cap, C.byref(n)))
-    return tuple(ty[:n.value])
-
-
-def _history(dev, count):
-    out = (C.c_int64 * count)()
-    dev.check(dev.lib.cc_read_history(dev.handle, 0, count, out))
-    return np.array(out[:], np.int64)
 
 
 def _decode(weights, sample=False):
@@ -140,7 +126,7 @@ def _samplers(n):
         t = e["T"](2.0 * e["rng"].standard_normal(64))
         for i in range(n):
             t.sample_to_slot(1.0, 0.9, 5, i, i, i)
-        return _history(e["dev"], n)
+        return e["dev"].read_history(0, n)
     return body
 
 
@@ -154,43 +140,35 @@ DECODE_7B = (48, 4115, 32, 4117, 4122, 10261, 0, 48, 4113, 96)     # embedding r
 #                                          down (k 11008) + res; final norm, a row copy, classifier + prologue, argmax
 TINY_LAYER = (19, 32, 0, 21, 26, 21)      # head_dim 48: qkv + prologue, attn, plain quantise of its output, wo + res, gate/up, down + res
 CASES = {
-    "7b-q8_0": (lambda fp: _decode(_synth(oc.Q8_0, oc.Q8_0)), 14, 0, 2, DECODE_7B),          # ring kernel
-    "7b-q4_0-q6k": (lambda fp: _decode(_synth(oc.Q4_0, oc.Q6_K)), 14, 0, 2, DECODE_7B),      # Q6_K classifier: a generic phase in the ring table
-    "7b-q4_k": (lambda fp: _decode(_synth(oc.Q4_K, oc.Q6_K)), 29, 0, 1, DECODE_7B),          # mega_kernel; mode 1 runs K-quant ops eagerly
+    "7b-q8_0": (lambda fp: _decode(_synth(oc.Q8_0, oc.Q8_0)), 14, 0, MEGA_RING, DECODE_7B),
+    "7b-q4_0-q6k": (lambda fp: _decode(_synth(oc.Q4_0, oc.Q6_K)), 14, 0, MEGA_RING, DECODE_7B),      # Q6_K classifier: a generic phase in the ring table
+    "7b-q4_k": (lambda fp: _decode(_synth(oc.Q4_K, oc.Q6_K)), 29, 0, MEGA_REGISTER, DECODE_7B),      # mode 1 runs K-quant ops eagerly
     # mixed q/k/v (wv Q6_K): the norm cannot fold into the wq/wk phase while wv still reads its row, so it is written back by a NORMQ
     # phase, then wq + wk (2 matrices) and wv (1) run as separate generic phases
-    "7b-q4_k_m": (lambda fp: _decode(_synth_q4_k_m), 28, 0, 1, (48, 0, 4114, 4113) + DECODE_7B[2:]),
-    "tinyllamas-q8_0": (_tinyllamas, 60, 0, 2, (48,) + TINY_LAYER * 6 + (0, 48, 17, 96)),
-    "7b-q8_0-sampled": (lambda fp: _decode(_synth(oc.Q8_0, oc.Q8_0), sample=True), 14, 0, 2, DECODE_7B[:-1] + (112,)),
-    "two-samplers": (lambda fp: _ops(_samplers(2)), 3, 0, 0, ()),                             # upload + 2 samplers, in the graph
-    "allreduce-add": (lambda fp: _ops(_exchange(False), comm=True), 5, 0, 2, (48, 48, 4125, 64)),   # x, r; matvec into the exchange, reduce + r
-    "allgather": (lambda fp: _ops(_exchange(True), comm=True), 5, 0, 2, (48, 48, 4125, 80)),
-    "gate-up-no-silu": (lambda fp: _ops(_gate_up_no_silu), 3, 0, 2, (48, 18)),               # x; one 2-matrix phase with a plain quantise
-    "three-then-silu": (lambda fp: _ops(_three_then_silu), 8, 0, 0, ()),                      # silu is an eager op: no persistent kernel
-    "kquant-self-residual": (lambda fp: _ops(_kquant_self_residual), 4, 0, 0, ()),             # the add is an eager op
-    "norm-weight-written": (lambda fp: _ops(_norm_weight_written), 6, 0, 2, (48, 48, 17, 0, 17)),    # z, x; nw; norm written back (x lives on), matvec
+    "7b-q4_k_m": (lambda fp: _decode(_synth_q4_k_m), 28, 0, MEGA_REGISTER, (48, 0, 4114, 4113) + DECODE_7B[2:]),
+    "tinyllamas-q8_0": (_tinyllamas, 60, 0, MEGA_RING, (48,) + TINY_LAYER * 6 + (0, 48, 17, 96)),
+    "7b-q8_0-sampled": (lambda fp: _decode(_synth(oc.Q8_0, oc.Q8_0), sample=True), 14, 0, MEGA_RING, DECODE_7B[:-1] + (112,)),
+    "two-samplers": (lambda fp: _ops(_samplers(2)), 3, 0, MEGA_NONE, ()),                             # upload + 2 samplers, in the graph
+    "allreduce-add": (lambda fp: _ops(_exchange(False), comm=True), 5, 0, MEGA_RING, (48, 48, 4125, 64)),   # x, r; matvec into the exchange, reduce + r
+    "allgather": (lambda fp: _ops(_exchange(True), comm=True), 5, 0, MEGA_RING, (48, 48, 4125, 80)),
+    "gate-up-no-silu": (lambda fp: _ops(_gate_up_no_silu), 3, 0, MEGA_RING, (48, 18)),               # x; one 2-matrix phase with a plain quantise
+    "three-then-silu": (lambda fp: _ops(_three_then_silu), 8, 0, MEGA_NONE, ()),                      # silu is an eager op: no persistent kernel
+    "kquant-self-residual": (lambda fp: _ops(_kquant_self_residual), 4, 0, MEGA_NONE, ()),             # the add is an eager op
+    "norm-weight-written": (lambda fp: _ops(_norm_weight_written), 6, 0, MEGA_RING, (48, 48, 17, 0, 17)),    # z, x; nw; norm written back (x lives on), matvec
 }
-
-
-def run_case(name, lazy, fixture_path):
-    """(launches per token, uncached flushes, variant, fingerprint, output) of one case in one lazy mode, on a fresh device."""
-    dev = make_device(lazy=lazy)
-    try:
-        launches, out = CASES[name][0](fixture_path)(dev)
-        st = dev.lazy_stats() if lazy else {"uncached": 0}
-        return launches, st["uncached"], dev.mega_variant(), _fingerprint(dev) if lazy == 2 else (), np.asarray(out).copy()
-    finally:
-        dev.close()
 
 
 @pytest.mark.parametrize("name", list(CASES))
 def test_fusion_plan(name, fixture_path, monkeypatch):
     monkeypatch.setenv("CRABML_MEGA_PROF", "1")
-    _, launches, uncached, variant, fingerprint = CASES[name]
-    _, _, _, _, ref = run_case(name, 0, fixture_path)
-    got1 = run_case(name, 1, fixture_path)
-    got2 = run_case(name, 2, fixture_path)
-    assert (got1[0], got1[1]) == (launches, uncached)
-    assert (got2[2], got2[3]) == (variant, fingerprint)
-    for got in (got1[4], got2[4]):
-        np.testing.assert_array_equal(got.view(np.uint32) if got.dtype == np.float32 else got, ref.view(np.uint32) if ref.dtype == np.float32 else ref)
+    case, launches, uncached, variant, fingerprint = CASES[name]
+
+    def body(dev):
+        n, out = case(fixture_path)(dev)
+        st = dev.lazy_stats()
+        return n, st and st["uncached"], dev.mega_variant(), dev.mega_phase_types() if dev.lazy == 2 else (), np.asarray(out).copy()
+    res = run_modes(body)
+    assert res[1][:2] == (launches, uncached), (name, "mode 1 (launches per token, uncached)", res[1][:2])
+    assert res[2][2:4] == (variant, fingerprint), (name, "mode 2 (variant, fingerprint)", res[2][2:4])
+    for mode in (1, 2):
+        assert_same_bits(res[mode][4], res[0][4], f"{name}: lazy={mode} vs eager")

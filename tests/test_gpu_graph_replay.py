@@ -16,8 +16,8 @@ import pytest
 
 from oracle import oracle as oc
 from crabml_b200.runner import synth_scale
-from tests.gpu_common import make_device
-from tests.test_gpu_stream_phase import full_grid
+from crabml_b200.tensor import MEGA_REGISTER, MEGA_RING
+from tests.gpu_common import assert_same_bits, full_grid, run_modes
 
 pytestmark = pytest.mark.gpu
 
@@ -28,10 +28,10 @@ CAPTURE, REPLAY, UNCACHED = (1, 0, 0), (0, 1, 0), (0, 0, 1)
 
 
 class _Run:
-    """One call sequence on one fresh device: the outputs of every step and, in the lazy modes, each step's lazy_stats() deltas."""
+    """One call sequence on one device: the outputs of every step and, in the lazy modes, each step's lazy_stats() deltas."""
 
-    def __init__(self, lazy):
-        self.lazy, self.dev, self.outs, self.delta = lazy, make_device(lazy=lazy), [], None
+    def __init__(self, dev):
+        self.lazy, self.dev, self.outs, self.delta = dev.lazy, dev, [], None
 
     def step(self, what, fn, want=None):
         """fn() -> None, an array or a tuple of arrays (host copies, read after the step's flush).  want: (captures, replays, uncached)
@@ -48,31 +48,19 @@ class _Run:
         return out
 
 
-def _run(scenario, lazy):
-    run = _Run(lazy)
-    try:
+def _assert_modes(scenario):
+    """the scenario on a fresh device in eager mode and lazy modes 1 and 2 (which check their own deltas): every output bit-identical
+    to eager -> eager's [(step, output)]"""
+    def body(dev):
+        run = _Run(dev)
         scenario(run)
         return run.outs
-    finally:
-        run.dev.close()
-
-
-def _same(got, ref):
-    g, r = np.asarray(got), np.asarray(ref)
-    if r.dtype == np.float32:
-        return g.dtype == np.float32 and g.shape == r.shape and np.array_equal(g.view(np.uint32), r.view(np.uint32))
-    return np.array_equal(g, r)
-
-
-def _assert_modes(scenario):
-    """the scenario in eager mode, then lazy modes 1 and 2 (which check their own deltas): every output bit-identical to eager"""
-    ref = _run(scenario, 0)
+    res = run_modes(body)
     for mode in (1, 2):
-        got = _run(scenario, mode)
-        assert [w for w, _ in got] == [w for w, _ in ref], mode
-        for (what, g), (_, r) in zip(got, ref):
-            assert _same(g, r), (f"lazy={mode} vs eager", what)
-    return ref
+        assert [w for w, _ in res[mode]] == [w for w, _ in res[0]], mode
+        for (what, g), (_, r) in zip(res[mode], res[0]):
+            assert_same_bits(g, r, f"lazy={mode} vs eager: {what}")
+    return res[0]
 
 
 def _weight(dev, m, k, t, tid):
@@ -166,14 +154,14 @@ def test_second_prompt_regrows_scratch_under_decode_graphs():
         if run.lazy:
             assert run.delta[2] == 0 and run.delta[0] >= 2, run.delta
         if run.lazy == 2:
-            assert dev.mega_variant() == 1
+            assert dev.mega_variant() == MEGA_REGISTER
         r.close()
         r = R.LlamaRunner(dev, conf, w, conf.seq_len)
         lg = run.step("B-prompt", lambda: r.forward(PROMPT_B, 0), UNCACHED)
         nxt = len(lg) - 1 - int(np.argmax(lg[::-1]))        # the sampler's argmax: the last maximum
         run.step("B-decode", lambda: r.generate_greedy_logits([nxt], 6), (2, 4, 0))
         if run.lazy == 2:
-            assert dev.mega_variant() == 1
+            assert dev.mega_variant() == MEGA_REGISTER
         r.close()
     ref = dict(_assert_modes(scenario))
     assert np.isfinite(ref["B-decode[1]"]).all() and len(ref["B-decode[0]"]) == 6
@@ -231,7 +219,7 @@ def test_type_change_at_one_pooled_address():
 
 # ---- 3. the persistent grid changes after a capture --------------------------------------------------------------------------------
 L7B = (32, 32, 1, 4096, 11008, 64, 32000, 1e-5, 128)
-SM_CASES = {"q8_0-ring": (oc.Q8_0, oc.Q8_0, 2), "q4_k-mega": (oc.Q4_K, oc.Q6_K, 1)}
+SM_CASES = {"q8_0-ring": (oc.Q8_0, oc.Q8_0, MEGA_RING), "q4_k-mega": (oc.Q4_K, oc.Q6_K, MEGA_REGISTER)}
 
 
 @pytest.mark.parametrize("case", list(SM_CASES))
@@ -297,5 +285,5 @@ def test_lru_bound_of_the_graph_cache():
         for n, (p, want) in enumerate(seq):
             run.step(f"{n}:plan{p}", lambda: ws[p].matmul_vec(_row(dev, table, n, k)).export(), want)
         if run.lazy == 2:
-            assert dev.mega_variant() == 2
+            assert dev.mega_variant() == MEGA_RING
     _assert_modes(scenario)

@@ -6,7 +6,7 @@ import pytest
 
 from oracle.llama_replay import GGUFModel, Llama2Runner, LlamaTokenizer, decode_text, load_weights
 from oracle.tensor_ref import OracleDevice, OracleTensor
-from tests.gpu_common import make_device
+from tests.gpu_common import assert_same_bits, fresh_device
 from tests.test_oracle_golden_text import CASES, PROMPT, PROMPT_IDS
 
 pytestmark = pytest.mark.gpu
@@ -44,9 +44,8 @@ def test_exact_order_mode_is_bit_identical(fixture_path, fname, text, ids, f16_k
     gm = GGUFModel(fixture_path(fname))
     tok = LlamaTokenizer(gm.tokens, gm.scores, gm.bos, gm.eos)
     assert tok.encode(PROMPT, True, False) == PROMPT_IDS
-    gdev = make_device(debug_named_tensors=True, exact_order=True)
     odev = OracleDevice(debug_named_tensors=True)
-    try:
+    with fresh_device(debug_named_tensors=True, exact_order=True) as gdev:
         g_out, g_logits = _run(CudaTensor, gdev, gm, 11, f16_kv)
         o_out, o_logits = _run(OracleTensor, odev, gm, 11, f16_kv)
         assert g_out == o_out
@@ -54,14 +53,12 @@ def test_exact_order_mode_is_bit_identical(fixture_path, fname, text, ids, f16_k
             assert g_out == ids and decode_text(tok, g_out) == text
         rel = (np.abs(g_logits - o_logits) / np.abs(o_logits).max(axis=1, keepdims=True)).max()
         assert rel < REL_TOL, rel
-        np.testing.assert_array_equal(g_logits.view(np.uint32), o_logits.view(np.uint32))
+        assert_same_bits(g_logits, o_logits, "exact_order vs the oracle")
         # debug taps: the mechanism of the reference's own cross-backend test (llama2.rs:768-784)
         for name in ("attn_rmsnorm:0:0", "x_debug:0:0", "attn_out:0:0", "ffn_out:0:0", "ffn_out:5:9", "final_rmsnorm:9"):
             a, b = gdev.dump_debug_tensor(name), odev.dump_debug_tensor(name)
             assert a is not None and a.shape == b.shape, name
-            np.testing.assert_array_equal(a.view(np.uint32), b.view(np.uint32), err_msg=name)
-    finally:
-        gdev.close()
+            assert_same_bits(a, b, name)
 
 
 @pytest.mark.parametrize("fname,text,ids", CASES)
@@ -72,9 +69,8 @@ def test_fast_mode_generation_and_band(fixture_path, fname, text, ids):
     path = fixture_path(fname)
     gm = GGUFModel(path)
     tok = LlamaTokenizer(gm.tokens, gm.scores, gm.bos, gm.eos)
-    gdev = make_device(debug_named_tensors=True)
     odev = OracleDevice(debug_named_tensors=True)
-    try:
+    with fresh_device(debug_named_tensors=True) as gdev:
         g_out, g_logits = _run(CudaTensor, gdev, gm, 11)
         o_out, o_logits = _run(OracleTensor, odev, gm, 11)
         assert g_out == o_out == ids and decode_text(tok, g_out) == text
@@ -86,8 +82,6 @@ def test_fast_mode_generation_and_band(fixture_path, fname, text, ids):
         for name, eps in (("attn_rmsnorm:0:0", 1e-6), ("x_debug:0:0", 1e-6), ("attn_out:0:0", 1e-6)):
             a, b = gdev.dump_debug_tensor(name), odev.dump_debug_tensor(name)
             np.testing.assert_allclose(a, b, atol=eps * max(1.0, float(np.abs(b).max())), err_msg=name)
-    finally:
-        gdev.close()
 
 
 def test_long_decode_positions(fixture_path):
@@ -95,11 +89,8 @@ def test_long_decode_positions(fixture_path):
     a growing KV cache; logits must stay within the bar at every step."""
     from crabml_b200 import CudaTensor
     gm = GGUFModel(fixture_path("tinyllamas-stories-15m-q8_0.gguf"))
-    gdev = make_device(exact_order=True)
-    try:
+    with fresh_device(exact_order=True) as gdev:
         g_out, g_logits = _run(CudaTensor, gdev, gm, 100)
         o_out, o_logits = _run(OracleTensor, OracleDevice(), gm, 100)
         assert g_out == o_out
-        np.testing.assert_array_equal(g_logits.view(np.uint32), o_logits.view(np.uint32))
-    finally:
-        gdev.close()
+        assert_same_bits(g_logits, o_logits, "exact_order vs the oracle")

@@ -9,7 +9,7 @@ import pytest
 from crabml_b200.capi import ROPE_LLAMA, ROPE_NEOX
 from oracle import oracle as oc
 from tests.blockgen import random_weight
-from tests.gpu_common import make_device
+from tests.gpu_common import assert_same_bits, run_modes
 
 pytestmark = pytest.mark.gpu
 
@@ -36,12 +36,6 @@ def _f16_rows(dev, t):
     dev.flush()
     out.copy_rows_from(t, list(range(rows)))
     return out.export()
-
-
-def _history(dev, count):
-    out = (C.c_int64 * count)()
-    dev.check(dev.lib.cc_read_history(dev.handle, 0, count, out))
-    return np.array(out[:], np.int64)
 
 
 # Each case builds its inputs, flushes, runs ONE op, flushes, and returns the outputs.
@@ -162,13 +156,13 @@ def _matvec(wt, rows):
 def case_argmax_to_slot(dev):
     x = _new(dev, [300], 18); dev.flush()
     dev.check(dev.lib.cc_argmax_to_slot(dev.handle, C.byref(x._view()), 1, 0)); dev.flush()
-    return [_history(dev, 1)]
+    return [dev.read_history(0, 1)]
 
 
 def case_sample_to_slot(dev):
     x = _new(dev, [300], 19, 2.0); dev.flush()
     x.sample_to_slot(0.8, 0.9, 7, 3, 1, 0); dev.flush()
-    return [_history(dev, 1)]
+    return [dev.read_history(0, 1)]
 
 
 CASES = {
@@ -183,20 +177,8 @@ CASES = {
 }
 
 
-def _run(case, lazy):
-    dev = make_device(lazy=lazy)
-    try:
-        return case(dev)
-    finally:
-        dev.close()
-
-
 @pytest.mark.parametrize("name", list(CASES))
 def test_op_alone_is_bit_identical_in_every_mode(name):
-    want = _run(CASES[name], 0)
+    res = run_modes(CASES[name])
     for lazy in (1, 2):
-        got = _run(CASES[name], lazy)
-        assert len(got) == len(want)
-        for g, w in zip(got, want):
-            assert g.dtype == w.dtype and g.shape == w.shape, (name, lazy)
-            assert np.array_equal(g.view(np.uint8), w.view(np.uint8)), (name, lazy)
+        assert_same_bits(res[lazy], res[0], f"{name}: lazy={lazy} vs eager")

@@ -15,8 +15,9 @@ import pytest
 from oracle import oracle as oc
 from oracle.synth import synth_weight
 from oracle.tensor_ref import OracleDevice, OracleTensor
+from crabml_b200.tensor import MEGA_RING
 from tests.gpu_common import make_device
-from tests.test_gpu_qwen2 import MEGA_RING, SPLIT_FROM
+from tests.test_gpu_qwen2 import SPLIT_FROM
 
 pytestmark = pytest.mark.gpu
 

@@ -24,7 +24,7 @@ import pytest
 
 from oracle import oracle as oc
 from tests.blockgen import random_weight
-from tests.gpu_common import make_device
+from tests.gpu_common import assert_same_bits, fresh_device, run_modes
 
 pytestmark = pytest.mark.gpu
 
@@ -35,9 +35,8 @@ CHUNK = 2048                                                              # weig
 
 @pytest.fixture(scope="module")
 def gdev():
-    d = make_device()
-    yield d
-    d.close()
+    with fresh_device() as d:
+        yield d
 
 
 @pytest.fixture(scope="module", autouse=True)
@@ -231,31 +230,21 @@ def test_prefill_small_batches_keep_the_exact_block_path(gdev):
 def test_prefill_exact_order_bit_identical(t):
     """exact_order mode never takes the tensor cores: a batch of 40 rows is bit-identical to the reference's gemv"""
     from crabml_b200 import CudaTensor
-    dev = make_device(exact_order=True)
-    try:
+    with fresh_device(exact_order=True) as dev:
         rng = np.random.default_rng(600 + t)
         m, k, b = 19, 512, 40
         raw = random_weight(t, m, k, rng)
         x = rng.standard_normal((b, k)).astype(np.float32)
         got = CudaTensor.from_cpu(raw, [m, k], t, dev).matmul_vec(CudaTensor.new(x, [b, k], dev)).export()
         want = oc.gemv(t, raw, m, k, x).reshape(-1)
-        np.testing.assert_array_equal(got.view(np.uint32), want.view(np.uint32), err_msg=oc.TYPE_NAMES[t])
-    finally:
-        dev.close()
+        assert_same_bits(got, want, oc.TYPE_NAMES[t])
 
 
 def dense_once(t, raw, m, k, x, **dev_kw):
     """the (b, m) result of one batched matmul_vec on a fresh device"""
     from crabml_b200 import CudaTensor
-    dev = make_device(**dev_kw)
-    try:
+    with fresh_device(**dev_kw) as dev:
         return CudaTensor.from_cpu(raw, [m, k], t, dev).matmul_vec(CudaTensor.new(x, list(x.shape), dev)).export()
-    finally:
-        dev.close()
-
-
-def same_bits(a, b):
-    return np.array_equal(np.asarray(a, np.float32).view(np.uint32), np.asarray(b, np.float32).view(np.uint32))
 
 
 @pytest.mark.parametrize("t", [oc.Q8_0, oc.Q4_K])
@@ -268,21 +257,20 @@ def test_prefill_lazy_modes_match_eager(t):
     raw = random_weight(t, m, k, rng, 0.02)
     x = rng.standard_normal((b, k)).astype(np.float32)
     eager = dense_once(t, raw, m, k, x)
+
+    def body(dev):
+        w = CudaTensor.from_cpu(raw, [m, k], t, dev)
+        xt = CudaTensor.new(x, [b, k], dev)
+        outs, uncached = [], []
+        for _ in range(2):
+            u0 = dev.lazy_stats()["uncached"]
+            outs.append(w.matmul_vec(xt).export())
+            uncached.append(dev.lazy_stats()["uncached"] - u0)
+        return outs, uncached
+    res = run_modes(body, modes=(1, 2))
     for lazy in (1, 2):
-        dev = make_device(lazy=lazy)
-        try:
-            w = CudaTensor.from_cpu(raw, [m, k], t, dev)
-            xt = CudaTensor.new(x, [b, k], dev)
-            outs = []
-            for _ in range(2):
-                u0 = dev.lazy_stats()["uncached"]
-                outs.append(w.matmul_vec(xt).export())
-                st = dev.lazy_stats()
-                assert st["uncached"] == u0 + 1, (lazy, st)
-            for o in outs:
-                assert same_bits(o, eager), (lazy, oc.TYPE_NAMES[t])
-        finally:
-            dev.close()
+        assert res[lazy][1] == [1, 1], (lazy, "uncached flushes", res[lazy][1])
+        assert_same_bits(res[lazy][0], [eager, eager], f"lazy={lazy} {oc.TYPE_NAMES[t]} vs eager")
 
 
 def test_prefill_cached_weights_and_row_views(gdev):
@@ -298,21 +286,18 @@ def test_prefill_cached_weights_and_row_views(gdev):
     views = (64, 200)
     view_fresh = {mv: dense_once(t, raw[:oc.nbytes_for(t, mv * k)], mv, k, x).reshape(b, mv) for mv in views}
     for mv in views:
-        assert same_bits(view_fresh[mv], full_fresh[:, :mv]), mv
-    dev = make_device()
-    try:
+        assert_same_bits(view_fresh[mv], full_fresh[:, :mv], f"rows [0, {mv}) vs the full matrix")
+    with fresh_device() as dev:
         w = CudaTensor.from_cpu(raw, [m, k], t, dev)
         xt = CudaTensor.new(x, [b, k], dev)
         before = {mv: w.resize(0, mv).matmul_vec(xt).export().reshape(b, mv) for mv in views}     # scratch grows from 64 to 200 rows
         first = w.matmul_vec(xt).export().reshape(b, m)                                            # makes the cached f16 copy
         second = w.matmul_vec(xt).export().reshape(b, m)                                           # reuses it
         after = {mv: w.resize(0, mv).matmul_vec(xt).export().reshape(b, mv) for mv in views[::-1]}
-        assert same_bits(first, full_fresh) and same_bits(second, full_fresh)
+        assert_same_bits((first, second), (full_fresh, full_fresh), "first and second call vs a fresh device")
         for mv in views:
-            assert same_bits(before[mv], view_fresh[mv]) and same_bits(after[mv], view_fresh[mv]), mv
+            assert_same_bits((before[mv], after[mv]), (view_fresh[mv], view_fresh[mv]), f"view of {mv} rows before and after vs a fresh device")
         check_dense(t, raw, m, k, x, second, what="cached weight, second call")
-    finally:
-        dev.close()
 
 
 def test_prefill_scratch_regrowth(gdev):
@@ -325,13 +310,10 @@ def test_prefill_scratch_regrowth(gdev):
     xs = {b: rng.standard_normal((b, k)).astype(np.float32) for b in (40, 1000)}
     fresh = {b: dense_once(t, raw, m, k, x) for b, x in xs.items()}
     for order in ((40, 1000, 40), (1000, 40, 1000)):
-        dev = make_device()
-        try:
+        with fresh_device() as dev:
             w = CudaTensor.from_cpu(raw, [m, k], t, dev)
             for b in order:
-                assert same_bits(w.matmul_vec(CudaTensor.new(xs[b], [b, k], dev)).export(), fresh[b]), (order, b)
-        finally:
-            dev.close()
+                assert_same_bits(w.matmul_vec(CudaTensor.new(xs[b], [b, k], dev)).export(), fresh[b], (order, b))
     check_dense(t, raw, m, k, xs[1000], fresh[1000].reshape(1000, m), what="Q4_K b=1000")
 
 

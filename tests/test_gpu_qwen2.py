@@ -9,43 +9,41 @@ import pytest
 from oracle import oracle as oc
 from oracle.llama_replay import Llama2Runner, LlamaConfig as OConf, LlamaWeights
 from oracle.tensor_ref import OracleDevice, OracleTensor
+from crabml_b200.tensor import MEGA_RING
 from tests.blockgen import random_weight
-from tests.gpu_common import make_device
+from tests.gpu_common import assert_same_bits, fresh_device, run_modes
 
 pytestmark = pytest.mark.gpu
 
-MEGA_RING = 2                           # cc_lazy_mega_variant: mega_ring_kernel
 SPLIT_FROM = 320                        # AT_SPLIT_MIN_KV: from this many cached positions the persistent attention runs S CTAs per head
 
 
-def _run_modes(make, conf, tokens, checkpoints, f16_kv, kv_len, modes=(0, 1, 2)):
-    """logits at `checkpoints` for each lazy mode; in mode 2 every checkpoint is one persistent ring kernel"""
+def _run_modes(make, conf, tokens, checkpoints, f16_kv, kv_len):
+    """logits at `checkpoints` for each lazy mode, bit-identical; in mode 2 every checkpoint is one persistent ring kernel"""
     from crabml_b200 import runner as R
-    out = {}
-    for m in modes:
-        dev = make_device(lazy=m)
-        try:
-            r = R.LlamaRunner(dev, conf, make(dev), kv_len, f16_kv=f16_kv)
-            got = []
-            for p, t in enumerate(tokens):
-                if p not in checkpoints:
-                    r.forward([t], p, export=False)
-                    continue
-                l0 = dev.launch_count()
-                got.append(r.forward([t], p).copy())
-                if m == 2:
-                    assert dev.launch_count() - l0 == 1, (p, dev.launch_count() - l0)
-                    assert dev.mega_variant() == MEGA_RING
-            if m:
-                assert dev.lazy_stats()["uncached"] == 0
-            out[m] = np.stack(got)
-            r.close()
-        finally:
-            dev.close()
-    assert np.isfinite(out[modes[0]]).all() and np.abs(out[modes[0]]).max() > 1e-3
-    for m in modes[1:]:
-        np.testing.assert_array_equal(out[m].view(np.uint32), out[modes[0]].view(np.uint32), err_msg=f"lazy={m} vs lazy={modes[0]}")
-    return out
+
+    def body(dev):
+        r = R.LlamaRunner(dev, conf, make(dev), kv_len, f16_kv=f16_kv)
+        got, kernels = [], []
+        for p, t in enumerate(tokens):
+            if p not in checkpoints:
+                r.forward([t], p, export=False)
+                continue
+            l0 = dev.launch_count()
+            got.append(r.forward([t], p).copy())
+            kernels.append((p, dev.launch_count() - l0, dev.mega_variant()))
+        st = dev.lazy_stats()
+        r.close()
+        return np.stack(got), kernels, st
+    out = run_modes(body)
+    for p, launches, variant in out[2][1]:
+        assert (launches, variant) == (1, MEGA_RING), (p, launches, variant)
+    for m in (1, 2):
+        assert out[m][2]["uncached"] == 0, (m, out[m][2])
+    assert np.isfinite(out[0][0]).all() and np.abs(out[0][0]).max() > 1e-3
+    for m in (1, 2):
+        assert_same_bits(out[m][0], out[0][0], f"lazy={m} vs lazy=0")
+    return {m: v[0] for m, v in out.items()}
 
 
 # ---- Qwen2-7B shapes: dim 3584, 28 heads on 4 kv heads, head_dim 128, hidden 18944, vocab 152064; two layers ------------------------
@@ -119,14 +117,11 @@ def test_qwen2_small_exact_and_modes(wt, rope_dim, f16_kv):
     tokens = _tokens(wt, rope_dim)
     n_oracle = 12
     want = oracle_logits(wt, rope_dim, tokens[:n_oracle], f16_kv)
-    dev = make_device(exact_order=True)
-    try:
+    with fresh_device(exact_order=True) as dev:
         r = R.LlamaRunner(dev, conf, make_model(wt, _gpu_from_raw(dev)), n_oracle + 4, f16_kv=f16_kv)
         got = np.stack([r.forward([t], p).copy() for p, t in enumerate(tokens[:n_oracle])])
         r.close()
-    finally:
-        dev.close()
-    np.testing.assert_array_equal(got.view(np.uint32), want.view(np.uint32), err_msg="exact_order vs the oracle replay")
+    assert_same_bits(got, want, "exact_order vs the oracle replay")
     _small_fast_modes(wt, rope_dim, f16_kv, tokens, {0, 1, 2, SPLIT_FROM - 1, SPLIT_FROM, len(tokens) - 1})
 
 
@@ -189,8 +184,7 @@ def test_qwen2_gguf_loads_into_the_same_logits(tmp_path, tied, lazy):
     path = str(tmp_path / "qwen2.gguf")
     raw = _write_gguf(path, oc.Q8_0, 32, tied)
     tokens = [1, 77, 300, 5, 999, 42, 7]
-    dev = make_device(lazy=lazy)
-    try:
+    with fresh_device(lazy=lazy) as dev:
         conf, w, tok = R.load_gguf(path, dev)
         assert (conf.arch, conf.n_heads, conf.n_kv_heads, conf.n_layers, conf.embedding_dim, conf.hidden_dim, conf.seq_len, conf.vocab_size,
                 conf.rope_dim) == ("qwen2", HEADS, KV, NL, DIM, HID, 512, VOCAB, 32)
@@ -212,10 +206,8 @@ def test_qwen2_gguf_loads_into_the_same_logits(tmp_path, tied, lazy):
         r = R.LlamaRunner(dev, conf, direct, 16)
         want = np.stack([r.forward([t], p).copy() for p, t in enumerate(tokens)])
         r.close()
-    finally:
-        dev.close()
     assert np.isfinite(want).all() and np.abs(want).max() > 1e-3
-    np.testing.assert_array_equal(got.view(np.uint32), want.view(np.uint32))
+    assert_same_bits(got, want, "the gguf load vs the same weights passed in")
 
 
 def test_qwen2_gguf_sharded_load_is_refused(tmp_path):
@@ -223,9 +215,5 @@ def test_qwen2_gguf_sharded_load_is_refused(tmp_path):
     from crabml_b200.capi import TensorError
     path = str(tmp_path / "qwen2.gguf")
     _write_gguf(path, oc.Q8_0, 64, True)
-    dev = make_device()
-    try:
-        with pytest.raises(TensorError, match="sharding"):
-            R.load_gguf(path, dev, shard=(0, 2))
-    finally:
-        dev.close()
+    with fresh_device() as dev, pytest.raises(TensorError, match="sharding"):
+        R.load_gguf(path, dev, shard=(0, 2))

@@ -21,9 +21,10 @@ from oracle.llama_replay import Llama2Runner, LlamaConfig as OConf, LlamaWeights
 from oracle.synth import synth_weight
 from oracle.tensor_ref import OracleDevice, OracleTensor
 from tests import sampler_ref as S
+from crabml_b200.tensor import MEGA_NONE, MEGA_RING
 from tests.blockgen import random_weight
-from tests.gpu_common import make_device
-from tests.test_gpu_qwen2 import DIM, HEADS, HID, KV, MEGA_RING, NL, SPLIT_FROM, VOCAB, _gpu_from_raw, make_model
+from tests.gpu_common import assert_same_bits, fresh_device, run_modes
+from tests.test_gpu_qwen2 import DIM, HEADS, HID, KV, NL, SPLIT_FROM, VOCAB, _gpu_from_raw, make_model
 
 pytestmark = pytest.mark.gpu
 
@@ -91,11 +92,6 @@ def host_loop(r, prompt, steps, temperature, topp, pick):
     return ids, np.stack(lgs)
 
 
-def assert_bits(a, b, msg):
-    assert a.shape == b.shape, (msg, a.shape, b.shape)
-    np.testing.assert_array_equal(a.view(np.uint32), b.view(np.uint32), err_msg=msg)
-
-
 def eos_stop(ids, eos):
     """the reference's rule (llama2.rs:141-172): the first id, from the prompt pass, is always yielded; every later step stops before
     yielding EOS"""
@@ -113,8 +109,7 @@ def test_exact_order_generation_equals_the_oracle_replay(model, f16_kv):
     wt, ct, tied = MODELS[model]
     prompt, steps = [1, 600, 42], 24
     kv_len = len(prompt) + steps + 4
-    dev = make_device(exact_order=True)
-    try:
+    with fresh_device(exact_order=True) as dev:
         w = small_model(wt, ct, tied, _gpu_from_raw(dev))
         for temperature, topp in SAMPLERS:
             r = R.LlamaRunner(dev, small_conf(), w, kv_len, f16_kv=f16_kv)
@@ -124,11 +119,9 @@ def test_exact_order_generation_equals_the_oracle_replay(model, f16_kv):
             want_ids, want_logits = host_loop(oracle_small(wt, ct, tied, f16_kv, kv_len), prompt, steps, temperature, topp, S.sample)
             assert np.isfinite(want_logits).all() and np.abs(want_logits).max() > 1e-3
             assert ids == want_ids, (temperature, topp)
-            assert_bits(logits, want_logits, f"T={temperature} topp={topp}: exported logits vs the oracle replay")
+            assert_same_bits(logits, want_logits, f"T={temperature} topp={topp}: exported logits vs the oracle replay")
             if temperature == 0.8:
                 assert len(set(ids)) > 4, ids                       # the coin decides, the run is not stuck on one id
-    finally:
-        dev.close()
 
 
 # ---- 1. small qwen2, fast modes: one another, the fast sampler, the host loop, EOS -----------------------------------------------------
@@ -152,43 +145,44 @@ def test_small_device_loop_fast_modes(model, f16_kv):
     prompt, steps = [7], SPLIT_FROM + 8
     conf = small_conf()
     for temperature, topp in SAMPLERS:
-        runs, eos = {}, None
+        stop = []                        # (eos, k): the fifth id of eager mode, and where the reference stops on it
+
+        def body(dev):
+            w = small_model(wt, ct, tied, _gpu_from_raw(dev))
+            r = R.LlamaRunner(dev, conf, w, steps + 4, f16_kv=f16_kv)
+            l0 = dev.launch_count()
+            ids, logits = device_loop(r, prompt, steps, temperature, topp)
+            launches = (dev.launch_count() - l0) / len(ids)
+            assert len(ids) == steps and r.kv_cache_len() == len(prompt) + steps - 1
+            r.close()
+            print(f"{model} f16_kv={f16_kv} T={temperature} topp={topp} lazy={dev.lazy}: {launches:g} launches per token")
+            st, variant, host = dev.lazy_stats(), dev.mega_variant(), None
+            if dev.lazy == 2:
+                r = R.LlamaRunner(dev, conf, w, steps + 4, f16_kv=f16_kv)
+                host = host_loop(r, prompt, steps, temperature, topp, S.sample_fast)
+                r.close()
+            if not stop:
+                stop.append((ids[4], eos_stop(ids, ids[4])))
+                assert stop[0][1] < steps
+            eos, k = stop[0]
+            r = R.LlamaRunner(dev, conf, w, steps + 4, f16_kv=f16_kv)
+            e_ids = r.generate_greedy(prompt, steps, eos=eos) if temperature == 0.0 else r.generate(prompt, steps, temperature, topp, SEED, eos=eos)
+            assert e_ids == ids[:k], (dev.lazy, eos, e_ids, ids[:k + 1])
+            assert r.kv_cache_len() == len(prompt) + k        # the step that sampled EOS ran; nothing after it
+            r.close()
+            return ids, logits, launches, st, variant, host
+        runs = run_modes(body)
+        ids, logits = runs[0][:2]
         for m in (0, 1, 2):
-            dev = make_device(lazy=m)
-            try:
-                w = small_model(wt, ct, tied, _gpu_from_raw(dev))
-                r = R.LlamaRunner(dev, conf, w, steps + 4, f16_kv=f16_kv)
-                l0 = dev.launch_count()
-                ids, logits = device_loop(r, prompt, steps, temperature, topp)
-                launches = (dev.launch_count() - l0) / len(ids)
-                assert len(ids) == steps and r.kv_cache_len() == len(prompt) + steps - 1
-                r.close()
-                print(f"{model} f16_kv={f16_kv} T={temperature} topp={topp} lazy={m}: {launches:g} launches per token")
-                assert launches == LAUNCHES_PER_TOKEN[streaming][m], (m, launches)
-                if m:
-                    assert ids == runs[0][0], f"lazy={m} vs eager ids"
-                    assert_bits(logits, runs[0][1], f"lazy={m} vs eager logits")
-                    assert dev.lazy_stats()["uncached"] == 0, dev.lazy_stats()
-                if m == 2:
-                    assert dev.mega_variant() == (MEGA_RING if streaming else 0), dev.mega_variant()
-                    r = R.LlamaRunner(dev, conf, w, steps + 4, f16_kv=f16_kv)
-                    h_ids, h_logits = host_loop(r, prompt, steps, temperature, topp, S.sample_fast)
-                    r.close()
-                    assert h_ids == ids, "device loop vs host loop"
-                    assert_bits(logits, h_logits, "device loop vs host loop")
-                if eos is None:
-                    eos = ids[4]
-                    k = eos_stop(ids, eos)
-                    assert k < steps
-                r = R.LlamaRunner(dev, conf, w, steps + 4, f16_kv=f16_kv)
-                e_ids = r.generate_greedy(prompt, steps, eos=eos) if temperature == 0.0 else r.generate(prompt, steps, temperature, topp, SEED, eos=eos)
-                assert e_ids == ids[:k], (m, eos, e_ids, ids[:k + 1])
-                assert r.kv_cache_len() == len(prompt) + k        # the step that sampled EOS ran; nothing after it
-                r.close()
-                runs[m] = ids, logits
-            finally:
-                dev.close()
-        ids, logits = runs[0]
+            assert runs[m][2] == LAUNCHES_PER_TOKEN[streaming][m], (m, runs[m][2])
+        for m in (1, 2):
+            assert runs[m][0] == ids, f"lazy={m} vs eager ids"
+            assert_same_bits(runs[m][1], logits, f"lazy={m} vs eager logits")
+            assert runs[m][3]["uncached"] == 0, runs[m][3]
+        assert runs[2][4] == (MEGA_RING if streaming else MEGA_NONE), runs[2][4]
+        h_ids, h_logits = runs[2][5]
+        assert h_ids == runs[2][0], "device loop vs host loop"
+        assert_same_bits(runs[2][1], h_logits, "device loop vs host loop")
         assert np.isfinite(logits).all() and np.abs(logits).max() > 1e-3
         assert ids == [S.sample_fast(logits[i], temperature, topp, SEED, i) for i in range(steps)]
         if temperature == 0.8:
@@ -209,27 +203,24 @@ def test_qwen2_7b_device_loop_modes_bit_identical(wt, ct):
     conf = conf_7b(2)
     steps = SPLIT_FROM + 8
     samplers = [(0.0, 0.0), (0.8, 0.9)]
-    res = {}
-    for m in (0, 1, 2):
-        dev = make_device(lazy=m)
-        try:
-            w = R.synthetic_weights(dev, conf, wt, ct, seed=0x0E2)
-            for temperature, topp in samplers:
-                r = R.LlamaRunner(dev, conf, w, steps + 4)
-                res[m, temperature] = device_loop(r, [1], steps, temperature, topp)
-                r.close()
-            if m:
-                assert dev.lazy_stats()["uncached"] == 0
-            if m == 2:
-                assert dev.mega_variant() == MEGA_RING
-        finally:
-            dev.close()
+    def body(dev):
+        w = R.synthetic_weights(dev, conf, wt, ct, seed=0x0E2)
+        loops = {}
+        for temperature, topp in samplers:
+            r = R.LlamaRunner(dev, conf, w, steps + 4)
+            loops[temperature] = device_loop(r, [1], steps, temperature, topp)
+            r.close()
+        return loops, dev.lazy_stats(), dev.mega_variant()
+    res = run_modes(body)
+    for m in (1, 2):
+        assert res[m][1]["uncached"] == 0, (m, res[m][1])
+    assert res[2][2] == MEGA_RING, res[2][2]
     for temperature, topp in samplers:
-        ids, logits = res[0, temperature]
+        ids, logits = res[0][0][temperature]
         assert len(ids) == steps and np.isfinite(logits).all() and np.abs(logits).max() > 1e-3
         for m in (1, 2):
-            assert res[m, temperature][0] == ids, f"T={temperature}: lazy={m} vs eager ids"
-            assert_bits(res[m, temperature][1], logits, f"T={temperature}: lazy={m} vs eager logits")
+            assert res[m][0][temperature][0] == ids, f"T={temperature}: lazy={m} vs eager ids"
+            assert_same_bits(res[m][0][temperature][1], logits, f"T={temperature}: lazy={m} vs eager logits")
         assert ids == [S.sample_fast(logits[i], temperature, topp, SEED, i) for i in range(steps)], temperature
         if temperature:
             assert len(set(ids)) > 16, ids
@@ -291,15 +282,12 @@ def test_qwen2_7b_fast_mode_logits_inside_the_reference_order_band():
             ro = Llama2Runner(OracleTensor, oconf, lw, odev, 32, use_f16_kv_cache=f16_kv)
             logits[name] = np.stack([ro.forward([t], p).copy() for p, t in enumerate(toks)])
             del ro, lw
-        dev = make_device(lazy=2)
-        try:
+        with fresh_device(lazy=2) as dev:
             w = R.synthetic_weights(dev, conf, wt, wt, seed=seed)
             r = R.LlamaRunner(dev, conf, w, 32, f16_kv=f16_kv)
             logits["gpu"] = np.stack([r.forward([t], p).copy() for p, t in enumerate(toks)])
             assert dev.mega_variant() == MEGA_RING and dev.lazy_stats()["uncached"] == 0
             r.close()
-        finally:
-            dev.close()
         scale = np.abs(logits["avx2"]).max(axis=1)
         ours = np.abs(logits["gpu"] - logits["avx2"]).max(axis=1) / scale
         band = np.abs(logits["scalar"] - logits["avx2"]).max(axis=1) / scale

@@ -7,26 +7,27 @@ import numpy as np
 import pytest
 
 from oracle import oracle as oc
-from tests.gpu_common import make_device
+from crabml_b200.tensor import MEGA_RING
+from tests.gpu_common import assert_same_bits, run_modes
 
 pytestmark = pytest.mark.gpu
 
 TOKENS = 24
 
 
-def _logits(lazy, conf, wt, ct):
+def _logits(conf, wt, ct):
+    """-> body(dev): the logits of TOKENS tokens and the persistent kernel that ran"""
     from crabml_b200 import runner as R
-    dev = make_device(lazy=lazy)
-    try:
+
+    def body(dev):
         w = R.synthetic_weights(dev, conf, wt, ct, seed=0x5A6E)
         r = R.LlamaRunner(dev, conf, w, 64)
         toks = [int(t) for t in np.random.default_rng(5).integers(1, conf.vocab_size, TOKENS)]
         out = np.stack([r.forward([t], p).copy() for p, t in enumerate(toks)])
         variant = dev.mega_variant()
         r.close()
-    finally:
-        dev.close()
-    return out, variant
+        return out, variant
+    return body
 
 
 @pytest.mark.parametrize("shape,wt,ct", [
@@ -39,8 +40,8 @@ def _logits(lazy, conf, wt, ct):
 def test_ring_prologue_matches_eager(shape, wt, ct):
     from crabml_b200 import runner as R
     conf = R.LlamaConfig(*shape, 1e-5, shape[3] // shape[0])
-    ref, _ = _logits(0, conf, wt, ct)
-    got, variant = _logits(2, conf, wt, ct)
-    assert variant == 2, "expected the ring kernel"
+    res = run_modes(_logits(conf, wt, ct), modes=(0, 2))
+    (ref, _), (got, variant) = res[0], res[2]
+    assert variant == MEGA_RING, "expected the ring kernel"
     assert np.isfinite(ref).all() and np.abs(ref).max() > 1e-3
-    np.testing.assert_array_equal(got.view(np.uint32), ref.view(np.uint32))
+    assert_same_bits(got, ref, "lazy=2 vs eager")

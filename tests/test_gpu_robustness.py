@@ -57,21 +57,19 @@ def test_context_too_long_for_the_persistent_kernels_falls_back_to_the_graph_mod
     """A 40 K-token KV cache: the attention phase's score row alone (160 KB) leaves no room for its chunk buffers in shared memory, so
     lazy = 2 must run the token as the CUDA graph of fused kernels instead of failing -- same bits as the eager kernels."""
     import numpy as np
-    from crabml_b200 import CudaTensorDevice, capi
+    from crabml_b200 import capi
     from crabml_b200 import runner as R
+    from crabml_b200.tensor import MEGA_NONE
+    from tests.gpu_common import assert_same_bits, run_modes
     conf = R.LlamaConfig(32, 32, 1, 4096, 11008, 40000, 32000, 1e-5, 128)
-    res = {}
-    for lazy in (0, 2):
-        dev = CudaTensorDevice(0, lazy=lazy)
-        try:
-            w = R.synthetic_weights(dev, conf, capi.Q8_0, capi.Q8_0, seed=5)
-            r = R.LlamaRunner(dev, conf, w, 40000)
-            res[lazy] = np.stack([r.forward([t], p).copy() for p, t in enumerate([1, 9, 31999])])
-            if lazy:
-                assert dev.mega_variant() == 0, "expected the CUDA-graph fallback"
-                st = dev.lazy_stats()
-                assert st["uncached"] == 0, st
-            r.close()
-        finally:
-            dev.close()
-    np.testing.assert_array_equal(res[2].view(np.uint32), res[0].view(np.uint32))
+
+    def body(dev):
+        w = R.synthetic_weights(dev, conf, capi.Q8_0, capi.Q8_0, seed=5)
+        r = R.LlamaRunner(dev, conf, w, 40000)
+        logits = np.stack([r.forward([t], p).copy() for p, t in enumerate([1, 9, 31999])])
+        r.close()
+        return logits, dev.mega_variant(), dev.lazy_stats()
+    res = run_modes(body, modes=(0, 2))
+    assert res[2][1] == MEGA_NONE, "expected the CUDA-graph fallback"
+    assert res[2][2]["uncached"] == 0, res[2][2]
+    assert_same_bits(res[2][0], res[0][0], "lazy=2 vs eager")

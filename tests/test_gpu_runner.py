@@ -10,7 +10,8 @@ from oracle import oracle as oc
 from oracle.llama_replay import GGUFModel, Llama2Runner, LlamaConfig as OConf, LlamaTokenizer, LlamaWeights, decode_text, load_weights
 from oracle.synth import synth_weight
 from oracle.tensor_ref import OracleDevice, OracleTensor
-from tests.gpu_common import make_device
+from crabml_b200.tensor import MEGA_REGISTER, MEGA_RING
+from tests.gpu_common import assert_same_bits, fresh_device, run_modes
 from tests.test_oracle_golden_text import CASES, PROMPT_IDS
 
 pytestmark = pytest.mark.gpu
@@ -21,8 +22,7 @@ pytestmark = pytest.mark.gpu
 def test_cpp_runner_golden_generation(fixture_path, fname, text, ids, exact):
     from crabml_b200 import runner as R
     path = fixture_path(fname)
-    dev = make_device(exact_order=exact)
-    try:
+    with fresh_device(exact_order=exact) as dev:
         conf, w, tok = R.load_gguf(path, dev)
         assert conf.rope_dim == 48 and conf.head_size() == 48
         r = R.LlamaRunner(dev, conf, w, 200)
@@ -32,8 +32,6 @@ def test_cpp_runner_golden_generation(fixture_path, fname, text, ids, exact):
         assert decode_text(t, out) == text
         assert r.kv_cache_len() == len(PROMPT_IDS) + 10
         r.close()
-    finally:
-        dev.close()
 
 
 @pytest.mark.parametrize("f16_kv", [False, True])
@@ -43,17 +41,14 @@ def test_cpp_runner_exact_logits_bit_identical(fixture_path, f16_kv):
     gm = GGUFModel(path)
     odev = OracleDevice()
     ro = Llama2Runner(OracleTensor, gm.conf, load_weights(gm, OracleTensor, odev), odev, 64, use_f16_kv_cache=f16_kv)
-    dev = make_device(exact_order=True)
-    try:
+    with fresh_device(exact_order=True) as dev:
         conf, w, _ = R.load_gguf(path, dev)
         r = R.LlamaRunner(dev, conf, w, 64, f16_kv=f16_kv)
         for pos, t in enumerate(PROMPT_IDS + [29941, 2440]):
             a = r.forward([t], pos).copy()
             b = ro.forward([t], pos)
-            np.testing.assert_array_equal(a.view(np.uint32), b.view(np.uint32), err_msg=f"pos {pos}")
+            assert_same_bits(a, b, f"pos {pos}")
         r.close()
-    finally:
-        dev.close()
 
 
 @pytest.mark.parametrize("wt,ct", [(oc.Q8_0, oc.Q8_0), (oc.Q4_0, oc.Q6_K), (oc.Q4_K, oc.Q6_K)])
@@ -82,21 +77,18 @@ def test_llama2_7b_shaped_layer_on_synthetic_weights(wt, ct):
     ro = Llama2Runner(OracleTensor, oconf, lw, odev, 8)
     want = [ro.forward([t], p).copy() for p, t in enumerate([1, 777, 31999])]
     for exact in (True, False):
-        dev = make_device(exact_order=exact)
-        try:
+        with fresh_device(exact_order=exact) as dev:
             w = R.synthetic_weights(dev, conf, wt, ct, seed=seed)
             r = R.LlamaRunner(dev, conf, w, 8)
             for p, t in enumerate([1, 777, 31999]):
                 got = r.forward([t], p).copy()
                 assert np.isfinite(got).all() and np.abs(got).max() > 1e-3
                 if exact:
-                    np.testing.assert_array_equal(got.view(np.uint32), want[p].view(np.uint32))
+                    assert_same_bits(got, want[p], f"exact_order vs the oracle, pos {p}")
                 else:
                     rel = np.abs(got - want[p]).max() / np.abs(want[p]).max()
                     assert rel < 2e-2, rel          # one layer of order noise through truncating quantisers
             r.close()
-        finally:
-            dev.close()
 
 
 @pytest.mark.parametrize("fname,text,ids", CASES)
@@ -111,8 +103,7 @@ def test_lazy_fused_graph_mode_golden_generation(fixture_path, fname, text, ids,
     gm = GGUFModel(path)
     odev = OracleDevice()
     ro = Llama2Runner(OracleTensor, gm.conf, load_weights(gm, OracleTensor, odev), odev, 64, use_f16_kv_cache=f16_kv)
-    dev = make_device(lazy=mode)          # 1 = fused kernels in a CUDA graph, 2 = one persistent megakernel per token
-    try:
+    with fresh_device(lazy=mode) as dev:          # 1 = fused kernels in a CUDA graph, 2 = one persistent megakernel per token
         conf, w, tok = R.load_gguf(path, dev)
         r = R.LlamaRunner(dev, conf, w, 64, f16_kv=f16_kv)
         worst = 0.0
@@ -131,8 +122,6 @@ def test_lazy_fused_graph_mode_golden_generation(fixture_path, fname, text, ids,
         if not f16_kv or "q8_0" in fname:
             assert out == ids
         r2.close()
-    finally:
-        dev.close()
 
 
 def test_lazy_mode_matches_eager_ops_through_python_mirror(fixture_path):
@@ -141,15 +130,12 @@ def test_lazy_mode_matches_eager_ops_through_python_mirror(fixture_path):
     from crabml_b200 import CudaTensor
     path = fixture_path("tinyllamas-stories-15m-q8_0.gguf")
     gm = GGUFModel(path)
-    dev = make_device(lazy=True, debug_named_tensors=True)
-    try:
+    with fresh_device(lazy=True, debug_named_tensors=True) as dev:
         r = Llama2Runner(CudaTensor, gm.conf, load_weights(gm, CudaTensor, dev), dev, 64)
         pos, _, t0 = r.prefill(PROMPT_IDS)
         out = list(r.generate(pos, t0, 11, eos=gm.eos))
         assert out == CASES[0][2]
         assert dev.dump_debug_tensor("final_rmsnorm:9") is not None
-    finally:
-        dev.close()
 
 
 @pytest.mark.parametrize("wt,ct", [(oc.Q8_0, oc.Q8_0), (oc.Q4_0, oc.Q6_K), (oc.Q4_K, oc.Q6_K), (oc.Q5_K, oc.Q6_K), (oc.Q2_K, oc.Q6_K)])
@@ -160,28 +146,25 @@ def test_lazy_7b_shaped_layer(wt, ct):
     for the all-K-quant ones (Q4_K and Q6_K segmented, Q5_K and Q2_K row by row)."""
     from crabml_b200 import runner as R
     conf = R.LlamaConfig(32, 32, 2, 4096, 11008, 4096, 32000, 1e-5, 128)
-    res = {}
-    for lazy in (0, 1, 2):
-        dev = make_device(lazy=lazy)
-        try:
-            w = R.synthetic_weights(dev, conf, wt, ct, seed=7)
-            r = R.LlamaRunner(dev, conf, w, 16)
-            res[lazy] = np.stack([r.forward([t], p).copy() for p, t in enumerate([1, 777, 31999, 5, 6])])
-            if lazy:
-                st = dev.lazy_stats()
-                assert st["uncached"] == 0 and st["graph_replays"] >= 2, st
-            if lazy == 2:
-                streaming = wt in (oc.Q8_0, oc.Q4_0) or ct in (oc.Q8_0, oc.Q4_0)      # a table with no Q8_0 / Q4_0 matvec runs mega_kernel
-                assert dev.mega_variant() == (2 if streaming else 1), dev.mega_variant()
-            r.close()
-        finally:
-            dev.close()
+    def body(dev):
+        w = R.synthetic_weights(dev, conf, wt, ct, seed=7)
+        r = R.LlamaRunner(dev, conf, w, 16)
+        logits = np.stack([r.forward([t], p).copy() for p, t in enumerate([1, 777, 31999, 5, 6])])
+        r.close()
+        return logits, dev.lazy_stats(), dev.mega_variant()
+    res = run_modes(body)
+    for mode in (1, 2):
+        st = res[mode][1]
+        assert st["uncached"] == 0 and st["graph_replays"] >= 2, (mode, st)
+    streaming = wt in (oc.Q8_0, oc.Q4_0) or ct in (oc.Q8_0, oc.Q4_0)      # a table with no Q8_0 / Q4_0 matvec runs mega_kernel
+    assert res[2][2] == (MEGA_RING if streaming else MEGA_REGISTER), res[2][2]
     # Every mode reduces with the same grouping (canonical orders, csrc/common.cuh): the recorded/fused kernels and the megakernel
     # are BIT-IDENTICAL to the eager per-op kernels, which tests/test_gpu_matvec.py and test_gpu_ops.py pin to the oracle within
     # 1e-6 * sum|terms| -- so those bounds cover the benchmarked megakernel by transitivity.
-    assert np.isfinite(res[0]).all() and np.abs(res[0]).max() > 1e-3
+    ref = res[0][0]
+    assert np.isfinite(ref).all() and np.abs(ref).max() > 1e-3
     for mode in (1, 2):
-        np.testing.assert_array_equal(res[mode].view(np.uint32), res[0].view(np.uint32), err_msg=f"lazy={mode} vs eager")
+        assert_same_bits(res[mode][0], ref, f"lazy={mode} vs eager")
 
 
 @pytest.mark.parametrize("fname", ["tinyllamas-stories-15m-q8_0.gguf", "tinyllamas-stories-15m-q4_0.gguf"])
@@ -193,20 +176,16 @@ def test_execution_modes_bit_identical_on_fixture(fixture_path, fname, f16_kv):
     from crabml_b200 import runner as R
     path = fixture_path(fname)
     seq = (PROMPT_IDS + CASES[0][2])[:21] + [5, 6, 7] + [int(t) for t in np.random.default_rng(3).integers(1, 32000, 226)]
-    res = {}
-    for lazy in (0, 1, 2):
-        dev = make_device(lazy=lazy)
-        try:
-            conf, w, _ = R.load_gguf(path, dev)
-            r = R.LlamaRunner(dev, conf, w, 256, f16_kv=f16_kv)
-            res[lazy] = np.stack([r.forward([t], p).copy() for p, t in enumerate(seq)])
-            if lazy == 2:
-                assert dev.mega_variant() == 2, "expected the ring kernel"
-            r.close()
-        finally:
-            dev.close()
+    def body(dev):
+        conf, w, _ = R.load_gguf(path, dev)
+        r = R.LlamaRunner(dev, conf, w, 256, f16_kv=f16_kv)
+        logits = np.stack([r.forward([t], p).copy() for p, t in enumerate(seq)])
+        r.close()
+        return logits, dev.mega_variant()
+    res = run_modes(body)
+    assert res[2][1] == MEGA_RING, "expected the ring kernel"
     for mode in (1, 2):
-        np.testing.assert_array_equal(res[mode].view(np.uint32), res[0].view(np.uint32), err_msg=f"lazy={mode} vs eager")
+        assert_same_bits(res[mode][0], res[0][0], f"lazy={mode} vs eager")
 
 
 @pytest.mark.parametrize("n_kv,hidden", [(32, 11008), (8, 14336)], ids=["llama2-7b", "mistral-7b"])
@@ -218,26 +197,22 @@ def test_execution_modes_bit_identical_over_200_positions_on_7b_shapes(n_kv, hid
     conf = R.LlamaConfig(32, n_kv, 1, 4096, hidden, 256, 32000, 1e-5, 128)
     toks = [int(t) for t in np.random.default_rng(11).integers(1, 32000, 200)]
     check = [0, 1, 31, 32, 33, 36, 50, 63, 64, 65, 68, 95, 96, 97, 127, 128, 129, 191, 192, 193, 199]
-    res = {}
-    for lazy in (0, 1, 2):
-        dev = make_device(lazy=lazy)
-        try:
-            w = R.synthetic_weights(dev, conf, oc.Q8_0, oc.Q8_0, seed=0x7B)
-            r = R.LlamaRunner(dev, conf, w, 256)
-            res[lazy] = {}
-            for p, t in enumerate(toks):
-                lg = r.forward([t], p, export=p in check)
-                if p in check:
-                    res[lazy][p] = lg.copy()
-            if lazy == 2:
-                assert dev.mega_variant() == 2, "expected the ring kernel"
-            r.close()
-        finally:
-            dev.close()
-    for p in check:
-        assert np.isfinite(res[0][p]).all() and np.abs(res[0][p]).max() > 1e-3
+    def body(dev):
+        w = R.synthetic_weights(dev, conf, oc.Q8_0, oc.Q8_0, seed=0x7B)
+        r = R.LlamaRunner(dev, conf, w, 256)
+        logits = []
+        for p, t in enumerate(toks):
+            lg = r.forward([t], p, export=p in check)
+            if p in check:
+                logits.append(lg.copy())
+        r.close()
+        return logits, dev.mega_variant()
+    res = run_modes(body)
+    assert res[2][1] == MEGA_RING, "expected the ring kernel"
+    for i, p in enumerate(check):
+        assert np.isfinite(res[0][0][i]).all() and np.abs(res[0][0][i]).max() > 1e-3
         for mode in (1, 2):
-            np.testing.assert_array_equal(res[mode][p].view(np.uint32), res[0][p].view(np.uint32), err_msg=f"lazy={mode} vs eager, pos {p}")
+            assert_same_bits(res[mode][0][i], res[0][0][i], f"lazy={mode} vs eager, pos {p}")
 
 
 @pytest.mark.parametrize("mode", [0, 1, 2])
@@ -247,8 +222,7 @@ def test_device_side_greedy_loop_equals_the_host_sampled_loop(fixture_path, mode
     every generated position are bit-identical to the synchronously exported ones."""
     from crabml_b200 import runner as R
     path = fixture_path("tinyllamas-stories-15m-q8_0.gguf")
-    dev = make_device(lazy=mode)
-    try:
+    with fresh_device(lazy=mode) as dev:
         conf, w, tok = R.load_gguf(path, dev)
         steps = 12
         r = R.LlamaRunner(dev, conf, w, 64)
@@ -268,10 +242,8 @@ def test_device_side_greedy_loop_equals_the_host_sampled_loop(fixture_path, mode
             lg = r2.forward([nxt], pos).copy(); pos += 1
         r2.close()
         assert ids == want_ids
-        np.testing.assert_array_equal(logits.view(np.uint32), np.stack(want_logits).view(np.uint32))
+        assert_same_bits(logits, np.stack(want_logits), "device loop vs host loop")
         assert ids[:11] == CASES[0][2]                      # and they are the reference's golden generation
-    finally:
-        dev.close()
 
 
 def test_fast_mode_logits_inside_the_reference_order_band_on_7b_shapes():
@@ -311,15 +283,12 @@ def test_fast_mode_logits_inside_the_reference_order_band_on_7b_shapes():
         ro = Llama2Runner(OracleTensor, OConf(32, 32, nl, 4096, 11008, 4096, 32000, 1e-5, 128), lw, odev, 40)
         logits[name] = np.stack([ro.forward([t], p).copy() for p, t in enumerate(toks)])
         del ro, lw
-    dev = make_device(lazy=2)
-    try:
+    with fresh_device(lazy=2) as dev:
         w = R.synthetic_weights(dev, conf, wt, wt, seed=seed)
         r = R.LlamaRunner(dev, conf, w, 40)
         logits["gpu"] = np.stack([r.forward([t], p).copy() for p, t in enumerate(toks)])
         assert dev.launch_count() > 0 and dev.lazy_stats()["uncached"] == 0
         r.close()
-    finally:
-        dev.close()
     scale = np.abs(logits["avx2"]).max(axis=1)
     ours = np.abs(logits["gpu"] - logits["avx2"]).max(axis=1) / scale
     band = np.abs(logits["scalar"] - logits["avx2"]).max(axis=1) / scale

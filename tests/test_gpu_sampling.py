@@ -13,7 +13,8 @@ import pytest
 from oracle.llama_replay import GGUFModel, Llama2Runner, load_weights
 from oracle.tensor_ref import OracleDevice, OracleTensor
 from tests import sampler_ref as S
-from tests.gpu_common import make_device
+from crabml_b200.tensor import MEGA_REGISTER, MEGA_RING
+from tests.gpu_common import assert_same_bits, fresh_device, run_modes
 
 pytestmark = pytest.mark.gpu
 
@@ -41,23 +42,16 @@ def _row(kind, n, rng):
     return x
 
 
-def _history(dev, count):
-    out = (C.c_int64 * count)()
-    dev.check(dev.lib.cc_read_history(dev.handle, 0, count, out))
-    return [int(v) for v in out]
-
-
 def _sample_many(dev, t, temperature, topp, seed, count):
     for i in range(count):
         t.sample_to_slot(temperature, topp, seed, i, 0, i)
-    return _history(dev, count)
+    return dev.read_history(0, count).tolist()
 
 
 def test_exact_order_picks_equal_the_reference_bit_for_bit():
     from crabml_b200 import CudaTensor
-    dev = make_device(exact_order=True)
     rng = np.random.default_rng(5)
-    try:
+    with fresh_device(exact_order=True) as dev:
         for n in NS:
             for kind in KINDS:
                 x = _row(kind, n, rng)
@@ -70,9 +64,7 @@ def test_exact_order_picks_equal_the_reference_bit_for_bit():
                         want = [S.argmax_last(x) if walk is None else S.pick(walk, S.coin(seed, i)) for i in range(64)]
                         got = _sample_many(dev, t, T, topp, seed, 64)
                         assert got == want, (n, kind, T, topp)
-                assert np.array_equal(t.export().view(np.uint32), x.view(np.uint32)), "the sampler modified the logits"
-    finally:
-        dev.close()
+                assert_same_bits(t.export(), x, "the sampler modified the logits")
 
 
 def test_fast_order_picks_equal_the_emulation_of_its_sums_bit_for_bit():
@@ -80,10 +72,9 @@ def test_fast_order_picks_equal_the_emulation_of_its_sums_bit_for_bit():
     (tests/sampler_ref.py probs_fast / topp_walk_fast; tests/test_sampler_ref.py bounds that emulation's distance from the sequential
     reference entry by entry); how many picks differ from the sequential reference is reported."""
     from crabml_b200 import CudaTensor
-    dev = make_device()
     rng = np.random.default_rng(6)
     diffs, total = 0, 0
-    try:
+    with fresh_device() as dev:
         for n in NS:
             for kind in KINDS:
                 x = _row(kind, n, rng)
@@ -99,8 +90,6 @@ def test_fast_order_picks_equal_the_emulation_of_its_sums_bit_for_bit():
                         ref = [S.argmax_last(x) if wr is None else S.pick(wr, S.coin(seed, i)) for i in range(64)]
                         diffs += sum(g != r for g, r in zip(got, ref))
                         total += 64
-    finally:
-        dev.close()
     print(f"fast order: {diffs} of {total} picks differ from the sequential reference")
 
 
@@ -114,27 +103,22 @@ def test_lazy_megakernel_runs_one_sample_per_token_and_hands_the_rest_to_the_gra
     x = (2.0 * rng.standard_normal(n)).astype(np.float32)
     table = (2.0 * rng.standard_normal((n, n))).astype(np.float32)
 
-    def run(lazy):
-        dev = make_device(lazy=lazy)
-        try:
-            t = CudaTensor.new(x, [n], dev)
-            tab = CudaTensor.new(table.reshape(-1), [n, n], dev)
-            row = CudaTensor.alloc([n], 0, dev)
-            t.sample_to_slot(1.0, 0.9, 5, 0, 0, 0)                # a flush with one sampler, the last op
-            out = _history(dev, 1)
-            variant = dev.mega_variant() if lazy else 0
-            for i in range(1, 7):                                   # six samplers before one flush, into slots 1..6
-                t.sample_to_slot(0.8, 0.9, 5, i, i, i)
-            for i in range(7, 11):                                  # sample -> embedding row from the slot -> sample that row ...
-                dev.check(dev.lib.cc_copy_rows_from_slot(dev.handle, C.byref(row._view()), C.byref(tab._view()), 0))
-                row.sample_to_slot(1.0, 0.5, 5, i, 0, i)
-            out = _history(dev, 11)
-            return out, variant
-        finally:
-            dev.close()
-    eager, _ = run(0)
-    lazy, variant = run(2)
-    assert variant == 1                                             # the single-sampler flush ran in the (register) megakernel
+    def run(dev):
+        t = CudaTensor.new(x, [n], dev)
+        tab = CudaTensor.new(table.reshape(-1), [n, n], dev)
+        row = CudaTensor.alloc([n], 0, dev)
+        t.sample_to_slot(1.0, 0.9, 5, 0, 0, 0)                # a flush with one sampler, the last op
+        dev.read_history(0, 1)
+        variant = dev.mega_variant()
+        for i in range(1, 7):                                   # six samplers before one flush, into slots 1..6
+            t.sample_to_slot(0.8, 0.9, 5, i, i, i)
+        for i in range(7, 11):                                  # sample -> embedding row from the slot -> sample that row ...
+            dev.check(dev.lib.cc_copy_rows_from_slot(dev.handle, C.byref(row._view()), C.byref(tab._view()), 0))
+            row.sample_to_slot(1.0, 0.5, 5, i, 0, i)
+        return dev.read_history(0, 11).tolist(), variant
+    res = run_modes(run, modes=(0, 2))
+    eager, (lazy, variant) = res[0][0], res[2]
+    assert variant == MEGA_REGISTER                                 # the single-sampler flush ran in the (register) megakernel
     assert lazy == eager
     want = [S.sample_fast(x, 1.0, 0.9, 5, 0)] + [S.sample_fast(x, 0.8, 0.9, 5, i) for i in range(1, 7)]
     prev = want[0]
@@ -157,14 +141,14 @@ def test_fast_modes_sample_bit_identical_ids_on_ring_and_k_quant_kernels(tmp_pat
         subprocess.run([sys.executable, os.path.join(ROOT, "tests", "sampling_mode_worker.py"), str(lazy), gguf, out], check=True, cwd=ROOT,
                        env=env, timeout=900)
         got[name] = np.load(out)
-    assert int(got["mega"]["l7b_variant"]) == 2 and int(got["mega"]["tiny_variant"]) in (1, 2)
-    assert int(got["mega"]["l7bk_variant"]) == 1
+    assert int(got["mega"]["l7b_variant"]) == MEGA_RING and int(got["mega"]["tiny_variant"]) in (MEGA_REGISTER, MEGA_RING)
+    assert int(got["mega"]["l7bk_variant"]) == MEGA_REGISTER
     for key in ("tiny", "l7b", "l7bk"):
         ref_ids, ref_lg = got["eager"][f"{key}_ids"], got["eager"][f"{key}_logits"]
         assert ref_ids.size >= 64 and len(set(ref_ids.tolist())) > 8, ref_ids
         for name in ("graph", "mega"):
             np.testing.assert_array_equal(got[name][f"{key}_ids"], ref_ids, err_msg=f"{key}: {name} vs eager")
-            np.testing.assert_array_equal(got[name][f"{key}_logits"].view(np.uint32), ref_lg.view(np.uint32), err_msg=f"{key}: {name} vs eager")
+            assert_same_bits(got[name][f"{key}_logits"], ref_lg, f"{key}: {name} vs eager")
 
 
 @pytest.mark.parametrize("fname", ["tinyllamas-stories-15m-q8_0.gguf", "tinyllamas-stories-15m-q4_0.gguf"])
@@ -175,8 +159,7 @@ def test_exact_order_generation_equals_the_oracle_replay(fixture_path, fname, te
     from crabml_b200 import runner as R
     path = fixture_path(fname)
     prompt, steps, seed = [1, 365, 1424], 24, 31337
-    dev = make_device(exact_order=True)
-    try:
+    with fresh_device(exact_order=True) as dev:
         conf, w, _ = R.load_gguf(path, dev)
         r = R.LlamaRunner(dev, conf, w, 64)
         ids, logits = r.generate_logits(prompt, steps, temperature, topp, seed)
@@ -186,10 +169,8 @@ def test_exact_order_generation_equals_the_oracle_replay(fixture_path, fname, te
         for pos, tok in enumerate(seq[:-1]):
             lg = r.forward([tok], pos).copy()
             if pos >= len(prompt) - 1:
-                np.testing.assert_array_equal(lg.view(np.uint32), logits[pos - len(prompt) + 1].view(np.uint32))
+                assert_same_bits(lg, logits[pos - len(prompt) + 1], f"pos {pos}")
         r.close()
-    finally:
-        dev.close()
     gm = GGUFModel(path)
     odev = OracleDevice()
     ro = Llama2Runner(OracleTensor, gm.conf, load_weights(gm, OracleTensor, odev), odev, 64)
@@ -210,15 +191,15 @@ def test_runner_contract(fixture_path):
     from crabml_b200 import runner as R
     from crabml_b200.capi import TensorError
     path = fixture_path("tinyllamas-stories-15m-q8_0.gguf")
-    dev = make_device(lazy=2)
-    try:
+    with fresh_device(lazy=2) as dev:
         conf, w, _ = R.load_gguf(path, dev)
 
         def fresh():
             return R.LlamaRunner(dev, conf, w, 96)
         r = fresh(); g_ids, g_lg = r.generate_greedy_logits([1, 365], 40); r.close()
         r = fresh(); z_ids, z_lg = r.generate_logits([1, 365], 40, 0.0, 0.9, 5); r.close()
-        assert z_ids == g_ids and np.array_equal(z_lg.view(np.uint32), g_lg.view(np.uint32))
+        assert z_ids == g_ids
+        assert_same_bits(z_lg, g_lg, "temperature 0 vs greedy")
         r = fresh(); a = r.generate([1, 365], 40, 1.0, 0.9, 2024); r.close()
         r = fresh(); b = r.generate([1, 365], 40, 1.0, 0.9, 2024); r.close()
         r = fresh(); c = r.generate([1, 365], 40, 1.0, 0.9, 2025); r.close()
@@ -232,15 +213,12 @@ def test_runner_contract(fixture_path):
                 r.generate([1], 4, T, p, 1)
         assert r.kv_cache_len() == 0      # rejected before the prompt ran
         r.close()
-    finally:
-        dev.close()
 
 
 def test_sample_to_slot_argument_errors():
     from crabml_b200 import CudaTensor
     from crabml_b200.capi import TensorError
-    dev = make_device()
-    try:
+    with fresh_device() as dev:
         x = CudaTensor.new(np.arange(64, dtype=np.float32), [8, 8], dev)
         v = CudaTensor.new(np.arange(64, dtype=np.float32), [64], dev)
         v.sample_to_slot(1.0, 0.9, 1, 0)
@@ -257,9 +235,7 @@ def test_sample_to_slot_argument_errors():
         nanrow = np.full(64, np.nan, np.float32); nanrow[3] = 1.0
         CudaTensor.new(nanrow, [64], dev).sample_to_slot(1.0, 0.9, 1, 0, 0, 0)
         CudaTensor.new(np.full(64, np.nan, np.float32), [64], dev).sample_to_slot(1.0, 0.9, 1, 1, 0, 1)
-        assert all(0 <= i < 64 for i in _history(dev, 2))
-    finally:
-        dev.close()
+        assert all(0 <= i < 64 for i in dev.read_history(0, 2))
 
 
 def test_coin_distribution_fits_the_reference_tail_distribution():
@@ -270,11 +246,8 @@ def test_coin_distribution_fits_the_reference_tail_distribution():
     from crabml_b200 import CudaTensor
     rng = np.random.default_rng(9)
     x = (1.5 * rng.standard_normal(64)).astype(np.float32)
-    dev = make_device()
-    try:
+    with fresh_device() as dev:
         got = np.array(_sample_many(dev, CudaTensor.new(x, [64], dev), 1.0, 0.9, 424242, 20000))
-    finally:
-        dev.close()
     order, Cs, last = S.topp_walk(S.probs(x, 1.0), 0.9)
     q = np.diff(np.concatenate([[0.0], Cs[:last + 1].astype(np.float64)])) / float(Cs[last])
     ids = order[:last + 1]

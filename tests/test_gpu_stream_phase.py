@@ -19,9 +19,10 @@ import pytest
 from oracle import oracle as oc
 from oracle.synth import synth_weight
 from crabml_b200.runner import synth_scale
-from tests.gpu_common import make_device
+from crabml_b200.tensor import MEGA_NONE, MEGA_RING
+from tests.gpu_common import assert_same_bits, full_grid, run_modes
 from tests.test_gpu_matvec import gemv_budget
-from tests.test_gpu_weight_types import EPS, ORACLE_THREADS, WSEED, _Flush, _fingerprint, _mv_code
+from tests.test_gpu_weight_types import EPS, ORACLE_THREADS, WSEED, _mv_code, flushes
 
 pytestmark = pytest.mark.gpu
 
@@ -31,18 +32,7 @@ ROUNDS = 2
 
 @pytest.fixture(autouse=True)
 def _mega_prof(monkeypatch):
-    monkeypatch.setenv("CRABML_MEGA_PROF", "1")       # phase table fingerprints (cc_lazy_mega_profile)
-
-
-_SMS = []
-
-
-def full_grid():
-    """SMs of the device: the persistent grid when no limit is set"""
-    if not _SMS:
-        import torch
-        _SMS.append(torch.cuda.get_device_properties(0).multi_processor_count)
-    return _SMS[0]
+    monkeypatch.setenv("CRABML_MEGA_PROF", "1")       # phase table fingerprints (mega_phase_types)
 
 
 # Widest row (a multiple of 32 columns) whose streaming phase still gets the ring, by prologue: "norm" = a fused rms_norm * w (the
@@ -193,47 +183,21 @@ def _expected(case):
     gs = _groups(ms)
     launches = _uploads(case) + 1 + len(gs)
     if not _fits(t, pro, k, len(gs)):
-        return (0, ()), launches
+        return (MEGA_NONE, ()), launches
     normq = (0,) if pro == "wb" or len(gs) > 1 else ()
-    return (2, (48,) * _uploads(case) + normq + tuple(_mv_code(len(g), EPILOGUE[shape], k) for g in gs)), launches
-
-
-def _run(body, lazy, grid=0, comm=False, rounds=ROUNDS):
-    """The flush `rounds` times on a fresh device: (variant, fingerprint, lazy stats, launches of the last round, its output)."""
-    dev = make_device(lazy=lazy)
-    try:
-        if grid:
-            dev.set_sm_limit(grid)
-        if comm:
-            dev.init_comm(0, 1)
-        f = _Flush(dev)
-        for rnd in range(rounds):
-            l0 = dev.launch_count()
-            out = body(f, rnd)
-            n = dev.launch_count() - l0
-        st = dev.lazy_stats() if lazy else None
-        return dev.mega_variant(), (_fingerprint(dev) if lazy == 2 else ()), st, n, np.asarray(out).copy()
-    finally:
-        dev.close()
-
-
-def _bits(a):
-    return np.asarray(a, np.float32).view(np.uint32)
+    return (MEGA_RING, (48,) * _uploads(case) + normq + tuple(_mv_code(len(g), EPILOGUE[shape], k) for g in gs)), launches
 
 
 def _assert_modes(body, plan, launches, what, grid=0, comm=False, live=True):
     """lazy modes 1 and 2 bit-identical to eager, mode 1 with `launches` launches, mode 2 with plan (variant, fingerprint) -> eager output.
     live: the output is finite and not all zero"""
-    _, _, _, _, ref = _run(body, 0, grid, comm)
+    res = run_modes(flushes(body, grid, comm))
+    ref = res[0][4]
     for mode in (1, 2):
-        v, fp, st, n, got = _run(body, mode, grid, comm)
-        assert st["uncached"] == 0, (what, mode, st)
-        bad = np.flatnonzero(_bits(got) != _bits(ref))[:8]
-        np.testing.assert_array_equal(_bits(got), _bits(ref), err_msg=f"{what}: lazy={mode} vs eager, first at {bad.tolist()}")
-        if mode == 1:
-            assert n == launches, (what, "mode-1 launches", n, launches)
-        else:
-            assert (v, fp) == plan, (what, v, fp, plan)
+        assert res[mode][2]["uncached"] == 0, (what, mode, res[mode][2])
+        assert_same_bits(res[mode][4], ref, f"{what}: lazy={mode} vs eager")
+    assert res[1][3] == launches, (what, "mode-1 launches", res[1][3], launches)
+    assert res[2][:2] == plan, (what, res[2][:2], plan)
     if live:
         assert np.isfinite(ref).all() and np.abs(ref).max() > 1e-3, what
     return ref
@@ -282,7 +246,7 @@ def test_case_list_reaches_every_edge():
         assert {c[3] for c in cs} >= set(K_ALL), oc.TYPE_NAMES[t]
         assert {(c[4], c[5]) for c in cs} >= {(5, i) for i in range(6)} | {(0, i) for i in range(5)}, oc.TYPE_NAMES[t]
         assert any(c[1] == "three" and c[4] == 5 and c[5] in (0, 1, 3, 5) for c in cs)      # m0 % 5 != 0: units straddle matrices
-        ring = [c for c in cs if _expected(_resolve(c))[0][0] == 2]
+        ring = [c for c in cs if _expected(_resolve(c))[0][0] == MEGA_RING]
         assert {c[3] for c in ring} >= set(K_ALL), (oc.TYPE_NAMES[t], "every k through the ring")
 
 
@@ -291,7 +255,7 @@ def test_row_past_the_stream_limit():
     warp-per-row matvec) and the flush runs in the CUDA-graph mode -- and the result still matches the oracle"""
     for t in TYPES:
         case = (t, "one", "plain", 32800, 0, [40])
-        ref = _assert_modes(_body(case), (0, ()), 3, f"{oc.TYPE_NAMES[t]}-k32800")
+        ref = _assert_modes(_body(case), (MEGA_NONE, ()), 3, f"{oc.TYPE_NAMES[t]}-k32800")
         x, _, _ = _inputs(32800, 40, ROUNDS - 1)
         _assert_oracle(t, 32800, [40], x, ref, f"{oc.TYPE_NAMES[t]}-k32800")
 
@@ -308,16 +272,13 @@ def test_rows_do_not_depend_on_the_grid(c):
     t, shape, pro, k, ms = c
     outs = []
     for grid in (1, 2, 5, 7, 0):
-        case = (t, shape, pro, k, grid, ms)
-        for mode in (0, 2):
-            v, _, _, _, out = _run(_body(case), mode, grid)
-            if mode == 2:
-                assert v == 2, (c, grid, v)
-            outs.append((grid, mode, out))
+        res = run_modes(flushes(_body((t, shape, pro, k, grid, ms)), grid), modes=(0, 2))
+        assert res[2][0] == MEGA_RING, (c, grid, res[2][0])
+        outs += [(grid, mode, res[mode][4]) for mode in (0, 2)]
     g0, m0, ref = outs[0]
     assert np.isfinite(ref).all() and np.abs(ref).max() > 1e-3
     for grid, mode, out in outs[1:]:
-        np.testing.assert_array_equal(_bits(out), _bits(ref), err_msg=f"grid {grid} lazy={mode} vs grid {g0} eager")
+        assert_same_bits(out, ref, f"grid {grid} lazy={mode} vs grid {g0} eager")
 
 
 # ---- the exchange epilogue in a world of one --------------------------------------------------------------------------------------------
@@ -379,10 +340,10 @@ def _xchg_expected(c):
     uploads = {"gather": 1, "reduce": 2, "fold": 3}[kind]
     launches = uploads + 3 + (2 if kind == "fold" else 0)
     if ((m + g - 1) // g + 3) & ~3 > 512:
-        return (0, ()), launches
+        return (MEGA_NONE, ()), launches
     xmv = _mv_code(1, 3, k)
     fp = {"gather": (48, xmv, 80), "reduce": (48, 48, xmv, 64), "fold": (48, 48, 48, xmv, _mv_code(1, 0, m))}[kind]
-    return (2, fp), launches
+    return (MEGA_RING, fp), launches
 
 
 XCHG_CASES = _xchg_cases()
@@ -475,8 +436,7 @@ def _fit_case(t, pro, k):
 
 
 def _ring_takes(t, pro, k):
-    v, _, _, _, _ = _run(_body(_fit_case(t, pro, k)), 2, rounds=1)
-    return v == 2
+    return run_modes(flushes(_body(_fit_case(t, pro, k)), rounds=1), modes=(2,))[2][0] == MEGA_RING
 
 
 @pytest.mark.parametrize("pro", ["norm", "plain"])

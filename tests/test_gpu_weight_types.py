@@ -12,7 +12,6 @@ kernels bit for bit; that covers the benchmarked kernels only for the weight typ
  (b) small models laid out like llama.cpp's K-quant files (Q4_K_M, Q5_K_M, Q3_K_M, Q2_K: a few tensors in another type), with the
      Q8_0 / Q5_0 fallback tensors a dimension that is not a multiple of 256 gets, and the 32-block types, decoded through the C++ runner:
      exact_order logits equal the oracle replay, lazy modes 0-2 are bit-identical, and the expected persistent kernel ran."""
-import ctypes as C
 import os
 
 import numpy as np
@@ -23,7 +22,8 @@ from oracle.llama_replay import Llama2Runner, LlamaConfig as OConf, LlamaWeights
 from oracle.synth import synth_weight
 from oracle.tensor_ref import OracleDevice, OracleTensor
 from crabml_b200.runner import synth_scale
-from tests.gpu_common import make_device
+from crabml_b200.tensor import MEGA_NONE, MEGA_REGISTER, MEGA_RING
+from tests.gpu_common import assert_same_bits, fresh_device, run_modes
 from tests.test_gpu_matvec import gemv_budget
 
 pytestmark = pytest.mark.gpu
@@ -32,15 +32,6 @@ GENERIC = [oc.Q2_K, oc.Q3_K, oc.Q4_K, oc.Q5_K, oc.Q6_K, oc.Q8_K]
 WSEED = 0x6E7
 EPS = 1e-5
 ORACLE_THREADS = max(1, min(8, len(os.sched_getaffinity(0))))
-
-
-def _fingerprint(dev):
-    """Phase type codes of the last captured persistent kernel (CRABML_MEGA_PROF=1): 16 * type (0 NORMQ, 1 MATVEC, 2 ATTN, 3 ROWS, ...),
-    plus for a MATVEC phase its matrix count + 4 * epilogue + 1024 * (k >> 10) -- as in test_gpu_fusion_plan.py."""
-    cap = 9 * 4097
-    ts, ty, n = (C.c_uint64 * cap)(), (C.c_int32 * cap)(), C.c_int32(0)
-    dev.check(dev.lib.cc_lazy_mega_profile(dev.handle, ts, ty, cap, C.byref(n)))
-    return tuple(ty[:n.value])
 
 
 def _mv_code(n, epilogue, k):
@@ -172,34 +163,35 @@ def _expected_plan(case):
     fused -- or no persistent kernel at all when the epilogue would have to skip a tail"""
     t, shape, norm, dup, k, ms = case
     if EPILOGUE[shape] and _tail(ms[0]) != ms[0]:
-        return 0, ()
-    return 1, (48,) * _uploads(case) + (_mv_code(NMAT[shape], EPILOGUE[shape], k),)
+        return MEGA_NONE, ()
+    return MEGA_REGISTER, (48,) * _uploads(case) + (_mv_code(NMAT[shape], EPILOGUE[shape], k),)
 
 
-def _replay(body, lazy):
-    """The flush ROUNDS times on a fresh device (the first captures the graph, the last replays it): (variant, fingerprint, lazy stats,
-    output of the last round)."""
-    dev = make_device(lazy=lazy)
-    try:
+def flushes(body, grid=0, comm=False, rounds=ROUNDS):
+    """-> body(dev) for run_modes: the flush `rounds` times (the first captures the graph, the last replays it) at SM limit `grid`, with
+    a world of one if `comm` -> (variant, phase types in mode 2, lazy stats, launches of the last round, its output)"""
+    def run(dev):
+        if grid:
+            dev.set_sm_limit(grid)
+        if comm:
+            dev.init_comm(0, 1)
         f = _Flush(dev)
-        for rnd in range(ROUNDS):
+        for rnd in range(rounds):
+            l0 = dev.launch_count()
             out = body(f, rnd)
-        st = dev.lazy_stats() if lazy else None
-        return dev.mega_variant(), (_fingerprint(dev) if lazy == 2 else ()), st, np.asarray(out).copy()
-    finally:
-        dev.close()
+            n = dev.launch_count() - l0
+        return dev.mega_variant(), dev.mega_phase_types() if dev.lazy == 2 else (), dev.lazy_stats(), n, np.asarray(out).copy()
+    return run
 
 
 def _assert_modes(body, variant, fingerprint, what):
     """lazy modes 1 and 2 bit-identical to eager; mode 2 ran `variant` with phase table `fingerprint`.  -> the eager output"""
-    _, _, _, ref = _replay(body, 0)
+    res = run_modes(flushes(body))
+    ref = res[0][4]
     for mode in (1, 2):
-        v, fp, st, got = _replay(body, mode)
-        assert st["uncached"] == 0, (what, mode, st)
-        bad = np.flatnonzero(got.view(np.uint32) != ref.view(np.uint32))[:8]
-        np.testing.assert_array_equal(got.view(np.uint32), ref.view(np.uint32), err_msg=f"{what}: lazy={mode} vs eager, first at {bad.tolist()}")
-        if mode == 2:
-            assert (v, fp) == (variant, fingerprint), (what, v, fp)
+        assert res[mode][2]["uncached"] == 0, (what, mode, res[mode][2])
+        assert_same_bits(res[mode][4], ref, f"{what}: lazy={mode} vs eager")
+    assert res[2][:2] == (variant, fingerprint), (what, res[2][:2])
     assert np.isfinite(ref).all() and np.abs(ref).max() > 1e-3
     return ref
 
@@ -246,7 +238,7 @@ def test_generic_phases_of_every_type_in_the_ring_kernel(monkeypatch):
         ys += [z, f.W(300, k, oc.Q8_0, 10).matmul_vec(z)]                                  # streaming again, on the generic output
         return np.concatenate([y.export() for y in ys])
     code = _mv_code(1, 0, k)
-    _assert_modes(body, 2, (48, 48, 48, code) + (code,) * len(GENERIC) + (_mv_code(1, 1, k), code), "ring")
+    _assert_modes(body, MEGA_RING, (48, 48, 48, code) + (code,) * len(GENERIC) + (_mv_code(1, 1, k), code), "ring")
 
 
 # ---- (b) mixed-type models end to end ----------------------------------------------------------------------------------------------
@@ -278,17 +270,18 @@ def _uniform(t):
 
 # id: (type of (tensor, layer, n_layers), classifier type, shape overrides, f16 KV cache, expected mode-2 variant)
 LAYOUTS = {
-    "q4_k_m": (_qkm(oc.Q4_K, oc.Q6_K), oc.Q6_K, {}, False, 1),
-    "q5_k_m": (_qkm(oc.Q5_K, oc.Q6_K), oc.Q6_K, {}, True, 1),
-    "q3_k_m": (_q3km, oc.Q6_K, {}, False, 1),
-    "q2_k": (_q2k, oc.Q6_K, {}, True, 1),
-    "q8_k": (_uniform(oc.Q8_K), oc.Q8_K, {}, False, 1),
-    "q4_k-q8_0-fallback": (_fallback(oc.Q8_0), oc.Q6_K, {"hidden": 2720}, False, 2),     # ring kernel with generic phases
-    "q4_k-q5_0-fallback": (_fallback(oc.Q5_0), oc.Q6_K, {"hidden": 2720}, True, 0),      # an eager-only matvec: CUDA graph
-    "q4_1": (_uniform(oc.Q4_1), oc.Q6_K, {}, False, 0),
-    "q5_0": (_uniform(oc.Q5_0), oc.Q6_K, {}, True, 0),
-    "q5_1": (_uniform(oc.Q5_1), oc.Q6_K, {}, False, 0),
-    "mistral-q4_k_m": (_qkm(oc.Q4_K, oc.Q6_K), oc.Q6_K, dict(n_heads=32, n_kv=8, n_layers=1, dim=4096, hidden=14336, vocab=32000), True, 1),
+    "q4_k_m": (_qkm(oc.Q4_K, oc.Q6_K), oc.Q6_K, {}, False, MEGA_REGISTER),
+    "q5_k_m": (_qkm(oc.Q5_K, oc.Q6_K), oc.Q6_K, {}, True, MEGA_REGISTER),
+    "q3_k_m": (_q3km, oc.Q6_K, {}, False, MEGA_REGISTER),
+    "q2_k": (_q2k, oc.Q6_K, {}, True, MEGA_REGISTER),
+    "q8_k": (_uniform(oc.Q8_K), oc.Q8_K, {}, False, MEGA_REGISTER),
+    "q4_k-q8_0-fallback": (_fallback(oc.Q8_0), oc.Q6_K, {"hidden": 2720}, False, MEGA_RING),     # ring kernel with generic phases
+    "q4_k-q5_0-fallback": (_fallback(oc.Q5_0), oc.Q6_K, {"hidden": 2720}, True, MEGA_NONE),      # an eager-only matvec: CUDA graph
+    "q4_1": (_uniform(oc.Q4_1), oc.Q6_K, {}, False, MEGA_NONE),
+    "q5_0": (_uniform(oc.Q5_0), oc.Q6_K, {}, True, MEGA_NONE),
+    "q5_1": (_uniform(oc.Q5_1), oc.Q6_K, {}, False, MEGA_NONE),
+    "mistral-q4_k_m": (_qkm(oc.Q4_K, oc.Q6_K), oc.Q6_K, dict(n_heads=32, n_kv=8, n_layers=1, dim=4096, hidden=14336, vocab=32000), True,
+                       MEGA_REGISTER),
 }
 
 
@@ -328,22 +321,22 @@ def mixed_weights(type_of, ct, s, make, norm_tensor):
     return w
 
 
-def _gpu_logits(layout, tokens, **devkw):
+def _gpu_logits(layout, tokens):
+    """-> body(dev): the logits of every token, lazy stats, variant"""
     from crabml_b200 import CudaTensor
     from crabml_b200 import runner as R
     type_of, ct, over, f16_kv, _ = LAYOUTS[layout]
     s = _shape(over)
-    dev = make_device(**devkw)
-    try:
+
+    def body(dev):
         w = mixed_weights(type_of, ct, s, lambda r, c, t, i: CudaTensor.synth([r, c], t, dev, WSEED, i, synth_scale(t, c)),
                           lambda v: CudaTensor.from_cpu(v, [v.size], oc.F32, dev))
         conf = R.LlamaConfig(s["n_heads"], s["n_kv"], s["n_layers"], s["dim"], s["hidden"], 64, s["vocab"], EPS, s["dim"] // s["n_heads"])
         r = R.LlamaRunner(dev, conf, w, 16, f16_kv=f16_kv)
         out = np.stack([r.forward([t], p).copy() for p, t in enumerate(tokens)])
         r.close()
-        return out, dev.lazy_stats() if devkw.get("lazy") else None, dev.mega_variant()
-    finally:
-        dev.close()
+        return out, dev.lazy_stats(), dev.mega_variant()
+    return body
 
 
 def _oracle_logits(layout, tokens):
@@ -364,19 +357,15 @@ def test_mixed_type_model(layout):
     _, _, over, _, variant = LAYOUTS[layout]
     tokens = [1] + [int(t) for t in np.random.default_rng(len(layout)).integers(2, _shape(over)["vocab"], 9)]
     want = _oracle_logits(layout, tokens)
-    exact, _, _ = _gpu_logits(layout, tokens, exact_order=True)
-    for p in range(len(tokens)):
-        np.testing.assert_array_equal(exact[p].view(np.uint32), want[p].view(np.uint32), err_msg=f"{layout}: exact_order vs the oracle, pos {p}")
-    fast = {}
-    for mode in (0, 1, 2):
-        fast[mode], st, v = _gpu_logits(layout, tokens, lazy=mode)
-        if mode:
-            assert st["uncached"] == 0, (layout, mode, st)
-        if mode == 2:
-            assert v == variant, (layout, v)      # each token is one flush: 0 means no token ran a persistent kernel
+    with fresh_device(exact_order=True) as dev:
+        exact, _, _ = _gpu_logits(layout, tokens)(dev)
+    assert_same_bits(exact, want, f"{layout}: exact_order vs the oracle")
+    fast = run_modes(_gpu_logits(layout, tokens))
     for mode in (1, 2):
-        for p in range(len(tokens)):
-            np.testing.assert_array_equal(fast[mode][p].view(np.uint32), fast[0][p].view(np.uint32), err_msg=f"{layout}: lazy={mode} vs eager, pos {p}")
-    assert np.isfinite(fast[0]).all() and np.abs(fast[0]).max() > 1e-3
-    rel = float(np.abs(fast[0] - want).max() / np.abs(want).max())
+        assert fast[mode][1]["uncached"] == 0, (layout, mode, fast[mode][1])
+        assert_same_bits(fast[mode][0], fast[0][0], f"{layout}: lazy={mode} vs eager")
+    assert fast[2][2] == variant, (layout, fast[2][2])      # each token is one flush: MEGA_NONE means no token ran a persistent kernel
+    ref = fast[0][0]
+    assert np.isfinite(ref).all() and np.abs(ref).max() > 1e-3
+    rel = float(np.abs(ref - want).max() / np.abs(want).max())
     assert rel < 3e-2, (layout, rel)

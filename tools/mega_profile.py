@@ -1,6 +1,5 @@
 """Per-phase time inside the megakernel (CRABML_MEGA_PROF=1): which phases/barriers the token time goes to."""
 import collections
-import ctypes as C
 import os
 import sys
 
@@ -27,12 +26,9 @@ for i in range(40):
     r.forward([100 + i], pos, export=False); pos += 1
 ms = dev.timer_end()
 print(f"40 tokens back to back: {ms / 40 * 1e3:.1f} us per token by CUDA events (kernel time below + inter-launch gap)")
-SL = 10                                     # stamps per phase (common.cuh MK_PROF_SLOTS)
-CAP = SL * 4097
-ts = (C.c_uint64 * CAP)(); ty = (C.c_int32 * CAP)(); n = C.c_int32(0)
-dev.check(dev.lib.cc_lazy_mega_profile(dev.handle, ts, ty, CAP, C.byref(n)))
-n = n.value
-raw = np.array(ts[:(n + 1) * SL], dtype=np.float64).reshape(n + 1, SL)
+stamps, ty = dev.mega_profile()
+n = len(ty)
+raw = stamps.astype(np.float64)
 t = raw[:, 0]
 d = np.diff(t) / 1e3
 base = {0: "normq", 16 + 3: "qkv", 16 + 1 + 4: "mv+res", 16 + 2 + 8: "gate/up", 16 + 1: "mv", 32: "attn", 48: "rows",
@@ -57,7 +53,7 @@ for i in range(n):
     xs = (s4 - s0) / 1e3 if s4 > 0 else 0.0             # prologue: x landed in shared memory (mega.cu: x and weights)
     rm = (s5 - s4) / 1e3 if s5 > 0 and s4 > 0 else 0.0  # prologue: rms known
     qz = (s1 - s5) / 1e3 if s5 > 0 and s1 > 0 else 0.0  # prologue: quantised
-    cw, pk = int(ts[i * SL + 6]), int(ts[i * SL + 7])          # ring kernel: warp 0 wait cycles ; (row-loop cycles << 20) | entries
+    cw, pk = int(stamps[i, 6]), int(stamps[i, 7])          # ring kernel: warp 0 wait cycles ; (row-loop cycles << 20) | entries
     sub[k].append((act, (s2 - max(s0, s1)) / 1e3, (s3 - s2) / 1e3, (raw[i + 1, 0] - s3) / 1e3, xs, rm, qz, cw, pk >> 20, pk & 0xFFF, wa))
 print(f"phases {n}, token total {(t[-1] - t[0]) / 1e3:.1f} us (phase time includes the barrier that ends it)")
 print("  CTA 0 per phase: activation ready | rows of warp 0 done | arrive | barrier wait || prologue, from phase start: weights available | x landed"
@@ -66,7 +62,7 @@ for k, v in sorted(agg.items(), key=lambda kv: -sum(kv[1])):
     m = np.mean(np.array(sub[k]), axis=0)
     ringinfo = f" || ring w0: {m[9]:4.1f} entries, {m[8] / max(m[9], 1):6.0f} cyc/entry, waiting {100 * m[7] / max(m[8], 1):3.0f} %" if m[9] > 0 else ""
     print(f"  {k:16s} n={len(v):3d}  sum {sum(v):8.1f} us  avg {np.mean(v):6.2f}  min {min(v):6.2f}  max {max(v):6.2f}   | {m[0]:5.2f} | {m[1]:5.2f} | {m[2]:5.2f} | {m[3]:5.2f} || {m[10]:5.2f} | {m[4]:5.2f} || {m[5]:5.2f} | {m[6]:5.2f}{ringinfo}")
-tail = [int(ts[n * SL + i]) for i in range(1, 5)]      # producer trips, cycles, entries; ring slots
+tail = [int(stamps[n, i]) for i in range(1, 5)]      # producer trips, cycles, entries; ring slots
 if tail[0]:
     print(f"  ring producer (CTA 0, lane 0): {tail[0]} trips, {tail[2]} entries issued, {tail[1] / tail[0]:.0f} cycles per trip, {tail[1] / 1.965e3:.0f} us inside streaming phases")
     # ring occupancy of CTA 0 (slot 9) as the barrier in front of a phase opened: entries beyond the consumers' position that the producers
@@ -76,7 +72,7 @@ if tail[0]:
     print(f"  ring occupancy as the barrier in front of the phase opened (CTA 0, entries landed / issued ahead of the consumers; {nslots} slots):")
     occ = collections.defaultdict(list)
     for i in range(1, n):
-        o = int(ts[i * SL + 9])
+        o = int(stamps[i, 9])
         occ[name(ty[i])].append((o >> 8 & 0xFF, o & 0xFF))
     for k, v in occ.items():
         a = np.array(v, dtype=np.float64)

@@ -1,7 +1,6 @@
 """Per-phase time inside the megakernel on the SHARDED path: run under torchrun with N ranks (one per GPU); rank 0 prints its profile.
   python -m torch.distributed.run --nproc-per-node 2 --master-addr 127.0.0.1 tools/mega_profile_sharded.py"""
 import collections
-import ctypes as C
 import os
 import sys
 
@@ -38,13 +37,10 @@ dev.timer_begin()
 for i in range(40):
     r.forward([100 + i], pos, export=False); pos += 1
 ms = dev.timer_end()
-SL = 10                                     # stamps per phase (common.cuh MK_PROF_SLOTS)
-CAP = SL * 4097
-ts = (C.c_uint64 * CAP)(); ty = (C.c_int32 * CAP)(); n = C.c_int32(0)
-dev.check(dev.lib.cc_lazy_mega_profile(dev.handle, ts, ty, CAP, C.byref(n)))
-n = n.value
+stamps, ty = dev.mega_profile()
+n = len(ty)
 if rank == 0:
-    raw = np.array(ts[:(n + 1) * SL], dtype=np.float64).reshape(n + 1, SL)
+    raw = stamps.astype(np.float64)
     t = raw[:, 0]
     d = np.diff(t) / 1e3
     base = {0: "normq", 16 + 3: "qkv", 16 + 1 + 4: "mv+res", 16 + 2 + 8: "gate/up", 16 + 1: "mv", 32: "attn", 48: "rows", 16 + 1 + 12: "mv->xchg", 64: "reduce", 80: "gather"}
